@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — SVC inference throughput (audio samples/s) on N B200s of one node.
+"""bench.py — SVC inference throughput (audio samples/s) on N H100s of one node.
 
 Workload (BASELINE.json configs[3], the configuration the 1->8 GPU metric is quoted on): full
 SynthesizerInfer — NSF source + prior encoder + reverse flow + NSF-BigVGAN generator — on a batch
@@ -61,6 +61,8 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-subconfigs", action="store_true", help="skip the configs[1] / configs[2] sub-records")
     ap.add_argument("--no-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step as DIR/<name>.npy (float32, <= 64 MB)")
     return ap.parse_args()
 
 
@@ -70,11 +72,11 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm=float(d["hbm_gbs"]), tf_burst=float(d["bf16_tflops"]),
                     tf_sust=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="fallback")   # H100 SXM data sheet (dense BF16)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -223,7 +225,7 @@ def run_reference(args, hp, sd):
 
 
 # ------------------------------------------------------------------------------ roofline bookkeeping
-FP32_PEAK_TF = 148 * 128 * 2 * 1.965e9 / 1e12   # 148 SMs x 128 FMA lanes x 2 FLOP x max SM clock (nominal; no measured figure)
+FP32_PEAK_TF = 67.0   # H100 SXM data sheet, FP32 (132 SMs x 128 FMA lanes x 2 FLOP x ~1.98 GHz; nominal, no measured figure)
 
 
 def kernel_families(rep: str, steps: int):
@@ -263,7 +265,7 @@ def roofline_of(top, tot_ms, steps, peaks):
     elif not tensor and intensity > FP32_PEAK_TF * 1e12 / (peaks["hbm"] * 1e9):
         roof = {"kernel": top["name"], "bound": "fp32", "achieved": ach_tf, "peak": FP32_PEAK_TF, "unit": "TFLOP/s",
                 "frac": ach_tf / FP32_PEAK_TF, "frac_of_tensor_peak": ach_tf / peaks["tf_sust"],
-                "note": "CUDA-core (FFMA) kernel: peak = 148 SMs x 128 lanes x 2 x 1.965 GHz, nominal"}
+                "note": "CUDA-core (FFMA) kernel: peak = H100 SXM data-sheet FP32 rate, nominal"}
     else:
         ach = top["bytes"] / dur / 1e9
         roof = {"kernel": top["name"], "bound": "hbm", "achieved": ach, "peak": peaks["hbm"], "unit": "GB/s",
@@ -350,6 +352,24 @@ class E2EPipeline:
 
 
 # ------------------------------------------------------------------------------ our arm
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays: dict):
+    """Write each array as out_dir/<name>.npy in float32.  When all of them together exceed 64 MB, each is
+    replaced by the same fixed, seeded sample of its flattened elements (sorted indices, plus <name>_index.npy)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.ascontiguousarray(v, dtype=np.float32) for k, v in arrays.items()}
+    total = sum(v.nbytes for v in arrays.values())
+    for name, a in arrays.items():
+        if total > DUMP_LIMIT_BYTES:
+            keep = max(1, int(a.size * (DUMP_LIMIT_BYTES // 2) / total))
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def run_ours(args, hp, sd):
     from whisper_vits_svc_b200 import _lib, models, shard
 
@@ -415,12 +435,16 @@ def run_ours(args, hp, sd):
         ms = shard.max_over_ranks(float(e0.elapsed_time(e1)), dev)
         return ms, clocks
 
+    last = [None]
+
     def device_loop(n):
         for _ in range(n):
-            step_device()
+            last[0] = step_device()
 
     sampler = ClockSampler(local) if rank == 0 else None
     ms, clocks = timed(device_loop, args.steps, args.warmup, sampler)
+    if args.dump_outputs and rank == 0:   # the waveform [B, 1, L] of the last timed step
+        dump_outputs(args.dump_outputs, {"wave": last[0].float().cpu().numpy()})
     n_launch = launches[0]
     total_samples = float(world * B * L * args.steps)
     value = total_samples / (ms * 1e-3)
@@ -671,7 +695,7 @@ def bench_hubert(args, dev, lib, peaks):
     flops_item = (2 * 512 * 512 * (3 * 60011 + 2 * 3000) + 2 * 512 * 10 * 64015 + 2 * T * 768 * 48 * 128
                   + 2 * T * 512 * 768 + 12 * (2 * T * 768 * (2304 + 768 + 2 * 3072) + 4 * T * T * 768) + 2 * T * 768 * 256)
     out = {"metric": "audio seconds/sec (HuBERT-Soft units)", "value": audio_s / (ms * 1e-3), "unit": "audio s/s",
-           "ms_per_step": ms, "dtype": "bf16 (tcgen05 GEMMs / attention, fp32 accumulate, fp32 residual stream); conv0 + GroupNorm f32",
+           "ms_per_step": ms, "dtype": "bf16 (wgmma GEMMs / attention, fp32 accumulate, fp32 residual stream); conv0 + GroupNorm f32",
            "config": {"workload": f"SURVEY 8f-2: 16 x 20 s of 16 kHz audio [16, 320000] -> units [16, {T}, 256], 12 layers",
                       "tflops_model": flops_item * B / (ms * 1e-3) / 1e12},
            "e2e": {"value": audio_s / (ms_e2e * 1e-3), "unit": "audio s/s", "ms_per_step": ms_e2e,

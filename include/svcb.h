@@ -1,4 +1,4 @@
-/* svcb.h — C ABI of libsvc_b200.so: the sm_100a SVC inference hot path.
+/* svcb.h — C ABI of libsvc_b200.so: the sm_90a SVC inference hot path.
  *
  * The reference (PlayVoice/whisper-vits-svc) has no FFI / plugin layer: its hot path sits
  * behind nn.Module methods (SURVEY.md §8b).  This header is the boundary a maintainer binds
@@ -13,7 +13,7 @@
  *   - return 0 on success, <0 = svcb_status; svcb_last_error() gives a thread-local message;
  *   - a model handle is immutable after creation: concurrent calls on different streams
  *     are fine when their workspaces differ;
- *   - sm_100a only, no fallback: svcb_model_create fails with SVCB_E_UNSUPPORTED elsewhere.
+ *   - sm_90a only, no fallback: svcb_model_create fails with SVCB_E_UNSUPPORTED elsewhere.
  */
 #ifndef SVCB_H_
 #define SVCB_H_
@@ -55,8 +55,8 @@ typedef struct {
   int32_t res_dilations[SVCB_MAX_RES][3];
   int32_t sampling_rate;
   int32_t n_harmonics;   /* 11 = fundamental + 10 overtones (vits_decoder/nsf.py:368) */
-  int32_t precision;     /* AMP-block convs: 0 = fp32 CUDA cores, 3 = bf16x3 split tcgen05 MMA
-                          * (parity grade), 1 = plain bf16 tcgen05 MMA */
+  int32_t precision;     /* AMP-block convs: 0 = fp32 CUDA cores, 3 = bf16x3 split wgmma MMA
+                          * (parity grade), 1 = plain bf16 wgmma MMA */
 } svcb_config;
 
 /* One named tensor inside the packed weight blob (host-side table, read at create time). */
@@ -183,7 +183,7 @@ size_t svcb_hubert_workspace_bytes(const svcb_hubert* h, int32_t B, int32_t n_sa
 /* Replaces HubertSoft.units (hubert/hubert_model.py:68-72): wav [B, n_samples] fp32 (16 kHz, equal-length chunks) ->
  * out [B, svcb_hubert_frames(n_samples), 256] fp32.  taps: null, or 5 device pointers (each may be null) that receive
  * the time-major intermediates [B*T, 512 | 768]: 0 features, 1 projected, 2 embedded, 3 after layer 0, 4 encoded.
- * flags: bit 0 = the six stride-2 convs of the stem in fp32 on the CUDA cores instead of bf16 tcgen05 GEMMs,
+ * flags: bit 0 = the six stride-2 convs of the stem in fp32 on the CUDA cores instead of bf16 wgmma GEMMs,
  * bit 1 = the grouped positional convolution likewise. */
 int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_t B, int32_t n_samples, void* ws,
                       size_t ws_bytes, float* const* taps, int32_t flags, svcb_stream stream);
@@ -209,8 +209,8 @@ int svcb_op_gemm_bf16(const void* A_bf16, const void* W_bf16, const float* bias,
 /* softmax(q k^T / sqrt(64)) v per head: qkv bf16 [B*T, 3*D] rows (q|k|v), out bf16 [B*T, D]. */
 int svcb_op_attention_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, int32_t T, int32_t D, int32_t heads,
                            svcb_stream stream);
-/* The same attention as the encoder runs it (csrc/whisper_attn_tc.cu): q k^T and p v as tcgen05 MMAs with S and
- * O in tensor memory, operands taken from the head-major layout the QKV GEMM writes (built here from the row-major input).
+/* The same attention as the encoder runs it (csrc/whisper_attn_tc.cu): q k^T and p v as wgmma MMAs with S and
+ * O in registers, operands taken from the head-major layout the QKV GEMM writes (built here from the row-major input).
  * v_layout: 0 = the V panel read as an MN-major operand with LBO = 128 B between 8-key groups (what the encoder
  * uses), 1 = LBO / SBO exchanged (kept for the descriptor unit test).  scratch: 256-byte aligned. */
 size_t svcb_op_attention_tc_bf16_scratch_bytes(int32_t B, int32_t T, int32_t D);
@@ -253,7 +253,7 @@ int svcb_op_rel_attention(const float* qkv, const float* emb_rel_k, const float*
                           int32_t window, int32_t T, svcb_stream stream);
 
 /* The same attention on the tensor cores (csrc/rel_attn_tc.cu; what the pipeline runs in precision 1 / 3): q.k^T
- * and p.v as tcgen05 MMAs over bf16 hi/lo split operands, fp32 softmax; head dim 96 and window 4 only.
+ * and p.v as wgmma MMAs over bf16 hi/lo split operands, fp32 softmax; head dim 96 and window 4 only.
  * scratch >= svcb_op_rel_attention_tc_scratch_bytes(B, heads, T), 256-byte aligned. */
 size_t svcb_op_rel_attention_tc_scratch_bytes(int32_t B, int32_t heads, int32_t T);
 int svcb_op_rel_attention_tc(const float* qkv, const float* emb_rel_k, const float* emb_rel_v,
@@ -270,7 +270,7 @@ int svcb_op_conv_tc(const float* x, const void* w_tc, const float* bias, float* 
 
 /* One `SnakeAlias -> Conv1d(C->C, K, dilation, same padding) + bias (+ res)` link of
  * AMPBlock.forward (vits_decoder/bigv.py:50-58) on the tensor cores: snake_pack (bf16 hi/lo operand
- * image in `scratch`) followed by the tcgen05 convolution.  w_tc = pack.py:pack_conv_tc image;
+ * image in `scratch`) followed by the wgmma convolution.  w_tc = pack.py:pack_conv_tc image;
  * nsplit 1 = bf16, 3 = bf16x3 (parity grade). */
 size_t svcb_op_amp_conv_tc_scratch_bytes(int32_t B, int32_t C, int32_t L);
 int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float* ea, const float* inv_b,
@@ -280,7 +280,7 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
 
 /* One `SnakeAlias_in -> Conv1d(C->C, K, dilation) + bias (+ res) [-> SnakeAlias_out]` link of the narrow
  * generator stages (C = 20 or 10; vits_decoder/bigv.py:50-58) in space-to-depth form (csrc/amp_s2d.cu):
- * snake_pack_s2d, then the block-Toeplitz tcgen05 convolution whose epilogue writes y (fp32, may be NULL)
+ * snake_pack_s2d, then the block-Toeplitz wgmma convolution whose epilogue writes y (fp32, may be NULL)
  * and — when y_act != NULL — SnakeAlias_out(result) as the next link's bf16 hi/lo operand image, returned
  * here decoded to fp32 [B,C,L].  w_s2d = pack.py:pack_conv_s2d image; L % (160/C) == 0. */
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L);
@@ -292,8 +292,8 @@ int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_ac
                          const float* fd, const void* w_s2d, const float* bias, int32_t B, int32_t C, int32_t L,
                          int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes, svcb_stream stream);
 
-/* Self-test of the tcgen05/TMEM plumbing: D[128,N] = A[shift:shift+128, :K] . B[N,K]^T with
- * bf16 operands (row-major, device) and fp32 accumulation in tensor memory. */
+/* Self-test of the wgmma plumbing: D[128,N] = A[shift:shift+128, :K] . B[N,K]^T with
+ * bf16 operands (row-major, device) and fp32 accumulation in registers. */
 int svcb_op_tc_gemm_selftest(const void* A_bf16, const void* B_bf16, float* D, int32_t R, int32_t N,
                              int32_t K, int32_t shift, svcb_stream stream);
 

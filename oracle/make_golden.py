@@ -11,6 +11,7 @@ synthetic checkpoint through the loader surgery of whisper/inference.py:11-20 (d
 quarter of the encoder blocks deleted, strict=False load) and `model.encoder(mel)` is stored next to
 the mel; oracle/whisper_oracle.py must reproduce it.
 """
+import contextlib
 import math
 import os
 import sys
@@ -177,6 +178,61 @@ def hubert_case(name):
     print(name, tuple(units.shape), "units rms %.3f" % units.pow(2).mean().sqrt().item(), "oracle-vs-reference max abs", err)
 
 
+# (dims override, B, n_frames) of the Whisper encoder pins; stored in reference_pins.npz as whisper<index>_*
+WHISPER_PIN_CASES = [(dict(n_audio_state=256, n_audio_head=4, n_audio_layer=8), 2, 120),
+                     (dict(n_audio_state=384, n_audio_head=6, n_audio_layer=4), 1, 77)]
+
+
+def to_float64(x):
+    """Floating tensors of a (nested) dict / tensor as float64; everything else unchanged."""
+    if torch.is_tensor(x):
+        return x.double() if x.is_floating_point() else x
+    if isinstance(x, dict):
+        return {k: to_float64(v) for k, v in x.items()}
+    return x
+
+
+@contextlib.contextmanager
+def float64_default():
+    """The reference allocates some buffers with the default dtype (vits_decoder/nsf.py:292): float64 inside."""
+    torch.set_default_dtype(torch.float64)
+    try:
+        yield
+    finally:
+        torch.set_default_dtype(torch.float32)
+
+
+def reference_pins(hp):
+    """tests/golden/reference_pins.npz: what the pins of tests/test_oracle_cpu.py compare the oracle with — the
+    unmodified reference's outputs on the same seeded inputs, its state-dict keys / shapes and alias-filter taps.
+    The SVC and Whisper outputs are computed in float64 (model.double(), float64 inputs): fp32 CPU results move by
+    ~1e-6 with the host's thread count and instruction set, float64 ones by ~1e-15, so a stored float64 result pins
+    the restatement as tightly on any host as a live comparison on one."""
+    out = {}
+    sd = synth.svc_state_dict(hp, 1234)
+    d = to_float64(make_inputs(77, 2, 33, hp, ragged=True))
+    with torch.no_grad(), float64_default():
+        m = ref_model(hp, sd).double()
+        with FeedRNG([d["rand_ini"]], [d["noise"], d["eps"]]):
+            src = m.pitch2source(d["pit"])
+            wave = m.inference(d["ppg"], d["vec"], d["pit"], d["spk"], d["ppg_l"], src)
+    out["svc_source"], out["svc_wave"] = src.numpy(), wave.numpy()
+    Syn = ref_import.import_synthesizer()
+    ref_sd = Syn(513, 25, ref_import.to_attr(hp)).state_dict()
+    out["sd_keys"] = np.array(sorted(ref_sd))
+    out["sd_shapes"] = np.array([",".join(map(str, ref_sd[k].shape)) for k in sorted(ref_sd)])
+    out["up_filter"] = ref_sd["dec.activation_post.upsample.filter"].numpy()
+    for i, (over, B, n) in enumerate(WHISPER_PIN_CASES):
+        ck = synth.whisper_checkpoint(whisper_dims(over), seed=5)
+        model = ref_whisper(ck).double()   # built in fp32 exactly as whisper/inference.py loads it, then widened
+        with torch.no_grad():
+            out[f"whisper{i}_ppg"] = model.encoder(whisper_mel(6, B, n).double()).numpy()
+        out[f"whisper{i}_kept_layers"] = np.array(len(model.encoder.blocks))
+    with torch.no_grad():
+        out["hubert_units"] = ref_hubert(synth.hubert_checkpoint(7)).units(hubert_wav(8, 1, 5003)).numpy()
+    np.savez_compressed(os.path.join(GOLDEN, "reference_pins.npz"), **out)
+
+
 if __name__ == "__main__":
     os.makedirs(GOLDEN, exist_ok=True)
     hp = hparams.load_hparams(os.path.join(ROOT, "configs", "base.yaml"))
@@ -189,3 +245,4 @@ if __name__ == "__main__":
         whisper_case(name)
     for name in HUBERT_CASES:
         hubert_case(name)
+    reference_pins(hp)

@@ -5,7 +5,7 @@ device path running in libsvc_b200.so.
 
 Differences, by design (SURVEY.md §8 scope): the reference shells out to its Whisper / HuBERT /
 CREPE extractors when --ppg/--vec/--pit are missing (svc_inference.py:138-154).  Here --ppg and
---vec are produced in-process by the B200 Whisper encoder / HuBERT-Soft encoder when their
+--vec are produced in-process by the H100 Whisper encoder / HuBERT-Soft encoder when their
 checkpoints are available (whisper_pretrain/large-v2.pt, hubert_pretrain/hubert-soft-0d54a1f4.pt);
 CREPE is out of scope (SURVEY.md §8f-4), so --pit must be given.  Feature retrieval
 (faiss, off by default in the reference) is not built; its flags are accepted and rejected with
@@ -27,23 +27,23 @@ logger = logging.getLogger(__name__)
 
 def main(args):
     if args.enable_retrieval:
-        raise SystemExit("feature retrieval (faiss) is outside the B200 hot path; run without --enable-retrieval")
+        raise SystemExit("feature retrieval (faiss) is outside the H100 hot path; run without --enable-retrieval")
     if args.pit is None:
         raise SystemExit("--pit is required: the CREPE pitch extractor is out of scope of this build "
                          "(use the reference's pitch/inference.py to produce it)")
     if not torch.cuda.is_available():
-        raise SystemExit("this build has no CPU path: a CUDA (sm_100a) device is required")
+        raise SystemExit("this build has no CPU path: a CUDA (sm_90a) device is required")
     if args.vec is None:   # svc_inference.py:144-148 of the reference, in-process
         from whisper_vits_svc_b200 import hubert_infer
         args.vec = "svc_tmp.vec.npy"
-        print(f"Auto run : B200 hubert-soft encoder -w {args.wave} -v {args.vec}")
+        print(f"Auto run : H100 hubert-soft encoder -w {args.wave} -v {args.vec}")
         hm = hubert_infer.load_model(os.path.join("hubert_pretrain", "hubert-soft-0d54a1f4.pt"), "cuda")
         hubert_infer.pred_vec(hm, args.wave, args.vec)
         del hm
     if args.ppg is None:
         from whisper_vits_svc_b200 import whisper_infer
         args.ppg = "svc_tmp.ppg.npy"
-        print(f"Auto run : B200 whisper encoder -w {args.wave} -p {args.ppg}")
+        print(f"Auto run : H100 whisper encoder -w {args.wave} -p {args.ppg}")
         wm = whisper_infer.load_model(os.path.join("whisper_pretrain", "large-v2.pt"), "cuda")
         whisper_infer.pred_ppg(wm, args.wave, args.ppg, "cuda")
     logging.basicConfig(level=logging.DEBUG if args.debug else logging.INFO)

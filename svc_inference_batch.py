@@ -7,8 +7,8 @@ checkpoint and re-spawning the HuBERT / pitch extractors every time.  Here the m
 once per GPU, files are sharded across the ranks of a `torchrun` launch (one process per GPU, one
 NCCL broadcast of the packed weights, no collective on the data path), and per rank the chunks of ALL its
 files are bucketed by length and run as full device batches (hostio.BatchEngine) while host threads read
-features and write WAVs.  Missing `<name>.ppg.npy` / `<name>.vec.npy` are extracted in-process by the B200 Whisper /
-HuBERT-Soft encoders (one model load per rank).  CREPE is outside the B200 hot path (SURVEY.md §8f-4):
+features and write WAVs.  Missing `<name>.ppg.npy` / `<name>.vec.npy` are extracted in-process by the H100 Whisper /
+HuBERT-Soft encoders (one model load per rank).  CREPE is outside the H100 hot path (SURVEY.md §8f-4):
 `<name>.pit.csv` must sit next to `<name>.wav` (or in --feat); a file without it is reported and skipped — the
 reference would silently produce nothing for it either (subprocess exit codes are ignored there).
 
@@ -46,7 +46,7 @@ def main():
     os.makedirs(out_path, exist_ok=True)
     waves = sorted(f for f in os.listdir(wave_path) if f.endswith(".wav"))
     if not torch.cuda.is_available():
-        raise SystemExit("this build has no CPU path: a CUDA (sm_100a) device is required")
+        raise SystemExit("this build has no CPU path: a CUDA (sm_90a) device is required")
     rank, local, world = shard.init()
     device = torch.device("cuda", local)
     torch.cuda.set_device(device)

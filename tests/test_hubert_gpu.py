@@ -64,7 +64,7 @@ def test_units_stages_vs_oracle(models):
     print(f"features (fp32 stem) max-abs {e:.3e} (rms {feats_o.pow(2).mean().sqrt():.3f})")
     assert e <= 2e-4
     r = rel_l2(taps["features"].cpu(), feats_o)
-    print(f"features (tcgen05 stem, bf16) rel-l2 {r:.3e}; units fp32-stem vs tcgen05-stem rel-l2 {rel_l2(got, got32):.3e}")
+    print(f"features (tensor-core stem, bf16) rel-l2 {r:.3e}; units fp32-stem vs tensor-core-stem rel-l2 {rel_l2(got, got32):.3e}")
     assert r <= 1e-2 and rel_l2(got32, ref) <= 2e-2
     for nm in ("projected", "embedded", "layer0", "encoded"):
         r = rel_l2(taps[nm].cpu(), taps_o[nm])

@@ -97,7 +97,7 @@ def test_layernorm_c(ops, C, T, per_batch):
                                        (150, [150, 97], True), (64, [64, 64], True), (65, [65, 1], True), (300, [300, 201], True),
                                        (5, [5, 3], True), (129, [129, 64], True), (1000, [1000, 777, 1], True), (2520, [2520], True)])
 def test_rel_attention(ops, T, lens, tc):
-    """fp32 CUDA-core kernel (precision 0) and the tcgen05 kernel (bf16x3 split operands, precision 1 / 3)
+    """fp32 CUDA-core kernel (precision 0) and the wgmma kernel (bf16x3 split operands, precision 1 / 3)
     against the oracle's dense pad/reshape formulation.  Lengths: ragged masks, a fully valid item, tiles
     with a ragged last query / key tile, fewer keys than the relative window, the longest chunk (2520)."""
     g = torch.Generator().manual_seed(T)
@@ -127,7 +127,7 @@ def test_rel_attention(ops, T, lens, tc):
 @pytest.mark.parametrize("N,K,shift,R", [(160, 160, 0, 128), (160, 160, 7, 178), (80, 80, 25, 160), (48, 48, 3, 140),
                                          (32, 32, 1, 130), (16, 16, 0, 128), (256, 64, 9, 137)])
 def test_tcgen05_gemm_selftest(N, K, shift, R):
-    """tcgen05.mma + TMEM + row-shifted K-major SWIZZLE_NONE descriptors (the conv-tap trick):
+    """wgmma + row-shifted K-major no-swizzle descriptors (the conv-tap trick):
     bf16 inputs, fp32 accumulate -> exact up to fp32 summation order."""
     import ctypes
     from whisper_vits_svc_b200 import _lib
@@ -148,7 +148,7 @@ def test_tcgen05_gemm_selftest(N, K, shift, R):
     (160, 700, 11, 5, 3, 2e-4), (160, 300, 3, 1, 3, 2e-4), (80, 1000, 7, 3, 3, 2e-4), (40, 513, 11, 1, 3, 2e-4),
     (20, 1024, 7, 5, 3, 2e-4), (10, 2000, 3, 3, 3, 2e-4), (80, 640, 7, 1, 1, 5e-2), (10, 127, 11, 5, 3, 2e-4)])
 def test_amp_conv_tc(ops, sd, C, L, K, dil, nsplit, tol):
-    """Fused SnakeAlias -> Conv1d (+bias +residual) on tcgen05 vs the oracle's two torch ops.
+    """Fused SnakeAlias -> Conv1d (+bias +residual) on wgmma vs the oracle's two torch ops.
     bf16x3 split operands: expected error ~1e-5 on O(1) data; plain bf16 ~1e-2 (reported, loose)."""
     g = torch.Generator().manual_seed(C * 7 + L + K + dil)
     B = 2
@@ -172,7 +172,7 @@ def test_amp_conv_tc(ops, sd, C, L, K, dil, nsplit, tol):
     (96, 192, 130, 1, 1, 3, 2e-4), (192, 640, 500, 3, 1, 3, 2e-4), (192, 320, 64, 7, 1, 3, 2e-4),
     (1280, 192, 200, 5, 1, 3, 3e-4), (192, 96, 77, 1, 1, 1, 5e-2)])
 def test_conv_tc(ops, Cin, Cout, T, K, dil, nsplit, tol):
-    """General implicit-GEMM Conv1d on tcgen05 vs F.conv1d (fp32 CPU)."""
+    """General implicit-GEMM Conv1d on wgmma vs F.conv1d (fp32 CPU)."""
     g = torch.Generator().manual_seed(Cin + Cout + T + K)
     x = torch.randn(2, Cin, T, generator=g)
     w = torch.randn(Cout, Cin, K, generator=g) / (Cin * K) ** 0.5
@@ -212,7 +212,7 @@ def test_conv_tc_epilogues(ops):
                                        (40, 8, 7, 3), (40, 4 * 126, 11, 1), (40, 4 * 1002, 7, 5)])
 def test_amp_s2d_link(ops, sd, C, L, K, dil):
     """One AMP-block link of the narrow stages in space-to-depth form (csrc/amp_s2d.cu): block-Toeplitz
-    tcgen05 conv (bf16x3) with bias + residual, and the NEXT SnakeAlias computed in the epilogue — both
+    wgmma conv (bf16x3) with bias + residual, and the NEXT SnakeAlias computed in the epilogue — both
     against the oracle's torch ops.  Lengths cover: whole tiles (126 useful rows), ragged last tiles, a
     single row, items shorter than the Snake / conv reach (sequence-end clamps on both sides at once)."""
     g = torch.Generator().manual_seed(C * 11 + L + K + dil)

@@ -154,7 +154,7 @@ def test_empty_and_bad_inputs(model, hp):
 
 @pytest.mark.parametrize("precision,tol", [(3, WAVE_TOL), (1, 5e-2)])
 def test_tensor_core_generator_modes(hp, sd, precision, tol):
-    """AMP-block convs on tcgen05: bf16x3 split meets the 1e-3 waveform gate; plain bf16 reports
+    """AMP-block convs on the tensor cores (wgmma): bf16x3 split meets the 1e-3 waveform gate; plain bf16 reports
     its own error (CPU emulation predicts ~1e-2)."""
     from whisper_vits_svc_b200 import models
     m = models.SynthesizerInfer(513, 25, hp, precision=precision)

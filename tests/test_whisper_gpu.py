@@ -79,7 +79,7 @@ def test_attention_bf16(B, T, heads):
 @pytest.mark.parametrize("B,T,heads,v_layout", [(2, 100, 2, 0), (1, 64, 4, 0), (2, 1500, 2, 0), (1, 333, 20, 0), (3, 129, 4, 0),
                                                 (2, 100, 2, 1)])
 def test_attention_tc_bf16(B, T, heads, v_layout):
-    """The encoder's attention kernel (tcgen05: S and O in tensor memory, V read as an MN-major operand) on its
+    """The encoder's attention kernel (wgmma: S and O in registers, P fed from registers, V read as an MN-major operand) on its
     own, fed through the same tile image the QKV GEMM writes.  v_layout 1 exchanges LBO / SBO of the V
     descriptor: it must NOT match (pins the descriptor semantics the kernel relies on)."""
     from whisper_vits_svc_b200 import _lib

@@ -1,4 +1,4 @@
-"""B200-native SVC inference hot path behind the reference's Python surface.
+"""H100-native SVC inference hot path behind the reference's Python surface.
 
 Sub-modules are imported lazily by name so that host-only helpers (hparams, synth, hostio)
 work without the CUDA library; anything that computes goes through `_lib` and fails loudly

@@ -6,7 +6,7 @@
 // stage-mean bookkeeping of generator.py:188-194, in ONE kernel: x is read once, the result is
 // written once (SURVEY.md §8a row a9 "per-block fused kernel", row a10).
 //
-// Why CUDA cores here: with C = 10 / 20 a tcgen05 MMA has N = 16 / 32 and costs as much issue time
+// Why CUDA cores here: with C = 10 / 20 a tensor-core MMA has N = 16 / 32 and costs as much issue time
 // as a full-width one (measured: these two stages took 75 of 107 ms of the tensor-core AMP path
 // while holding 20 % of its FLOPs — profiles/r01_notes.md); their arithmetic intensity unfused is
 // ~45-330 FLOP/B (fp32-FMA side of the ridge).  Fused, the stage is bound by fp32 FMA issue and

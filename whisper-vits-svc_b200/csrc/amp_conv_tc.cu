@@ -1,15 +1,13 @@
-// AMP-block link on the 5th-gen tensor cores, as two kernels that each stream at their own roofline:
+// AMP-block link on the tensor cores, as two kernels that each stream at their own roofline:
 //
 //   snake_pack   SnakeAlias(x) -> bf16 hi/lo operand image in HBM            (CUDA cores, 8 B/element)
-//   amp_conv_tc  Conv1d(C->C, K, dilation) + bias (+residual, stage mean)    (tcgen05 + TMEM)
+//   amp_conv_tc  Conv1d(C->C, K, dilation) + bias (+residual, stage mean)    (wgmma)
 //
 // Together they replace one `SnakeAlias -> Conv1d [-> + x]` link of AMPBlock.forward
 // (vits_decoder/bigv.py:50-58; SnakeAlias = vits_decoder/alias/act.py:124-128), SURVEY.md §8a rows
-// a9/a10.  A first version fused both into one CTA-per-tile kernel; measured on B200 it ran at the
-// CUDA-core path's speed (15 TFLOP/s) because the per-tile Snake prologue (20 x load->sync->FIR->
-// sync->FIR->sync with one resident CTA) was latency-bound and left the tensor pipe idle
-// (profiles/r01_notes.md).  Splitting lets the Snake pass run with 32 warps/SM and lets the conv
-// kernel feed its A operand with bulk (TMA-engine) copies.
+// a9/a10.  Fusing both into one CTA-per-tile kernel leaves the tensor pipe idle behind a latency-bound
+// per-tile Snake prologue (20 x load->sync->FIR->sync->FIR->sync with one resident CTA); split, the Snake
+// pass runs with 32 warps/SM and the conv kernel feeds its A operand with bulk (TMA-engine) copies.
 //
 // Operand image ("P8" layout): hi/lo bf16 [B][Cp/8][Lp][8], Lp = 32 + roundup(L,128) + 32, row =
 // 32 + t; rows outside the sequence and channels >= C are zero.  One (octet, row-range) of the A
@@ -25,8 +23,6 @@
 #include "tc.cuh"
 
 namespace svcb {
-
-static inline unsigned tc_cols_host(int n) { return n <= 32 ? 32u : n <= 64 ? 64u : n <= 128 ? 128u : n <= 256 ? 256u : 512u; }
 
 constexpr int TC_M = 128;
 constexpr int P8_PAD = 32;
@@ -162,85 +158,53 @@ int launch_snake_pack(const float* x, void* hi, void* lo, const float* ea, const
 }
 
 // ------------------------------------------------------------------------------------ amp_conv_tc
-// Persistent: each CTA walks tiles (item, 128 samples) with a static stride.  Three roles pipeline
-// across tiles through mbarriers:
+// Persistent: each CTA walks tiles (item, 128 samples) with a static stride.
 //   producer thread  A image rows of tile i+1 (bulk copies, 1-2 buffers) and the weight tiles
 //                    (all taps resident in shared memory when they fit, else a 2-slot ring per tile)
-//   MMA warp         all taps x split parts of tile i into TMEM accumulator (i & 1); one elected lane
-//                    issues (tc::elect_one) inside warp-uniform control flow
-//   8 epilogue warps tile i-1: tcgen05.ld -> +bias (+res, +stage accumulation, /3) -> coalesced stores
-struct AmpPlan { int resident, nabuf, acc_stride, ncols, ncat, nw; size_t smem; };
-constexpr int AMP_WMAX = 8;   // deepest weight ring
+//   2 warpgroups     64 rows each: all taps x split parts of tile i as wgmma m64nCpk16 into register
+//                    accumulators, then +bias (+res, +stage accumulation, /3) through a shared-memory strip
+//                    (64 columns at a time) -> coalesced stores
+struct AmpPlan { int resident, nabuf, nw; size_t smem; };
+constexpr int AMP_WMAX = 2;     // weight ring depth when the taps do not stay resident
+constexpr int AMP_EPI_LD = 72;  // floats per row of an epilogue strip
+constexpr int AMP_THREADS = 288;
+constexpr size_t AMP_STRIP_BYTES = 2 * 64 * AMP_EPI_LD * 4;
 
-// NK MMAs of one (tap, split part, A part) group: the operands' descriptor low words advance by
-// kk * kstep with kk a compile-time constant.
-template <int NK>
-__device__ __forceinline__ void amp_issue(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                          uint32_t idesc, uint32_t kstep_a, uint32_t kstep_b, uint32_t first_acc) {
-  tc::mma_bf16_lohi(d_tmem, a_lo, a_hi, b_lo, b_hi, idesc, first_acc);
-#pragma unroll
-  for (int kk = 1; kk < NK; ++kk) tc::mma_bf16_lohi(d_tmem, a_lo + kk * kstep_a, a_hi, b_lo + kk * kstep_b, b_hi, idesc, 1u);
-}
-
-__global__ void __launch_bounds__(320, 1)
-amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, const int nw, const int acc_stride,
-                   const uint32_t ncols, const int ncat) {
+template <int NC>
+__global__ void __launch_bounds__(AMP_THREADS, 1)
+amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, const int nw) {
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t a_full[2], a_empty[2], w_full[AMP_WMAX], w_empty[AMP_WMAX], w_res, t_full[2], t_empty[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t a_full[2], a_empty[2], w_full[AMP_WMAX], w_empty[AMP_WMAX], w_res;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int warp_u = tc::warp_uniform_idx();
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int P = p.dil * (p.K - 1) / 2;
   const int R = TC_M + (p.K - 1) * p.dil;
-  const int KC = p.Cp / 8;
+  const int KC = NC / 8;
   const int parts = p.nsplit == 3 ? 2 : 1;
   const uint32_t a_part = (uint32_t)KC * R * 16u;
   const uint32_t a_buf = a_part * parts;
-  const uint32_t wb = (uint32_t)p.Cp * p.Cp * 2u;
+  const uint32_t wb = (uint32_t)NC * NC * 2u;
   const int nch = p.K * parts;
   uint8_t* Abase = smem;
   uint8_t* Wbase = smem + (size_t)nabuf * a_buf;
+  float* Strips = reinterpret_cast<float*>(Wbase + (size_t)(resident ? nch : nw) * wb);
   const int tpi = (p.L + TC_M - 1) / TC_M;
   const int ntiles = p.B * tpi;
 
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&a_full[i], 1); tc::mbar_init(&a_empty[i], 1);
-      tc::mbar_init(&t_full[i], 1); tc::mbar_init(&t_empty[i], 256);
-    }
-    for (int i = 0; i < AMP_WMAX; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 1); }
+    for (int i = 0; i < 2; ++i) { tc::mbar_init(&a_full[i], 1); tc::mbar_init(&a_empty[i], 2); }
+    for (int i = 0; i < AMP_WMAX; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 2); }
     tc::mbar_init(&w_res, 1);
     tc::fence_barrier_init();
   }
-  __syncwarp();
-  if (warp == 8) tc::tmem_alloc(&tmem_slot, ncols);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = tmem_slot;
 
   if (tid == 256) {
     // ---------------------------------------------------------------- producer
-    // ncat: the hi and lo weight tiles of a tap are interleaved per K-chunk ([kc][hi rows | lo rows][8])
-    // so that ONE descriptor with N = 2*Cp multiplies A_hi by [W_hi | W_lo]; the hi-only view of the
-    // same bytes (N = Cp, same stride) serves A_lo * W_hi.  The packed blob keeps its layout: the
-    // interleave happens here, one bulk copy per (tap, part, K-chunk).
-    const uint32_t wrow = (uint32_t)p.Cp * 16u;   // one K-chunk of one part
-    auto load_tap_cat = [&](uint8_t* dst, int tap, uint64_t* bar) {
-      for (int part = 0; part < 2; ++part)
-        for (int kc = 0; kc < KC; ++kc)
-          tc::bulk_g2s(dst + (size_t)kc * 2 * wrow + (size_t)part * wrow,
-                       p.wpk + ((size_t)tap * 2 + part) * wb + (size_t)kc * wrow, wrow, bar);
-    };
     if (resident) {
       tc::mbar_arrive_expect_tx(&w_res, wb * (uint32_t)nch);
-      if (ncat) {
-        for (int tap = 0; tap < p.K; ++tap) load_tap_cat(Wbase + (size_t)tap * 2 * wb, tap, &w_res);
-      } else {
-        for (int i = 0; i < nch; ++i)
-          tc::bulk_g2s(Wbase + (size_t)i * wb, p.wpk + ((size_t)(i / parts) * 2 + (i % parts)) * wb, wb, &w_res);
-      }
+      for (int i = 0; i < nch; ++i)
+        tc::bulk_g2s(Wbase + (size_t)i * wb, p.wpk + ((size_t)(i / parts) * 2 + (i % parts)) * wb, wb, &w_res);
     }
     const uint32_t run = (uint32_t)R * 16u;
     int it = 0, wi = 0;
@@ -256,14 +220,7 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
         for (int kc = 0; kc < KC; ++kc)
           tc::bulk_g2s(dst + (size_t)kc * run, src + (((long long)b * KC + kc) * p.Lp + row) * 16, run, &a_full[buf]);
       }
-      if (!resident && ncat) {
-        for (int tap = 0; tap < p.K; ++tap, ++wi) {
-          const int st = wi % nw;
-          if (wi >= nw) tc::mbar_wait(&w_empty[st], (uint32_t)(((wi / nw) - 1) & 1));
-          tc::mbar_arrive_expect_tx(&w_full[st], 2 * wb);
-          load_tap_cat(Wbase + (size_t)st * 2 * wb, tap, &w_full[st]);
-        }
-      } else if (!resident) {
+      if (!resident) {
         for (int i = 0; i < nch; ++i, ++wi) {
           const int st = wi % nw;
           if (wi >= nw) tc::mbar_wait(&w_empty[st], (uint32_t)(((wi / nw) - 1) & 1));
@@ -272,71 +229,28 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
         }
       }
     }
-  } else if (warp_u == 9) {
-    // ---------------------------------------------------------------- MMA issuer (whole warp, uniform
-    // control flow; one elected lane issues — see tc::elect_one)
-    const uint32_t idesc = tc::idesc_bf16(TC_M, p.Cp);
+  } else if (warp < 8) {
+    // ---------------------------------------------------------------- MMA + epilogue (warpgroup wg: rows 64 wg ..)
+    const int wg = warp >> 2, t = tid & 127;
+    float* strip = Strips + wg * 64 * AMP_EPI_LD;
     const uint32_t a0 = tc::smem_u32(Abase), w0 = tc::smem_u32(Wbase);
-    const uint32_t lbo_a = (uint32_t)R * 16u, lbo_b = (uint32_t)p.Cp * 16u;
+    const uint32_t lbo_a = (uint32_t)R * 16u, lbo_b = (uint32_t)NC * 16u;
+    const uint64_t ks_a = (2u * lbo_a) >> 4, ks_b = (2u * lbo_b) >> 4;
+    constexpr int NK = NC / 16;
+    const bool do_div = p.out_div != 0.f;
     if (resident) tc::mbar_wait(&w_res, 0);
     int it = 0, wi = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int buf = it % nabuf, acc = it & 1;
+      const int buf = it % nabuf;
+      const int b = tile / tpi, t0 = (tile - b * tpi) * TC_M;
       tc::mbar_wait(&a_full[buf], (uint32_t)((it / nabuf) & 1));
-      if (it >= 2) tc::mbar_wait(&t_empty[acc], (uint32_t)(((it >> 1) - 1) & 1));
-      tc::fence_after_sync();
-      const uint32_t d_tmem = tmem + (uint32_t)(acc * acc_stride);
-      const uint32_t a_hi = a0 + (uint32_t)buf * a_buf, a_lo = a_hi + a_part;
-      // descriptors differ only in the start-address field (units of 16 B): advance by addition
-      const uint64_t ad_hi0 = tc::smem_desc(a_hi, lbo_a), ad_lo0 = tc::smem_desc(a_lo, lbo_a);
-      const uint32_t kstep_a = (2u * lbo_a) >> 4, kstep_b = (2u * lbo_b) >> 4;
-      const int nk = p.Cp / 16;
-      uint32_t accumulate = 0;
+      const uint32_t a_hi = a0 + (uint32_t)buf * a_buf + (uint32_t)wg * 64u * 16u, a_lo = a_hi + a_part;
+      float acc[NC / 2];
+#pragma unroll
+      for (int i = 0; i < NC / 2; ++i) acc[i] = 0.f;
       int i = 0;
-      if (ncat) {
-        // two MMA groups per tap instead of three: A_hi x [W_hi | W_lo] (N = 2*Cp, columns [0,Cp) and
-        // [Cp,2Cp) of the accumulator) and A_lo x W_hi (N = Cp, into columns [0,Cp)); the epilogue adds
-        // the two column halves.  An MMA costs ~110 cycles here whatever its N (r01 captures), so the
-        // instruction count is what matters.
-        const uint32_t idesc_cat = tc::idesc_bf16(TC_M, 2 * p.Cp);
-        const uint32_t lbo_c = 2u * lbo_b, kstep_c = (2u * lbo_c) >> 4;
-        for (int tap = 0; tap < p.K; ++tap) {
-          const uint32_t tap_off = (uint32_t)(tap * p.dil);
-          uint32_t wbase;
-          int st = 0;
-          if (resident) {
-            wbase = w0 + (uint32_t)tap * 2u * wb;
-          } else {
-            st = wi % nw;
-            tc::mbar_wait(&w_full[st], (uint32_t)((wi / nw) & 1));
-            tc::fence_after_sync();
-            wbase = w0 + (uint32_t)st * 2u * wb;
-          }
-          const uint64_t bd0 = tc::smem_desc(wbase, lbo_c);
-          if (tc::elect_one()) {
-            uint32_t acc_flag = accumulate;
-            const uint32_t a_hiw = (uint32_t)(ad_hi0 >> 32), b_hiw = (uint32_t)(bd0 >> 32);
-            uint32_t ad = (uint32_t)ad_hi0 + tap_off, bd = (uint32_t)bd0;
-            for (int kk = 0; kk < nk; ++kk) {
-              tc::mma_bf16_lohi(d_tmem, ad, a_hiw, bd, b_hiw, idesc_cat, acc_flag);
-              acc_flag = 1;
-              ad += kstep_a;
-              bd += kstep_c;
-            }
-            ad = (uint32_t)ad_lo0 + tap_off; bd = (uint32_t)bd0;
-            for (int kk = 0; kk < nk; ++kk) {
-              tc::mma_bf16_lohi(d_tmem, ad, a_hiw, bd, b_hiw, idesc, 1u);
-              ad += kstep_a;
-              bd += kstep_c;
-            }
-            if (!resident) tc::mma_commit(&w_empty[st]);
-          }
-          accumulate = 1;
-          if (!resident) ++wi;
-        }
-      }
-      for (int tap = 0; tap < (ncat ? 0 : p.K); ++tap) {
-        const uint32_t tap_off = (uint32_t)(tap * p.dil);  // rows -> 16-byte units
+      for (int tap = 0; tap < p.K; ++tap) {
+        const uint32_t tap_off = (uint32_t)(tap * p.dil) * 16u;
         for (int part = 0; part < parts; ++part, ++i) {
           uint32_t wbase;
           int st = 0;
@@ -345,114 +259,59 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
           } else {
             st = wi % nw;
             tc::mbar_wait(&w_full[st], (uint32_t)((wi / nw) & 1));
-            tc::fence_after_sync();
             wbase = w0 + (uint32_t)st * wb;
           }
-          const uint64_t bd0 = tc::smem_desc(wbase, lbo_b);
           const int n_a = (part == 0 && parts == 2) ? 2 : 1;  // Wh meets Ah and Al; Wl meets Ah
-          // descriptor low words of this group, computed in uniform code; the unrolled issue below adds
-          // compile-time multiples of the K steps only (the per-MMA `ad += kstep` of round 1 lived in a vector
-          // register inside the elected branch: IMAD + R2UR per operand per MMA, ~110 cycles per MMA where
-          // the instruction itself needs 52 at N = 80 — profiles/r02_mma_probe.txt)
-          const uint32_t a_hiw = (uint32_t)(ad_hi0 >> 32), b_hiw = (uint32_t)(bd0 >> 32);
-          const uint32_t a0w = (uint32_t)ad_hi0 + tap_off, a1w = (uint32_t)ad_lo0 + tap_off, bw = (uint32_t)bd0;
-          if (tc::elect_one()) {
-            if (nk == 5) {
-              amp_issue<5>(d_tmem, a0w, a_hiw, bw, b_hiw, idesc, kstep_a, kstep_b, accumulate);
-              if (n_a == 2) amp_issue<5>(d_tmem, a1w, a_hiw, bw, b_hiw, idesc, kstep_a, kstep_b, 1u);
-            } else if (nk == 10) {
-              amp_issue<10>(d_tmem, a0w, a_hiw, bw, b_hiw, idesc, kstep_a, kstep_b, accumulate);
-              if (n_a == 2) amp_issue<10>(d_tmem, a1w, a_hiw, bw, b_hiw, idesc, kstep_a, kstep_b, 1u);
-            } else {
-              uint32_t acc_flag = accumulate;
-              for (int ap = 0; ap < n_a; ++ap) {
-                uint32_t ad = ap == 0 ? a0w : a1w, bd = bw;
-                for (int kk = 0; kk < nk; ++kk) {
-                  tc::mma_bf16_lohi(d_tmem, ad, a_hiw, bd, b_hiw, idesc, acc_flag);
-                  acc_flag = 1;
-                  ad += kstep_a;
-                  bd += kstep_b;
-                }
-              }
-            }
-            if (!resident) tc::mma_commit(&w_empty[st]);
+          const uint64_t bd = tc::smem_desc(wbase, lbo_b);
+          tc::wg_fence();
+          for (int ap = 0; ap < n_a; ++ap) {
+            const uint64_t ad = tc::smem_desc((ap == 0 ? a_hi : a_lo) + tap_off, lbo_a);
+#pragma unroll
+            for (int kk = 0; kk < NK; ++kk) tc::Wg<NC, 0>::ss(acc, ad + kk * ks_a, bd + kk * ks_b, 1u);
           }
-          accumulate = 1;
-          if (!resident) ++wi;
+          tc::wg_commit();
+          if (!resident) {
+            tc::wg_wait<0>();
+            if (t == 0) tc::mbar_arrive(&w_empty[st]);
+            ++wi;
+          }
         }
       }
-      if (tc::elect_one()) {
-        tc::mma_commit(&a_empty[buf]);
-        tc::mma_commit(&t_full[acc]);
-      }
-    }
-  } else if (warp < 8) {
-    // ---------------------------------------------------------------- epilogue
-    // Two groups of four warps (warp w reads TMEM lanes 32*(w%4)..+31) take alternate 16-column
-    // strips; inside a group the residual / accumulator loads of the NEXT strip are issued before
-    // the current strip is stored, so ~2 x 16 loads per thread are in flight (the epilogue is a
-    // DRAM-latency pipeline: measured 1.4 us per strip when each strip waited for its own loads).
-    const int grp = warp >> 2, wq = warp & 3;
-    const int nstrips = p.Cp / 16;
-    const bool do_div = p.out_div != 0.f;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const int b = tile / tpi, t0 = (tile - b * tpi) * TC_M;
-      const int t = t0 + wq * 32 + lane;
-      const bool live = t < p.L;
-      const long long rowb = (long long)b * p.C * p.L + t;
-      auto load_adds = [&](int strip, float (&add)[16]) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int co = strip * 16 + j;
-          float a = 0.f;
-          if (live && co < p.C) {
-            const long long off = rowb + (long long)co * p.L;
-            if (p.res) a = p.res[off];
-            if (p.accum) a += p.y[off];
-          }
-          add[j] = a;
-        }
-      };
-      float cur[16], nxt[16];
-      if (grp < nstrips) load_adds(grp, cur);   // independent of the accumulator: overlaps the MMA
-      tc::mbar_wait(&t_full[acc], (uint32_t)((it >> 1) & 1));
-      tc::fence_after_sync();
-      const uint32_t tbase = tmem + ((uint32_t)(wq * 32) << 16) + (uint32_t)(acc * acc_stride);
-      for (int strip = grp; strip < nstrips; strip += 2) {
-        uint32_t v[16], v2[16];
-        tc::tmem_ld16(tbase + (uint32_t)(strip * 16), v);
-        if (ncat) tc::tmem_ld16(tbase + (uint32_t)(p.Cp + strip * 16), v2);   // the A_hi x W_lo half
-        if (strip + 2 < nstrips) load_adds(strip + 2, nxt);
-        tc::tmem_ld_wait();
-        if (ncat) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-        }
-        if (live) {
+      tc::wg_wait<0>();
+      tc::wg_hold(acc);
+      if (t == 0) tc::mbar_arrive(&a_empty[buf]);
+
+      // epilogue: thread = (row t % 64, 32-column half t / 64) of every 64-column chunk
+      const int tt = t0 + wg * 64 + (t & 63);
+      const bool live = tt < p.L;
+      const long long rowb = (long long)b * p.C * p.L + tt;
+#pragma unroll 1
+      for (int ch = 0; ch < (NC + 63) / 64; ++ch) {
+        tc::named_sync(1 + wg, 128);
+        tc::acc_to_smem<NC>(acc, strip, AMP_EPI_LD, 8 * ch, 8 * ch + 8);
+        tc::named_sync(1 + wg, 128);
+#pragma unroll 1
+        for (int sub = 0; sub < 2; ++sub) {
+          const int cl = (t >> 6) * 32 + sub * 16, c0 = ch * 64 + cl;
+          if (c0 >= NC || !live) continue;
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            const int co = strip * 16 + j;
+            const int co = c0 + j;
             if (co < p.C) {
-              float o = __uint_as_float(v[j]) + __ldg(p.bias + co) + cur[j];
-              // a real (uniform) branch: if-converted, the division ran its x/0 slow path per element
-              // on every launch without a divisor (r01 source-level capture: 30 % of all instructions)
+              const long long off = rowb + (long long)co * p.L;
+              float a = 0.f;
+              if (p.res) a = p.res[off];
+              if (p.accum) a += p.y[off];
+              float o = strip[(t & 63) * AMP_EPI_LD + cl + j] + __ldg(p.bias + co) + a;
+              // a real (uniform) branch: if-converted, the division would run its x/0 slow path per element
               if (do_div) { asm volatile(""); o = o / p.out_div; }
-              p.y[rowb + (long long)co * p.L] = o;
+              p.y[off] = o;
             }
           }
         }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) cur[j] = nxt[j];
       }
-      tc::fence_before_sync();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(&t_empty[acc])) : "memory");
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 8) tc::tmem_dealloc(tmem, ncols);
 }
 
 static AmpPlan amp_plan(int Cp, int K, int dil, int nsplit) {
@@ -461,30 +320,19 @@ static AmpPlan amp_plan(int Cp, int K, int dil, int nsplit) {
   const size_t a_buf = (size_t)(Cp / 8) * R * 16 * parts;
   const size_t wb = (size_t)Cp * Cp * 2;
   const size_t nch = (size_t)K * parts;
-  const size_t limit = 227 * 1024 - 1024;
+  const size_t limit = 227 * 1024 - 1024 - AMP_STRIP_BYTES;
   AmpPlan pl;
-  // split operands, narrow tiles: W_hi | W_lo side by side along N (2 MMA groups per tap, not 3).
-  // Measured: C=40 (N 48 -> 96) k=11 0.98 -> 0.61 ms per launch, k=7 0.70 -> 0.52; C=80 (N 80 -> 160)
-  // got slower (k=11 0.41 -> 0.53 ms: an N=160 MMA costs twice an N=80 one and the ring needs 20
-  // small weight copies per tap), so the concatenation is used up to N = 128 only.
-  pl.ncat = (nsplit == 3 && 2 * Cp <= 128) ? 1 : 0;
-  const size_t wslot = pl.ncat ? 2 * wb : wb;   // one ring slot (ncat: both parts of a tap)
-  pl.acc_stride = ((pl.ncat ? 2 * Cp : Cp) + 31) / 32 * 32;
-  pl.ncols = (int)tc_cols_host(2 * pl.acc_stride);
-  // Measured (r01): resident weights + 2 A buffers (one CTA per SM) beat streaming weights with two
-  // CTAs per SM on the C=40/80 stages (33.0 vs 37.1 ms per step), so residency is preferred.
   pl.nw = 2;
-  if (2 * a_buf + nch * wb + 128 <= limit) { pl.resident = 1; pl.nabuf = 2; pl.smem = 2 * a_buf + nch * wb + 128; }
+  // resident weights + 2 A buffers when they fit, else a 2-slot weight ring with 2 (or 1) A buffers, else
+  // (wide dilated taps: C = 160, k = 11, dilation 5) one A buffer and one weight slot
+  if (2 * a_buf + nch * wb + 128 <= limit) { pl.resident = 1; pl.nabuf = 2; pl.smem = 2 * a_buf + nch * wb; }
   else {
-    // streaming weights.  A deeper ring (up to AMP_WMAX slots) was measured for C = 80 (8 x 12.8 KB instead of
-    // 2): no change — these launches are not waiting for weights (nor for the issue loop: the unrolled
-    // amp_issue<> path changed nothing either); their 23.5k cycles per tile against 8.6k of MMAs sit in the
-    // epilogue's residual-load / store round trips.  Two slots are kept.
     pl.resident = 0;
-    pl.nabuf = (2 * a_buf + 2 * wslot + 128 <= limit) ? 2 : 1;
-    pl.nw = 2;
-    pl.smem = pl.nabuf * a_buf + pl.nw * wslot + 128;
+    pl.nabuf = (2 * a_buf + 2 * wb + 128 <= limit) ? 2 : 1;
+    if (pl.nabuf == 1 && a_buf + 2 * wb + 128 > limit) pl.nw = 1;
+    pl.smem = pl.nabuf * a_buf + pl.nw * wb;
   }
+  pl.smem += AMP_STRIP_BYTES + 128;
   return pl;
 }
 
@@ -501,21 +349,27 @@ int launch_amp_conv_tc(const AmpConvParams& p, cudaStream_t s) {
   }
   const AmpPlan pl = amp_plan(p.Cp, p.K, p.dil, p.nsplit);
   if (pl.smem > 227 * 1024 - 512) { set_error("amp_conv_tc: tile does not fit shared memory"); return SVCB_E_UNSUPPORTED; }
-  static DevSmemCache attr_cache;  // the dynamic limit excludes the kernel's (small) static shared memory
-  SVCB_CUDA_CHECK(ensure_dyn_smem(amp_conv_tc_kernel, pl.smem, attr_cache));
   const int n_sm = device_sm_count();
   if (n_sm <= 0) { set_error("amp_conv_tc: cannot query the SM count"); return SVCB_E_CUDA; }
-  int occ = 1;
-  SVCB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, amp_conv_tc_kernel, 320, pl.smem));
-  occ = std::max(1, std::min(occ, 512 / pl.ncols));
   const int ntiles = p.B * ((p.L + TC_M - 1) / TC_M);
-  const int grid = std::min(ntiles, n_sm * occ);
+  const int grid = std::min(ntiles, n_sm);
   const double macs = (double)p.B * p.L * p.C * p.C * p.K;
   char kname[64];
   snprintf(kname, sizeof(kname), "amp_conv_tc_%s_c%dk%d", p.nsplit == 3 ? "bf16x3" : "bf16", p.C, p.K);
   KernelScope ks(kname, s, 2.0 * macs,
                  (double)p.B * p.C * p.L * ((p.nsplit == 3 ? 4.0 : 2.0) + 4.0 * (p.res ? 2 : 1)));
-  amp_conv_tc_kernel<<<grid, 320, pl.smem, s>>>(p, pl.resident, pl.nabuf, pl.nw, pl.acc_stride, (uint32_t)pl.ncols, pl.ncat);
+  switch (p.Cp / 16) {
+#define SVCB_AMP_NC(nb)                                                                                          \
+  case nb: {                                                                                                     \
+    static DevSmemCache attr_cache;                                                                              \
+    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_conv_tc_kernel<16 * nb>, pl.smem, attr_cache));                          \
+    amp_conv_tc_kernel<16 * nb><<<grid, AMP_THREADS, pl.smem, s>>>(p, pl.resident, pl.nabuf, pl.nw);             \
+    break;                                                                                                       \
+  }
+    SVCB_AMP_NC(1) SVCB_AMP_NC(2) SVCB_AMP_NC(3) SVCB_AMP_NC(4) SVCB_AMP_NC(5) SVCB_AMP_NC(6) SVCB_AMP_NC(7) SVCB_AMP_NC(8)
+    SVCB_AMP_NC(9) SVCB_AMP_NC(10) SVCB_AMP_NC(11) SVCB_AMP_NC(12) SVCB_AMP_NC(13) SVCB_AMP_NC(14) SVCB_AMP_NC(15) SVCB_AMP_NC(16)
+#undef SVCB_AMP_NC
+  }
   SVCB_LAUNCH_CHECK("amp_conv_tc");
   return SVCB_OK;
 }

@@ -3,20 +3,17 @@
 // One launch = one `Conv1d(C->C, k, dilation) [+ x] -> SnakeAlias` link of AMPBlock.forward
 // (vits_decoder/bigv.py:50-58; SnakeAlias = vits_decoder/alias/act.py:124-128), SURVEY.md §8a rows a9/a10.
 //
-// Why space-to-depth.  A tcgen05.mma (SS form, M = 128, K = 16) costs max(N/2, 32 + N/4) cycles on B200
-// (profiles/r02_mma_probe.txt): at N = C = 16..32 the tensor pipe idles on the A-operand read, which is
-// why round 1 ran C = 10 / 20 on the fp32 FMA pipe (26 % of ITS roof).  Folding r consecutive samples
-// into the channel dimension (C * r = 160: r = 8 for C = 20, 16 for C = 10) turns the dilated conv into
-// `ntaps` dense 160 x 160 block-Toeplitz products over rows of r samples (pack.py:conv_s2d_matrices):
-// 2-8x more MACs, all of them at the full-rate N = 160 shape (80 cycles per MMA = 8192 FLOP/cycle/SM).
+// Why space-to-depth.  At N = C = 16..32 an MMA spends its time reading the A operand and the tensor
+// pipe idles.  Folding r consecutive samples into the channel dimension (C * r = 160: r = 8 for C = 20,
+// 16 for C = 10) turns the dilated conv into `ntaps` dense 160 x 160 block-Toeplitz products over rows of
+// r samples (pack.py:conv_s2d_matrices): 2-8x more MACs, all of them at the wide N = 160 shape.
 //
 // Why the Snake lives in the epilogue.  In this layout an accumulator row holds r CONSECUTIVE samples of
-// each channel: the epilogue thread that owns TMEM lane tau has, per channel, exactly the register-resident
+// each channel: the epilogue thread that owns accumulator row tau has, per channel, exactly the register-resident
 // run of samples the SnakeAlias code of round 1 works on.  It adds bias (+ residual), parks the run in a
 // 4 KB shared strip so that neighbouring rows are visible, and computes the anti-aliased Snake of the
 // NEXT link straight into that link's bf16 hi/lo operand image — no snake_pack pass, no fp32 round trip:
-// 8-12 B of HBM traffic per element and link (was 20-24), and the CUDA-core work overlaps the MMAs of
-// the next tile (two TMEM accumulators).
+// 8-12 B of HBM traffic per element and link (was 20-24).
 //
 // Data layout ("S2D image"): bf16 hi and lo, [B][20 octets][Rp][8]; element (octet o, row, e) is
 // snake(x)[b][c][r*(row - 16) + p] with 8*o + e = c*r + p.  Rows outside the sequence are zero (the
@@ -41,15 +38,16 @@ constexpr int PADR = 16;          // zero rows in front of every (item, octet) o
 constexpr int TILE = 128;         // accumulator rows per tile
 constexpr uint32_t A_PART = KC * RA * 16;       // 46,080 B
 constexpr uint32_t W_SLOT = KC * N * 16;        // 51,200 B: one (tap, hi|lo) matrix
-constexpr int GROUPS = 5;                       // epilogue column groups (x 4 TMEM lane quadrants = 20 warps)
+constexpr int GROUPS = 3;                       // epilogue column groups (x 4 row quadrants of 32 = 12 warps)
 constexpr int STRIP = TILE * 8;                 // floats of one group's strip: 128 rows x (first 4 | last 4 samples) of one channel,
                                                 // or 128 rows x 4 samples of two channels (r = 4)
 constexpr uint32_t STG_BYTES = 64 + GROUPS * STRIP * 4 + 64 + GROUPS * 128 * 4;  // sample strips (+ guards) + edge buffers
 constexpr uint32_t SMEM = 2 * A_PART + 2 * W_SLOT + STG_BYTES;
 static_assert(SMEM + 1024 <= 227 * 1024, "A panel + weight ring + strips must fit the 227 KB of one CTA");
 constexpr int EPI_WARPS = 4 * GROUPS;
-constexpr int THREADS = (EPI_WARPS + 2) * 32;
-constexpr uint32_t ACC_STRIDE = 256;            // TMEM columns between the two accumulators
+constexpr int THREADS = (EPI_WARPS + 1) * 32;
+constexpr int ACC_LD = N + 4;                   // floats per row of the staged accumulator (over the A panel)
+static_assert(TILE * ACC_LD * 4 <= 2 * A_PART, "the staged accumulator must fit over the A panel");
 }  // namespace s2d
 
 int s2d_halo_rows(int r) { return r >= 8 ? 1 : 2; }                 // SnakeAlias reaches +-5 samples
@@ -163,21 +161,18 @@ int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, in
 // ------------------------------------------------------------------------------------------------ link
 // Persistent: every CTA walks tiles (item, 126 useful rows) with a static stride.
 //   producer warp  A panel of the tile (40 bulk copies) and the (tap, hi|lo) weight matrices through a
-//                  2-slot ring (one 51,200-byte bulk copy each)
-//   MMA warp       per tap: A_hi x W_hi, A_lo x W_hi, A_hi x W_lo — 30 MMAs (N = 160) with compile-time
-//                  descriptor offsets (no per-MMA integer work in the issuing thread)
-//   20 epilogue warps = 5 column groups x 4 TMEM lane quadrants: group g owns units u = g (mod 5), a unit
-//                  being one channel (r >= 8) or a channel pair (r = 4): 4 / 4 / 2 units per group for
-//                  C = 20 / 40 / 10 — balanced for every stage
-#define S2D_TRACE(slot) do { if (p.trace && blockIdx.x == 0 && it < 32 && lane == 0) p.trace[it * 16 + (slot)] = clock64(); } while (0)
-
+//                  2-slot ring (four bulk copies each)
+//   warpgroups 0-1 per tap: A_hi x W_hi, A_lo x W_hi, A_hi x W_lo — 30 wgmma m64n160k16 each for its 64 rows,
+//                  register accumulators, then staged as fp32 rows over the (consumed) A panel
+//   12 epilogue warps = 3 column groups x 4 row quadrants: group g owns units u = g (mod 3), a unit
+//                  being one channel (r >= 8) or a channel pair (r = 4): 6-7 / 6-7 / 3-4 units per group for
+//                  C = 20 / 40 / 10 (13 warps leave the MMA warpgroups the registers of 160 accumulator columns)
 template <int R>
 __global__ void __launch_bounds__(s2d::THREADS, 1)
 amp_s2d_link_kernel(const AmpS2dParams p) {
   using namespace s2d;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t a_full, a_empty, w_full[2], w_empty[2], t_full[2], t_empty[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t a_full, a_empty, w_full[2], w_empty[2];
   __shared__ float s_par[3][40];      // bias | exp(alpha) | 1 / (exp(beta) + 1e-9) of every channel (C <= 40)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -195,21 +190,14 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
   uint8_t* Abase = smem;
   uint8_t* Wbase = smem + 2 * A_PART;
   float* Stg = reinterpret_cast<float*>(smem + 2 * A_PART + 2 * W_SLOT);
+  float* Acc = reinterpret_cast<float*>(smem);   // staged accumulator [TILE][ACC_LD], over the A panel
 
   if (tid == 0) {
     tc::mbar_init(&a_full, 1); tc::mbar_init(&a_empty, 1);
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 1);
-      tc::mbar_init(&t_full[i], 1); tc::mbar_init(&t_empty[i], EPI_WARPS * 32);
-    }
+    for (int i = 0; i < 2; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 2); }
     tc::fence_barrier_init();
   }
-  __syncwarp();
-  if (warp == EPI_WARPS) tc::tmem_alloc(&tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = tmem_slot;
 
   if (warp_u == EPI_WARPS) {
     // ------------------------------------------------------------------------------------ producer
@@ -221,19 +209,15 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
         const int b = tile / tpi, t = tile - b * tpi;
         const long long row0 = (long long)t * S - HS - A_OFF + PADR;     // image row of A-panel row 0 (>= 6)
-        if (p.trace && blockIdx.x == 0 && it < 32) p.trace[it * 16 + 0] = clock64();
         if (it >= 1) tc::mbar_wait_parked(&a_empty, (uint32_t)((it - 1) & 1));
-        if (p.trace && blockIdx.x == 0 && it < 32) p.trace[it * 16 + 1] = clock64();
         tc::mbar_arrive_expect_tx(&a_full, 2 * A_PART);
         for (int part = 0; part < 2; ++part)
           for (int kc = 0; kc < KC; ++kc)
             tc::bulk_g2s(Abase + (size_t)part * A_PART + (size_t)kc * RA * 16,
                          img[part] + ((((long long)b * KC + kc) * p.Rp) + row0) * 16, RA * 16, &a_full);
-        if (p.trace && blockIdx.x == 0 && it < 32) p.trace[it * 16 + 2] = clock64();
         for (int c = 0; c < 2 * p.ntaps; ++c, ++wi) {
           const int st = wi & 1;
           if (wi >= 2) tc::mbar_wait_parked(&w_empty[st], (uint32_t)(((wi >> 1) - 1) & 1));
-          if (c == 0 && p.trace && blockIdx.x == 0 && it < 32) p.trace[it * 16 + 3] = clock64();
           tc::mbar_arrive_expect_tx(&w_full[st], W_SLOT);
 #pragma unroll
           for (int piece = 0; piece < 4; ++piece)    // four requests in flight per matrix instead of one long one
@@ -242,67 +226,18 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
         }
       }
     }
-  } else if (warp_u == EPI_WARPS + 1) {
-    // ------------------------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = tc::idesc_bf16(TILE, N);
-    constexpr uint32_t LBO_A = RA * 16, LBO_B = N * 16;
-    constexpr uint32_t KSA = (2 * LBO_A) >> 4, KSB = (2 * LBO_B) >> 4;      // descriptor step per K = 16
-    const uint64_t adh = tc::smem_desc(tc::smem_u32(Abase), LBO_A), adl = tc::smem_desc(tc::smem_u32(Abase + A_PART), LBO_A);
-    const uint64_t bd0 = tc::smem_desc(tc::smem_u32(Wbase), LBO_B), bd1 = tc::smem_desc(tc::smem_u32(Wbase + W_SLOT), LBO_B);
-    const uint32_t d_hi = (uint32_t)(adh >> 32);          // identical high words (SBO, version) for A and B
-    int it = 0, wi = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      S2D_TRACE(4);
-      tc::mbar_wait_parked(&a_full, (uint32_t)(it & 1));
-      S2D_TRACE(5);
-      if (it >= 2) tc::mbar_wait_parked(&t_empty[acc], (uint32_t)(((it >> 1) - 1) & 1));
-      S2D_TRACE(6);
-      tc::fence_after_sync();
-      const uint32_t d_tmem = tmem + (uint32_t)acc * ACC_STRIDE;
-      for (int tap = 0; tap < p.ntaps; ++tap) {
-        const uint32_t arow = (uint32_t)(A_OFF - p.mlo + tap);            // row shift = 16-byte units
-        const uint32_t a_h = (uint32_t)adh + arow, a_l = (uint32_t)adl + arow;
-        {  // W_hi of this tap: A_hi x W_hi, A_lo x W_hi
-          const int st = wi & 1;
-          tc::mbar_wait_parked(&w_full[st], (uint32_t)((wi >> 1) & 1));
-          if (tap == 0) S2D_TRACE(7);
-          if (tap == 1) S2D_TRACE(8);
-          tc::fence_after_sync();
-          const uint32_t bw = (uint32_t)(st ? bd1 : bd0);
-          if (tc::elect_one()) {
-            tc::mma_bf16_lohi(d_tmem, a_h, d_hi, bw, d_hi, idesc, tap > 0 ? 1u : 0u);
-#pragma unroll
-            for (int kk = 1; kk < N / 16; ++kk) tc::mma_bf16_lohi(d_tmem, a_h + kk * KSA, d_hi, bw + kk * KSB, d_hi, idesc, 1u);
-#pragma unroll
-            for (int kk = 0; kk < N / 16; ++kk) tc::mma_bf16_lohi(d_tmem, a_l + kk * KSA, d_hi, bw + kk * KSB, d_hi, idesc, 1u);
-            tc::mma_commit(&w_empty[st]);
-          }
-          ++wi;
-        }
-        {  // W_lo of this tap: A_hi x W_lo
-          const int st = wi & 1;
-          tc::mbar_wait_parked(&w_full[st], (uint32_t)((wi >> 1) & 1));
-          tc::fence_after_sync();
-          const uint32_t bw = (uint32_t)(st ? bd1 : bd0);
-          if (tc::elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < N / 16; ++kk) tc::mma_bf16_lohi(d_tmem, a_h + kk * KSA, d_hi, bw + kk * KSB, d_hi, idesc, 1u);
-            tc::mma_commit(&w_empty[st]);
-          }
-          ++wi;
-        }
-      }
-      if (tc::elect_one()) {
-        tc::mma_commit(&a_empty);
-        tc::mma_commit(&t_full[acc]);
-      }
-      S2D_TRACE(9);
-    }
-  } else {
+    return;
+  }
+  {
     // ------------------------------------------------------------------------------------ epilogue
     const int q = warp & 3, g = warp >> 2;
     const int row = q * 32 + lane;
+    const int wg = warp >> 2, tw = tid & 127;
+    constexpr uint32_t LBO_A = RA * 16, LBO_B = N * 16;
+    constexpr uint64_t KSA = (2 * LBO_A) >> 4, KSB = (2 * LBO_B) >> 4;      // descriptor step per K = 16
+    const uint32_t a_h0 = tc::smem_u32(Abase) + (uint32_t)wg * 64u * 16u, a_l0 = a_h0 + A_PART, w_s0 = tc::smem_u32(Wbase);
+    const float* arow = Acc + row * ACC_LD;
+    int wi = 0;
     constexpr int CU = R >= 8 ? R : 8;            // accumulator columns per unit: whole channels, >= one image octet
     constexpr int NCH = CU / R;                   // channels per unit (2 for R = 4)
     const int NU = p.C / NCH;
@@ -313,7 +248,6 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
     const bool do_div = p.out_div != 0.f;
     int it = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
       const int b = tile / tpi, t = tile - b * tpi;
       const int tau0 = t * S - HS;
       const int tau = tau0 + row;
@@ -332,32 +266,59 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
         }
       };
       load_res(g, rcur);
-      if (warp == 0) S2D_TRACE(10);
-      tc::mbar_wait_parked(&t_full[acc], (uint32_t)((it >> 1) & 1));
-      if (warp == 0) S2D_TRACE(11);
-      tc::fence_after_sync();
-      const uint32_t tbase = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * ACC_STRIDE;
-      // accumulator columns are fetched one unit ahead (8-column units): the tcgen05.ld of unit u+4 is in
-      // flight while unit u runs its Snake
+      if (wg < 2) {
+        // ---------------------------------------------------------------- MMAs of this warpgroup's 64 rows
+        tc::mbar_wait_parked(&a_full, (uint32_t)(it & 1));
+        float acc[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+        for (int tap = 0; tap < p.ntaps; ++tap) {
+          const uint32_t arow_off = (uint32_t)(A_OFF - p.mlo + tap) * 16u;   // row shift
+          const uint64_t ah = tc::smem_desc(a_h0 + arow_off, LBO_A), al = tc::smem_desc(a_l0 + arow_off, LBO_A);
+          for (int part = 0; part < 2; ++part, ++wi) {   // W_hi: A_hi x W_hi, A_lo x W_hi;  W_lo: A_hi x W_lo
+            const int st = wi & 1;
+            tc::mbar_wait_parked(&w_full[st], (uint32_t)((wi >> 1) & 1));
+            const uint64_t bw = tc::smem_desc(w_s0 + (uint32_t)st * W_SLOT, LBO_B);
+            tc::wg_fence();
+#pragma unroll
+            for (int kk = 0; kk < N / 16; ++kk) tc::Wg<N, 0>::ss(acc, ah + kk * KSA, bw + kk * KSB, 1u);
+            if (part == 0) {
+#pragma unroll
+              for (int kk = 0; kk < N / 16; ++kk) tc::Wg<N, 0>::ss(acc, al + kk * KSA, bw + kk * KSB, 1u);
+            }
+            tc::wg_commit();
+            tc::wg_wait<0>();
+            if (tw == 0) tc::mbar_arrive(&w_empty[st]);
+          }
+        }
+        tc::wg_hold(acc);
+        tc::named_sync(6, 256);                   // both warpgroups' MMAs are done: the A panel is free
+        tc::acc_to_smem<N>(acc, Acc + wg * 64 * ACC_LD, ACC_LD, 0, N / 8);
+      }
+      tc::named_sync(7, EPI_WARPS * 32);          // accumulator rows staged
+      auto ld_acc = [&](int col, uint32_t* dst, int n) {
+        for (int k = 0; k < n; k += 4) {
+          const float4 q4 = *reinterpret_cast<const float4*>(arow + col + k);
+          dst[k] = __float_as_uint(q4.x); dst[k + 1] = __float_as_uint(q4.y); dst[k + 2] = __float_as_uint(q4.z); dst[k + 3] = __float_as_uint(q4.w);
+        }
+      };
       uint32_t wpre[8];
-      if constexpr (CU == 8) tc::tmem_ld8(tbase + (uint32_t)(g * CU), wpre);
+      if constexpr (CU == 8) ld_acc(g * CU, wpre, 8);
       for (int u = g; u < NU; u += GROUPS) {                     // unit = one channel (R >= 8) or a channel pair (R = 4)
         if (u + GROUPS < NU) load_res(u + GROUPS, rnext);
         const int c0 = u * NCH;
         float v[CU];
         if constexpr (CU == 8) {
-          tc::tmem_ld_wait8(wpre);
 #pragma unroll
           for (int k = 0; k < NCH; ++k) {
             const float bias = s_par[0][c0 + k];
 #pragma unroll
             for (int j = 0; j < R; ++j) v[k * R + j] = __uint_as_float(wpre[k * R + j]) + bias;
           }
-          if (u + GROUPS < NU) tc::tmem_ld8(tbase + (uint32_t)((u + GROUPS) * CU), wpre);
+          if (u + GROUPS < NU) ld_acc((u + GROUPS) * CU, wpre, 8);
         } else {
           uint32_t w[CU];
-          tc::tmem_ld16(tbase + (uint32_t)(u * CU), w);
-          tc::tmem_ld_wait();
+          ld_acc(u * CU, w, CU);
           const float bias = s_par[0][c0];
 #pragma unroll
           for (int j = 0; j < R; ++j) v[j] = __uint_as_float(w[j]) + bias;
@@ -404,7 +365,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
           asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
           // 2x-rate Snake values as (even, odd) pairs V[a + 3], a = position relative to the row's first sample:
           // own a = 0 .. R-1; the previous row's last five values are V[0].y, V[1], V[2], the next row's first five
-          // V[R+3], V[R+4], V[R+5].x.  All FIR / range-reduction arithmetic runs as packed f32x2 FMAs (FFMA2 /
+          // V[R+3], V[R+4], V[R+5].x.  All FIR / range-reduction arithmetic runs as f32x2 pair operations (f2_fma /
           // FMUL2 / FADD2: one issue slot for the even and the odd phase), taps as uniform-register pairs.
           float2 V[NCH][R + 6];
 #pragma unroll
@@ -421,7 +382,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
             for (int j = 0; j < R; ++j) xw[4 + j] = v[k * R + j];
             xw[R + 4] = r4.x; xw[R + 5] = r4.y; xw[R + 6] = r4.z; xw[R + 7] = r4.w;
             // consecutive-sample pairs in both alignments, each held in its own (aligned) register pair so that
-            // every FIR step is one FFMA2: XE[m] = (x[2m], x[2m+1]), XO[m] = (x[2m+1], x[2m+2])  (x = xw)
+            // every FIR step is one f2_fma: XE[m] = (x[2m], x[2m+1]), XO[m] = (x[2m+1], x[2m+2])  (x = xw)
             float2 XE[(R + 8) / 2], XO[(R + 6) / 2];
 #pragma unroll
             for (int m2 = 0; m2 < (R + 8) / 2; ++m2) XE[m2] = make_float2(xw[2 * m2], xw[2 * m2 + 1]);
@@ -435,18 +396,18 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
               for (int i = 0; i < 6; ++i) {
                 const int j = a + 1 + i;
                 const float2 pr = (j & 1) ? XO[(j - 1) / 2] : XE[j / 2];
-                U = i == 0 ? __fmul2_rn(pr, p.fup[0]) : __ffma2_rn(pr, p.fup[i], U);
+                U = i == 0 ? f2_mul(pr, p.fup[0]) : f2_fma(pr, p.fup[i], U);
               }
               // u + sin^2(a u) / (e^beta + 1e-9) = (u + b/2) - (b/2) cos(2 a u); a u = k pi + r, |r| <= pi/2
-              const float2 t = __fmul2_rn(U, make_float2(a_, a_));
-              const float2 kq = __fadd2_rn(__ffma2_rn(t, make_float2(0.3183098861837907f, 0.3183098861837907f),
+              const float2 t = f2_mul(U, make_float2(a_, a_));
+              const float2 kq = f2_add(f2_fma(t, make_float2(0.3183098861837907f, 0.3183098861837907f),
                                                       make_float2(12582912.f, 12582912.f)),
                                            make_float2(-12582912.f, -12582912.f));
-              float2 rr = __ffma2_rn(kq, make_float2(-3.140625f, -3.140625f), t);
-              rr = __ffma2_rn(kq, make_float2(-9.676535897932e-4f, -9.676535897932e-4f), rr);
-              rr = __fadd2_rn(rr, rr);
+              float2 rr = f2_fma(kq, make_float2(-3.140625f, -3.140625f), t);
+              rr = f2_fma(kq, make_float2(-9.676535897932e-4f, -9.676535897932e-4f), rr);
+              rr = f2_add(rr, rr);
               const float2 cs = make_float2(__cosf(rr.x), __cosf(rr.y));
-              V[k][a + 3] = __ffma2_rn(make_float2(-hb_, -hb_), cs, __fadd2_rn(U, make_float2(hb_, hb_)));
+              V[k][a + 3] = f2_fma(make_float2(-hb_, -hb_), cs, f2_add(U, make_float2(hb_, hb_)));
             }
             float* edge = edge_g + (q * NCH + k) * 16;
             if (lane == 0) {
@@ -488,9 +449,9 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
 #pragma unroll
             for (int n = 0; n < R; ++n) {
               // out[n] = v[2n-5] f0 + sum_i (v[2n-4+2i], v[2n-3+2i]) . (f[2i+1], f[2i+2]) + v[2n+6] f11
-              float2 acc2 = __fmul2_rn(V[k][n + 1], p.fdp[0]);
+              float2 acc2 = f2_mul(V[k][n + 1], p.fdp[0]);
 #pragma unroll
-              for (int i = 1; i < 5; ++i) acc2 = __ffma2_rn(V[k][n + 1 + i], p.fdp[i], acc2);
+              for (int i = 1; i < 5; ++i) acc2 = f2_fma(V[k][n + 1 + i], p.fdp[i], acc2);
               float o1 = acc2.x + acc2.y;
               o1 = fmaf(V[k][n].y, p.fd0, o1);
               out[k * R + n] = fmaf(V[k][n + 6].x, p.fd11, o1);
@@ -509,15 +470,11 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
           }
         }
       }
-      tc::fence_before_sync();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(&t_empty[acc])) : "memory");
-      if (warp == 0) S2D_TRACE(12);
-      if (warp == 15) S2D_TRACE(13);
+      tc::fence_proxy_async_smem();               // staged rows (generic proxy) -> the next tile's bulk copies
+      tc::named_sync(7, EPI_WARPS * 32);
+      if (tid == 0) tc::mbar_arrive(&a_empty);
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == s2d::EPI_WARPS) tc::tmem_dealloc(tmem, 512);
 }
 
 static long long* g_s2d_trace = nullptr;

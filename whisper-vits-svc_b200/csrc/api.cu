@@ -387,7 +387,7 @@ static int run_amp_stage(const svcb_model* m, Ctx& ctx, int stage, const float* 
   for (int j = 0; j < nres; ++j) {
     const ResBlock& R = m->res[stage * nres + j];
     if (prec == 3 && R.s2d_r && S2D[0] && L % R.s2d_r == 0 && L % 8 == 0) {
-      // narrow stages: every link = block-Toeplitz tcgen05 conv with the next SnakeAlias in its epilogue
+      // narrow stages: every link = block-Toeplitz wgmma conv with the next SnakeAlias in its epilogue
       const int Rp = s2d_rows(L, R.s2d_r);
       void *ia_hi = S2D[0], *ia_lo = S2D[1], *ib_hi = S2D[2], *ib_lo = S2D[3];
       const SnakeTapsV tv0 = R.act[0].tapsv();
@@ -904,8 +904,8 @@ int svcb_model_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor
   SVCB_CUDA_CHECK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   SVCB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) {
-    set_error("libsvc_b200 is built for sm_100a only; device is sm_" + std::to_string(prop.major) +
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("libsvc_b200 is built for sm_90a only; device is sm_" + std::to_string(prop.major) +
               std::to_string(prop.minor));
     return SVCB_E_UNSUPPORTED;
   }

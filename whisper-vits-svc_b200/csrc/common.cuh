@@ -1,4 +1,4 @@
-// Shared declarations for libsvc_b200.so (sm_100a only).
+// Shared declarations for libsvc_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -92,7 +92,7 @@ __device__ __forceinline__ float snake_cos2(float x) {
   return __cosf(r + r);
 }
 
-// The 12 + 12 alias-filter taps of a SnakeAlias BY VALUE, paired for packed f32x2 FMAs (FFMA2 takes a uniform-
+// The 12 + 12 alias-filter taps of a SnakeAlias BY VALUE, paired for the f32x2 pair FMAs (f2_fma; a tap pair is a uniform-
 // register pair as an operand: no register holds a tap).  fup[j] = 2 * (up[11-2j], up[10-2j]) (UpSample1d's
 // ratio gain folded in, exact); fdp[m] = (dn[2m+1], dn[2m+2]); the decimator's two end taps apart.
 struct SnakeTapsV {
@@ -113,10 +113,18 @@ int launch_post_fused(const float* x, float* wave, const float* ea, const float*
 int snake_taps_from_device(const float* fu_dev, const float* fd_dev, SnakeTapsV* out);
 
 #ifdef __CUDACC__
+// f32x2 pair arithmetic, one correctly rounded fp32 operation per lane (Hopper has no packed FFMA2 / FMUL2 / FADD2:
+// the pairs keep the even / odd phases of the FIRs together and compile to two scalar instructions each).
+__device__ __forceinline__ float2 f2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 f2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 f2_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+#endif
+
+#ifdef __CUDACC__
 // SnakeAlias of 8 consecutive samples n0 .. n0+7 from the 24 inputs x[0..24) = signal[n0-8 .. n0+16)
 // (alias/resample.py:25-33 up x2, alias/act.py:79-92 Snake, alias/filter.py:86-94 + resample.py:52-58 down x2),
 // all FIR and range-reduction arithmetic as packed f32x2 FMAs: the pair V[p] = (v[2p], v[2p+1]) of the 2x signal
-// is one FFMA2 chain over the input pairs (x[p+2+j], x[p+3+j]); sin^2 = (1 - cos 2r) / 2 with the two-constant
+// is one f2_fma chain over the input pairs (x[p+2+j], x[p+3+j]); sin^2 = (1 - cos 2r) / 2 with the two-constant
 // reduction of snake_cos2; the decimator sums five pair products + its two end taps.  hb = 0.5 / (exp(beta) + eps).
 // first / last: the run starts at sample 0 / ends at the last sample — the 2x signal is replicate-padded there.
 __device__ __forceinline__ void snake8_packed(const float (&x)[24], const SnakeTapsV& tp, float a_, float hb_, float (&o)[8],
@@ -125,17 +133,17 @@ __device__ __forceinline__ void snake8_packed(const float (&x)[24], const SnakeT
   const float2 a2 = make_float2(a_, a_), hb2 = make_float2(hb_, hb_), nhb2 = make_float2(-hb_, -hb_);
 #pragma unroll
   for (int p = 0; p < 14; ++p) {
-    float2 U = __fmul2_rn(make_float2(x[p + 2], x[p + 3]), tp.fup[0]);
+    float2 U = f2_mul(make_float2(x[p + 2], x[p + 3]), tp.fup[0]);
 #pragma unroll
-    for (int j = 1; j < 6; ++j) U = __ffma2_rn(make_float2(x[p + 2 + j], x[p + 3 + j]), tp.fup[j], U);
-    const float2 t = __fmul2_rn(U, a2);
-    const float2 kq = __fadd2_rn(__ffma2_rn(t, make_float2(0.3183098861837907f, 0.3183098861837907f), make_float2(12582912.f, 12582912.f)),
+    for (int j = 1; j < 6; ++j) U = f2_fma(make_float2(x[p + 2 + j], x[p + 3 + j]), tp.fup[j], U);
+    const float2 t = f2_mul(U, a2);
+    const float2 kq = f2_add(f2_fma(t, make_float2(0.3183098861837907f, 0.3183098861837907f), make_float2(12582912.f, 12582912.f)),
                                  make_float2(-12582912.f, -12582912.f));
-    float2 rr = __ffma2_rn(kq, make_float2(-3.140625f, -3.140625f), t);
-    rr = __ffma2_rn(kq, make_float2(-9.676535897932e-4f, -9.676535897932e-4f), rr);
-    rr = __fadd2_rn(rr, rr);
+    float2 rr = f2_fma(kq, make_float2(-3.140625f, -3.140625f), t);
+    rr = f2_fma(kq, make_float2(-9.676535897932e-4f, -9.676535897932e-4f), rr);
+    rr = f2_add(rr, rr);
     const float2 cs = make_float2(__cosf(rr.x), __cosf(rr.y));
-    V[p] = __ffma2_rn(nhb2, cs, __fadd2_rn(U, hb2));
+    V[p] = f2_fma(nhb2, cs, f2_add(U, hb2));
   }
   if (first) {   // v[0 .. 6) = v[6]
     const float2 e = make_float2(V[3].x, V[3].x);
@@ -147,9 +155,9 @@ __device__ __forceinline__ void snake8_packed(const float (&x)[24], const SnakeT
   }
 #pragma unroll
   for (int i = 0; i < 8; ++i) {   // o_i = sum_k v[2i + 1 + k] dn[k]
-    float2 acc = __fmul2_rn(V[i + 1], tp.fdp[0]);
+    float2 acc = f2_mul(V[i + 1], tp.fdp[0]);
 #pragma unroll
-    for (int m = 1; m < 5; ++m) acc = __ffma2_rn(V[i + 1 + m], tp.fdp[m], acc);
+    for (int m = 1; m < 5; ++m) acc = f2_fma(V[i + 1 + m], tp.fdp[m], acc);
     o[i] = fmaf(V[i].y, tp.fd0, fmaf(V[i + 6].x, tp.fd11, acc.x + acc.y));
   }
 }

@@ -1,4 +1,4 @@
-// General Conv1d as an implicit GEMM on tcgen05/TMEM (bf16 or bf16x3 operands, fp32 accumulate).
+// General Conv1d as an implicit GEMM on wgmma (bf16 or bf16x3 operands, fp32 accumulate).
 //
 // Serves every dense convolution of the prior encoder, the flow and the generator head
 // (vits/models.py:44-49, vits/attentions.py:215-223,390-398, vits/modules.py:184-198,296-299,
@@ -6,15 +6,15 @@
 // the tensor cores (SURVEY.md §8a rows a2-a7).
 //
 //   D[t, co] = sum_cc sum_tap  A_cc[t + tap*dil, :] . W[tap, cc][co, :]      M = 128, N = BN, K = KCH
-// * Input channels are processed in chunks of KCH (32 or 64).  Eight producer warps gather one
-//   chunk of x (fp32, any strides — the time-major PPG input included), apply the optional input
-//   mask and the conv's zero padding, split to bf16 hi/lo and write the K-major panel layout of
-//   tc.cuh into a 2-deep A ring (generic proxy -> fence.proxy.async -> mbarrier).
+// * Input channels are processed in chunks of KCH (32 or 64).  Two warpgroups gather one chunk of x
+//   (fp32, any strides — the time-major PPG input included), apply the optional input mask and the
+//   conv's zero padding, split to bf16 hi/lo and write the K-major panel layout of tc.cuh into a
+//   2-deep A ring; the gather of chunk cc+1 overlaps the MMAs of chunk cc still in flight.
 // * For every (chunk, tap) the pre-packed weight tiles (hi, lo) arrive by 1-D bulk copy into a
-//   3-deep W ring.  One thread issues the MMAs: taps reuse the same A chunk through a row-shifted
-//   descriptor; tcgen05.commit releases W slots and A buffers.
-// * Epilogue (the producer warps again): tcgen05.ld -> bias -> {none, ReLU, Mish, tanh, WaveNet
-//   gate on interleaved channel pairs} -> output mask -> residual -> accumulate -> store [B,C,T].
+//   3-deep W ring (producer thread).  Each warpgroup issues wgmma m64nBNk16 for its 64 rows: taps
+//   reuse the same A chunk through a row-shifted descriptor.
+// * Epilogue (the same warpgroups, through a shared-memory strip): bias -> {none, ReLU, Mish, tanh,
+//   WaveNet gate on interleaved channel pairs} -> output mask -> residual -> accumulate -> store [B,C,T].
 #include <cstdio>
 
 #include "common.cuh"
@@ -24,7 +24,9 @@ namespace svcb {
 
 constexpr int CT_M = 128;
 constexpr int CT_WST = 3;  // W ring depth (max)
-static inline unsigned tc_cols(int n) { return n <= 32 ? 32u : n <= 64 ? 64u : n <= 128 ? 128u : n <= 256 ? 256u : 512u; }
+constexpr int CT_EPI_LD = 72;   // floats per row of an epilogue strip
+constexpr int CT_THREADS = 288;
+constexpr size_t CT_STRIP_BYTES = 2 * 64 * CT_EPI_LD * 4;
 
 __device__ __forceinline__ float ct_act(float v, int act) {
   switch (act) {
@@ -36,17 +38,12 @@ __device__ __forceinline__ float ct_act(float v, int act) {
   }
 }
 
-__device__ __forceinline__ void ct_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(bar)) : "memory");
-}
-
-__global__ void __launch_bounds__(320, 1)
+template <int BN>
+__global__ void __launch_bounds__(CT_THREADS, 1)
 conv_tc_kernel(const ConvTcParams p, const int wst) {
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t a_full[2], a_empty[2], w_full[CT_WST], w_empty[CT_WST], bar_acc;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int warp_u = tc::warp_uniform_idx();
+  __shared__ __align__(8) uint64_t w_full[CT_WST], w_empty[CT_WST];
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int b = blockIdx.z, nt = blockIdx.y;
   const int t0 = blockIdx.x * CT_M;
   const int P = p.pad;
@@ -56,32 +53,36 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
   const uint32_t a_part = (uint32_t)KC * R * 16u; // one of hi / lo
   const int nparts = p.nsplit == 3 ? 2 : 1;
   const uint32_t a_buf = a_part * nparts;
-  const uint32_t w_tile = (uint32_t)p.kch * p.bn * 2u;
+  const uint32_t w_tile = (uint32_t)p.kch * BN * 2u;
   uint8_t* A0 = smem;
   uint8_t* W0 = smem + 2 * a_buf;
+  float* Strips = reinterpret_cast<float*>(W0 + (size_t)wst * w_tile);
   const int ncc = p.cin_pad / p.kch;
   const long long len = p.lengths ? p.lengths[b] : (long long)1 << 60;
 
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&a_full[i], 256); tc::mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < wst; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 1); }
-    tc::mbar_init(&bar_acc, 1);
+    for (int i = 0; i < wst; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 2); }
     tc::fence_barrier_init();
   }
-  const uint32_t ncols = tc::tmem_cols_for(p.bn);
-  __syncwarp();
-  if (warp == 4) tc::tmem_alloc(&tmem_slot, ncols);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = tmem_slot;
 
-  if (warp < 4 || warp >= 6) {
-    // ---------------------------------------------------------------- A producers: the eight warps that run the
-    // epilogue later.  A thread fetches TWO items (16 scalar or 4 vector loads in flight) before it converts either:
-    // with four warps and one item at a time a chunk cost ~4 global-load latencies and the gather, not the MMAs,
-    // set the pace of every small convolution (profiles/r02_notes.md §9).
-    const int pid = warp < 4 ? tid : tid - 64;   // 0 .. 255
+  if (tid == 256) {
+    // ---------------------------------------------------------------- W producer
+    const int total = ncc * p.K * nparts;
+    for (int i = 0; i < total; ++i) {
+      const int st = i % wst;
+      if (i >= wst) tc::mbar_wait(&w_empty[st], (uint32_t)(((i / wst) - 1) & 1));
+      const int part = i % nparts, tap = (i / nparts) % p.K, cc = i / (nparts * p.K);
+      const size_t tile = (((size_t)tap * ncc + cc) * 2 + part) * p.ntiles + nt;
+      tc::mbar_arrive_expect_tx(&w_full[st], w_tile);
+      tc::bulk_g2s(W0 + (size_t)st * w_tile, p.wpk + tile * w_tile, w_tile, &w_full[st]);
+    }
+  }
+  if (warp == 8) return;
+  // -------------------------------------------------------------------- gather + MMA + epilogue (warps 0-7)
+  // A thread fetches TWO items (16 scalar or 4 vector loads in flight) before it converts either.
+  const int pid = tid;   // 0 .. 255
+  const int wg = warp >> 2, t = tid & 127;
     const float* xb = p.x + (long long)b * p.sxb;
     const float* x2b = p.x2 ? p.x2 + (long long)b * p.sx2b : nullptr;
     const int n_items = R * KC;
@@ -121,50 +122,86 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
       if (nparts == 2)
         *reinterpret_cast<uint4*>(Al + ((size_t)kc * R + r) * 16) = *reinterpret_cast<const uint4*>(lo);
     };
-    for (int cc = 0; cc < ncc; ++cc) {
-      const int buf = cc & 1;
-      if (cc >= 2) tc::mbar_wait(&a_empty[buf], (uint32_t)(((cc >> 1) - 1) & 1));
-      uint8_t* Ah = A0 + (size_t)buf * a_buf;
-      uint8_t* Al = Ah + a_part;
-      for (int it0 = pid; it0 < n_items; it0 += 512) {
-        const int it1 = it0 + 256;
-        float va[8], vb[8];
-        fetch(it0, cc, va);
-        if (it1 < n_items) fetch(it1, cc, vb);
-        put(it0, Ah, Al, va);
-        if (it1 < n_items) put(it1, Ah, Al, vb);
-      }
-      tc::fence_proxy_async_smem();
-      ct_arrive(&a_full[buf]);
+  auto gather = [&](int cc) {
+    uint8_t* Ah = A0 + (size_t)(cc & 1) * a_buf;
+    uint8_t* Al = Ah + a_part;
+    for (int it0 = pid; it0 < n_items; it0 += 512) {
+      const int it1 = it0 + 256;
+      float va[8], vb[8];
+      fetch(it0, cc, va);
+      if (it1 < n_items) fetch(it1, cc, vb);
+      put(it0, Ah, Al, va);
+      if (it1 < n_items) put(it1, Ah, Al, vb);
     }
+    tc::fence_proxy_async_smem();
+  };
+  const uint32_t a_base = tc::smem_u32(A0) + (uint32_t)wg * 64u * 16u, w_base = tc::smem_u32(W0);
+  const uint32_t lbo_a = (uint32_t)R * 16u, lbo_b = (uint32_t)BN * 16u;
+  const uint64_t ks_a = (2u * lbo_a) >> 4, ks_b = (2u * lbo_b) >> 4;
+  const int nk = p.kch / 16;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  gather(0);
+  int wi = 0;
+  for (int cc = 0; cc < ncc; ++cc) {
+    tc::named_sync(1, 256);                    // chunk cc gathered by both warpgroups; no MMA reads the other buffer
+    const uint32_t ah = a_base + (uint32_t)(cc & 1) * a_buf, al = ah + a_part;
+    for (int tap = 0; tap < p.K; ++tap) {
+      const uint32_t row_off = (uint32_t)(tap * p.dil) * 16u;
+      for (int part = 0; part < nparts; ++part, ++wi) {
+        const int st = wi % wst;
+        tc::mbar_wait(&w_full[st], (uint32_t)((wi / wst) & 1));
+        const uint64_t bd = tc::smem_desc(w_base + (uint32_t)st * w_tile, lbo_b);
+        const int n_a = (part == 0 && nparts == 2) ? 2 : 1;
+        tc::wg_fence();
+        for (int ap = 0; ap < n_a; ++ap) {
+          const uint64_t ad = tc::smem_desc((ap == 0 ? ah : al) + row_off, lbo_a);
+          for (int kk = 0; kk < nk; ++kk) tc::Wg<BN, 0>::ss(acc, ad + kk * ks_a, bd + kk * ks_b, 1u);
+        }
+        tc::wg_commit();
+        tc::wg_wait<1>();                      // the previous weight slot's MMAs are done: release it
+        if (wi > 0 && t == 0) tc::mbar_arrive(&w_empty[(wi - 1) % wst]);
+      }
+    }
+    if (cc + 1 < ncc) gather(cc + 1);          // overlaps the last MMAs of this chunk
+    tc::wg_wait<0>();
   }
-  if (warp < 4 || warp >= 6) {
-    // ---------------------------------------------------------------- epilogue: two groups of four warps
-    // (the A producers, now idle, and warps 6-9) take alternate 16-column strips.  A warp may only
-    // read the TMEM lane quarter warp%4, so warps 6..9 own quarters 2,3,0,1.
-    const int grp = warp < 4 ? 0 : 1, wq = warp & 3;
-    tc::mbar_wait(&bar_acc, 0);
-    tc::fence_after_sync();
-    const int t = t0 + wq * 32 + lane;
-    const bool gate = (p.flags & CONV_GATE) != 0;
-    const int cout_real = gate ? p.Cout / 2 : p.Cout;
-    const bool keep = !(p.flags & CONV_OUT_MASK) || t < len;
-    float* yb = p.y + (long long)b * cout_real * p.Tout;
-    const float* rb = p.res ? p.res + (long long)b * cout_real * p.Tout : nullptr;
+  tc::wg_hold(acc);
+  if (t == 0) tc::mbar_arrive(&w_empty[(wi - 1) % wst]);
+
+  // ---------------------------------------------------------------- epilogue: thread = (row t % 64, 32-column half)
+  float* strip = Strips + wg * 64 * CT_EPI_LD;
+  const int tq = t0 + wg * 64 + (t & 63);
+  const bool gate = (p.flags & CONV_GATE) != 0;
+  const int cout_real = gate ? p.Cout / 2 : p.Cout;
+  const bool keep = !(p.flags & CONV_OUT_MASK) || tq < len;
+  float* yb = p.y + (long long)b * cout_real * p.Tout;
+  const float* rb = p.res ? p.res + (long long)b * cout_real * p.Tout : nullptr;
+#pragma unroll 1
+  for (int ch = 0; ch < (BN + 63) / 64; ++ch) {
+    tc::named_sync(2 + wg, 128);
+    tc::acc_to_smem<BN>(acc, strip, CT_EPI_LD, 8 * ch, 8 * ch + 8);
+    tc::named_sync(2 + wg, 128);
+#pragma unroll 1
+    for (int sub = 0; sub < 2; ++sub) {
+      const int cl = (t >> 6) * 32 + sub * 16, c0 = ch * 64 + cl;
+      if (c0 >= BN) continue;
+      float vf[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) vf[j] = strip[(t & 63) * CT_EPI_LD + cl + j];
+      const int t = tq;
     if (p.ilv) {   // interleaved store: ilv consecutive samples of one channel per thread (one 8 / 16-byte store)
       float* yi = p.y + (long long)b * p.Cout * p.Tout;   // = [Cout / ilv][Tout * ilv]
-      for (int c0 = grp * 16; c0 < p.bn; c0 += 32) {
-        uint32_t v[16];
-        tc::tmem_ld16(tmem + ((uint32_t)(wq * 32) << 16) + (uint32_t)c0, v);
-        tc::tmem_ld_wait();
+      {
         if (t < p.Tout) {
 #pragma unroll
           for (int j = 0; j < 16; j += 4) {
-            const int cp = nt * p.bn + c0 + j;
+            const int cp = nt * BN + c0 + j;
             if (cp < p.Cout) {
               float o[4];
 #pragma unroll
-              for (int e = 0; e < 4; ++e) o[e] = ct_act(__uint_as_float(v[j + e]) + (p.bias ? __ldg(p.bias + cp + e) : 0.f), p.act);
+              for (int e = 0; e < 4; ++e) o[e] = ct_act(vf[j + e] + (p.bias ? __ldg(p.bias + cp + e) : 0.f), p.act);
               if (p.ilv == 4) {
                 *reinterpret_cast<float4*>(yi + ((long long)(cp >> 2) * p.Tout + t) * 4) = make_float4(o[0], o[1], o[2], o[3]);
               } else {
@@ -176,9 +213,7 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
         }
       }
     } else
-    for (int c0 = grp * 16; c0 < p.bn; c0 += 32) {
-      uint32_t v[16];
-      tc::tmem_ld16(tmem + ((uint32_t)(wq * 32) << 16) + (uint32_t)c0, v);
+    {
       const bool live = t < p.Tout;
       const int step = gate ? 2 : 1;
       // residual / accumulator loads of the strip first (all in flight), stores afterwards
@@ -186,7 +221,7 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         float a = 0.f;
-        const int cp = nt * p.bn + c0 + j;
+        const int cp = nt * BN + c0 + j;
         if (live && (j % step) == 0 && cp + (step - 1) < p.Cout) {
           const long long off = (long long)(gate ? (cp >> 1) : cp) * p.Tout + t;
           if (rb) a = rb[off];
@@ -194,15 +229,14 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
         }
         add[j] = a;
       }
-      tc::tmem_ld_wait();
       if (live) {
         if (gate) {
 #pragma unroll
           for (int j = 0; j < 16; j += 2) {
-            const int cp = nt * p.bn + c0 + j;
+            const int cp = nt * BN + c0 + j;
             if (cp + 1 < p.Cout) {
-              const float a = __uint_as_float(v[j]) + __ldg(p.bias + cp);
-              const float g = __uint_as_float(v[j + 1]) + __ldg(p.bias + cp + 1);
+              const float a = vf[j] + __ldg(p.bias + cp);
+              const float g = vf[j + 1] + __ldg(p.bias + cp + 1);
               float o = tanhf(a) * (1.f / (1.f + expf(-g)));
               if (!keep) o = 0.f;
               yb[(long long)(cp >> 1) * p.Tout + t] = o + add[j];
@@ -211,9 +245,9 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
         } else {
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            const int co = nt * p.bn + c0 + j;
+            const int co = nt * BN + c0 + j;
             if (co < p.Cout) {
-              float o = ct_act(__uint_as_float(v[j]) + (p.bias ? __ldg(p.bias + co) : 0.f), p.act);
+              float o = ct_act(vf[j] + (p.bias ? __ldg(p.bias + co) : 0.f), p.act);
               if (!keep) o = 0.f;
               yb[(long long)co * p.Tout + t] = o + add[j];
             }
@@ -221,72 +255,14 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
         }
       }
     }
-  } else if (tid == 128) {
-    // ---------------------------------------------------------------- W producer
-    const int total = ncc * p.K * nparts;
-    for (int i = 0; i < total; ++i) {
-      const int st = i % wst;
-      if (i >= wst) tc::mbar_wait(&w_empty[st], (uint32_t)(((i / wst) - 1) & 1));
-      const int part = i % nparts, tap = (i / nparts) % p.K, cc = i / (nparts * p.K);
-      const size_t tile = (((size_t)tap * ncc + cc) * 2 + part) * p.ntiles + nt;
-      tc::mbar_arrive_expect_tx(&w_full[st], w_tile);
-      tc::bulk_g2s(W0 + (size_t)st * w_tile, p.wpk + tile * w_tile, w_tile, &w_full[st]);
     }
-  } else if (warp_u == 5) {
-    // ---------------------------------------------------------------- MMA issuer (whole warp walks the
-    // uniform loop, one elected lane issues: tc::elect_one)
-    const uint32_t idesc = tc::idesc_bf16(CT_M, p.bn);
-    const uint32_t a_base = tc::smem_u32(A0), w_base = tc::smem_u32(W0);
-    const uint32_t lbo_a = (uint32_t)R * 16u, lbo_b = (uint32_t)p.bn * 16u;
-    const uint32_t kstep_a = (2u * lbo_a) >> 4, kstep_b = (2u * lbo_b) >> 4;
-    const int nk = p.kch / 16;
-    uint32_t accumulate = 0;
-    int wi = 0;
-    for (int cc = 0; cc < ncc; ++cc) {
-      const int buf = cc & 1;
-      tc::mbar_wait(&a_full[buf], (uint32_t)((cc >> 1) & 1));
-      tc::fence_after_sync();
-      const uint32_t ah = a_base + (uint32_t)buf * a_buf, al = ah + a_part;
-      for (int tap = 0; tap < p.K; ++tap) {
-        const uint32_t row_off = (uint32_t)(tap * p.dil) * 16u;
-        for (int part = 0; part < nparts; ++part, ++wi) {
-          const int st = wi % wst;
-          tc::mbar_wait(&w_full[st], (uint32_t)((wi / wst) & 1));
-          tc::fence_after_sync();
-          const uint64_t bd0 = tc::smem_desc(w_base + (uint32_t)st * w_tile, lbo_b);
-          const int n_a = (part == 0 && nparts == 2) ? 2 : 1;
-          if (tc::elect_one()) {
-            uint32_t acc_flag = accumulate;
-            const uint32_t b_hiw = (uint32_t)(bd0 >> 32);
-            for (int ap = 0; ap < n_a; ++ap) {
-              const uint64_t ad0 = tc::smem_desc((ap == 0 ? ah : al) + row_off, lbo_a);
-              const uint32_t a_hiw = (uint32_t)(ad0 >> 32);
-              uint32_t ad = (uint32_t)ad0, bd = (uint32_t)bd0;   // low words: only the start-address field moves
-              for (int kk = 0; kk < nk; ++kk) {
-                tc::mma_bf16_lohi(tmem, ad, a_hiw, bd, b_hiw, idesc, acc_flag);
-                acc_flag = 1;
-                ad += kstep_a;
-                bd += kstep_b;
-              }
-            }
-            tc::mma_commit(&w_empty[st]);
-          }
-          accumulate = 1;
-        }
-      }
-      if (tc::elect_one()) tc::mma_commit(&a_empty[buf]);
-    }
-    if (tc::elect_one()) tc::mma_commit(&bar_acc);
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 4) tc::tmem_dealloc(tmem, ncols);
 }
 
 static size_t conv_tc_smem_bytes(const ConvTcParams& p, int wst) {
   const int R = CT_M + (p.K - 1) * p.dil;
   const size_t a_buf = (size_t)(p.kch / 8) * R * 16 * (p.nsplit == 3 ? 2 : 1);
-  return 2 * a_buf + (size_t)wst * p.kch * p.bn * 2 + 128;
+  return 2 * a_buf + (size_t)wst * p.kch * p.bn * 2 + CT_STRIP_BYTES + 128;
 }
 
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
@@ -308,11 +284,9 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
   // a 2-deep weight ring when that lets two CTAs share an SM (one CTA's epilogue then overlaps the
   // other's gather + MMA; the 1x1 convolutions are epilogue-bound), else the 3-deep ring
   int wst = CT_WST;
-  if (conv_tc_smem_bytes(p, 2) <= 113 * 1024 && tc_cols(p.bn) <= 256) wst = 2;
+  if (conv_tc_smem_bytes(p, 2) <= 113 * 1024) wst = 2;
   const size_t smem = conv_tc_smem_bytes(p, wst);
   if (smem > 227 * 1024 - 512) { set_error("conv_tc: tile does not fit shared memory"); return SVCB_E_UNSUPPORTED; }
-  static DevSmemCache attr_cache;
-  SVCB_CUDA_CHECK(ensure_dyn_smem(conv_tc_kernel, smem, attr_cache));
   dim3 grid((p.Tout + CT_M - 1) / CT_M, p.ntiles, p.B);
   const int cout_real = (p.flags & CONV_GATE) ? p.Cout / 2 : p.Cout;
   char kname[64];
@@ -321,7 +295,18 @@ int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
                  2.0 * p.Cin * p.K * p.Cout * (double)p.Tout * p.B,
                  4.0 * ((double)p.B * p.Cin * p.Tin + (double)p.B * cout_real * p.Tout * (p.res ? 2 : 1)) +
                      2.0 * (double)p.Cin * p.K * p.Cout);
-  conv_tc_kernel<<<grid, 320, smem, s>>>(p, wst);
+  switch (p.bn / 16) {
+#define SVCB_CONV_BN(nb)                                                           \
+  case nb: {                                                                       \
+    static DevSmemCache attr_cache;                                                \
+    SVCB_CUDA_CHECK(ensure_dyn_smem(conv_tc_kernel<16 * nb>, smem, attr_cache));   \
+    conv_tc_kernel<16 * nb><<<grid, CT_THREADS, smem, s>>>(p, wst);                \
+    break;                                                                         \
+  }
+    SVCB_CONV_BN(1) SVCB_CONV_BN(2) SVCB_CONV_BN(3) SVCB_CONV_BN(4) SVCB_CONV_BN(5) SVCB_CONV_BN(6) SVCB_CONV_BN(7) SVCB_CONV_BN(8)
+    SVCB_CONV_BN(9) SVCB_CONV_BN(10) SVCB_CONV_BN(11) SVCB_CONV_BN(12) SVCB_CONV_BN(13) SVCB_CONV_BN(14) SVCB_CONV_BN(15) SVCB_CONV_BN(16)
+#undef SVCB_CONV_BN
+  }
   SVCB_LAUNCH_CHECK("conv_tc");
   return SVCB_OK;
 }

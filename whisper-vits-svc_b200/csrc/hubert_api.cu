@@ -5,12 +5,12 @@
 //   -> FeatureProjection (:98-109: LayerNorm(512) -> Linear(512,768)) -> x + GELU(pos_conv(x)[..., :-1]) (:112-128:
 //   Conv1d(768,768,128, pad 64, groups 16), weight_norm folded by the packer) -> LayerNorm(768) -> 12 x
 //   nn.TransformerEncoderLayer(768, 12, 3072, gelu, post-LN) (:131-153) -> Linear(768,256).
-// The transformer runs on the PPG extractor's kernels: tcgen05 GEMMs over bf16 tile images (whisper_gemm.cu), the
-// tcgen05 attention with P in tensor memory (whisper_attn_tc.cu: 12 heads of 64, scores / 8), `ln_rows` writing the
+// The transformer runs on the PPG extractor's kernels: wgmma GEMMs over bf16 tile images (whisper_gemm.cu), the
+// wgmma attention with P fed from registers (whisper_attn_tc.cu: 12 heads of 64, scores / 8), `ln_rows` writing the
 // normalised rows both as the next GEMM's A image and as the fp32 residual stream (post-LN).
 // Convolutional stem (97 GFLOP per 20 s chunk): conv0 (one input channel, 10 taps) + GroupNorm + GELU in fp32 as two
 // passes over the audio (statistics, then normalise-and-pack) that write conv1's im2col tile image directly; the six
-// stride-2 convs as tcgen05 GEMMs over such images — every GEMM's epilogue (6) applies GELU and scatters straight into the NEXT
+// stride-2 convs as wgmma GEMMs over such images — every GEMM's epilogue (6) applies GELU and scatters straight into the NEXT
 // conv's image, the last one writes the fp32 time-major rows LayerNorm reads.  flags bit 0 selects the all-fp32 stem
 // (`conv1d`, the last conv writing time-major rows through its output strides) for parity work.
 // Positional conv (Conv1d(768, 768, 128, groups 16): 9.4 GFLOP per 1000 frames): per group an im2col tile image
@@ -226,7 +226,7 @@ int svcb_hubert_create(const void* dev_blob, size_t blob_bytes, const svcb_tenso
   SVCB_CUDA_CHECK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   SVCB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) { set_error("libsvc_b200 is built for sm_100a only"); return SVCB_E_UNSUPPORTED; }
+  if (prop.major != 9 || prop.minor != 0) { set_error("libsvc_b200 is built for sm_90a only"); return SVCB_E_UNSUPPORTED; }
   svcb_hubert* h = new svcb_hubert();
   h->n_layer = n_layer;
   const char* blob = static_cast<const char*>(dev_blob);

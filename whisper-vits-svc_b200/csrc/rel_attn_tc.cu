@@ -1,24 +1,24 @@
-// Windowed relative-position self-attention of the prior encoder on the 5th-gen tensor cores.
+// Windowed relative-position self-attention of the prior encoder on the Hopper tensor cores.
 //
 // Replaces MultiHeadAttention.attention (vits/attentions.py:225-274, rel-pos helpers :294-347) in its banded
 // form, SURVEY.md §8a row a3:
 //   s_ij = (q_i/sqrt(d)) . k_j + [|j-i|<=w] (q_i/sqrt(d)) . Ek[j-i+w];  masked_fill(-1e4) where i or j >= len;
 //   p = softmax_j(s);  o_i = sum_j p_ij v_j + sum_{|r|<=w} p_{i,i+r} Ev[r+w]
 // (2 heads, d = 96, w = 4, T <= 2520).  Round 1 ran this on the fp32 FMA pipe at 18 TFLOP/s (8.1 ms per
-// 32 x 10 s step); the two contractions are dense and belong on tcgen05 with split bf16 operands
-// (a = a_hi + a_lo: a.b ~ a_hi.b_hi + a_lo.b_hi + a_hi.b_lo, fp32 accumulate in TMEM, error ~2^-16 relative).
+// 32 x 10 s step); the two contractions are dense and belong on wgmma with split bf16 operands
+// (a = a_hi + a_lo: a.b ~ a_hi.b_hi + a_lo.b_hi + a_hi.b_lo, fp32 accumulate, error ~2^-16 relative).
 //
 // Two kernels:
 //   rel_attn_pack   q (pre-scaled by 1/sqrt(d)), k, v of [B, 3H, T] -> bf16 hi/lo operand images in tile
 //                   order (one contiguous bulk copy per tile), K-major SWIZZLE_NONE panels of tc.cuh
-//   rel_attn_tc     one CTA = (item, head, 128 queries).  Two passes over the 64-key tiles:
-//                   pass 1  S = Q K^T (18 MMAs, N = 64) -> row max and row sum (4 softmax warps, one query row
-//                           per thread, S read from TMEM);
-//                   pass 2  S again, P = exp(S - m) / l written as the bf16 hi/lo A operand of O += P V
-//                           (12 MMAs, N = 96); no rescaling of O is ever needed.
+//   rel_attn_tc     one CTA = (item, head, 128 queries) = two warpgroups of 64 query rows and a producer warp.
+//                   Two passes over the 64-key tiles:
+//                   pass 1  S = Q K^T (18 MMAs, N = 64, accumulators in registers) -> row max and row sum;
+//                   pass 2  S again, P = exp(S - m) / l split to bf16 hi/lo in registers as the A operand of
+//                           O += P V (12 MMAs, N = 96); no rescaling of O is ever needed.
 //                   The relative-key logits q.Ek are ONE extra MMA group (N = 16) whose 9 values per row the
-//                   softmax thread adds on the band; the relative-value term is added to O in the epilogue
-//                   from the 9 band probabilities.  Scores never leave the SM.
+//                   softmax adds on the band; the relative-value term is added to O in the epilogue from the
+//                   9 band probabilities.  Scores never leave the SM.
 #include <cstdint>
 #include <cstdio>
 
@@ -32,14 +32,12 @@ constexpr int D = 96, KCD = D / 8, TQ = 128, TK = 64, NREL = 9, W = 4;
 constexpr uint32_t Q_PART = KCD * TQ * 16, Q_TILE = 2 * Q_PART;          // 49,152
 constexpr uint32_t K_PART = KCD * TK * 16, K_TILE = 2 * K_PART;          // 24,576
 constexpr uint32_t V_PART = (TK / 8) * D * 16, V_TILE = 2 * V_PART;      // 24,576
-constexpr uint32_t P_PART = (TK / 8) * TQ * 16, P_BYTES = 2 * P_PART;    // 32,768
 constexpr uint32_t E_PART = KCD * 16 * 16, E_BYTES = 2 * E_PART;         // 6,144 (Ek padded to 16 rows)
-constexpr uint32_t OFF_Q = 0, OFF_K = OFF_Q + Q_TILE, OFF_V = OFF_K + 2 * K_TILE, OFF_P = OFF_V + 2 * V_TILE,
-                   OFF_E = OFF_P + P_BYTES, OFF_QE = OFF_E + E_BYTES, OFF_PB = OFF_QE + TQ * 12 * 4,
-                   OFF_EV = OFF_PB + TQ * 12 * 4, OFF_ML = OFF_EV + NREL * D * 4, SMEM = OFF_ML + 2 * TQ * 2 * 4;
-constexpr uint32_t COL_S = 0, COL_QE = 128, COL_O = 160, TMEM_COLS = 256;
-constexpr int SM_WARPS = 8;          // softmax warps: two per TMEM lane quadrant, 32 of the 64 key columns each
-constexpr int THREADS = (SM_WARPS + 2) * 32;
+constexpr uint32_t OFF_Q = 0, OFF_K = OFF_Q + Q_TILE, OFF_V = OFF_K + 2 * K_TILE,
+                   OFF_E = OFF_V + 2 * V_TILE, OFF_QE = OFF_E + E_BYTES, OFF_PB = OFF_QE + TQ * 12 * 4,
+                   OFF_EV = OFF_PB + TQ * 12 * 4, SMEM = OFF_EV + NREL * D * 4;
+constexpr int SM_WARPS = 8;          // two warpgroups of 64 query rows
+constexpr int THREADS = (SM_WARPS + 1) * 32;
 }  // namespace ra
 
 size_t rel_attention_ws_bytes(int B, int heads, int T) {
@@ -114,13 +112,24 @@ rel_attn_pack_kernel(const float* __restrict__ qkv, uint8_t* __restrict__ qimg, 
 }
 
 // ------------------------------------------------------------------------------------------------ attention
-__device__ __forceinline__ void ra_mma3(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
-                                        uint32_t hiw, uint32_t idesc, int nk, uint32_t ksa, uint32_t ksb, uint32_t first_acc) {
-  // D (+)= A_hi B_hi + A_lo B_hi + A_hi B_lo over nk K-chunks of 16
-  uint32_t acc = first_acc;
-  for (int kk = 0; kk < nk; ++kk) { tc::mma_bf16_lohi(d_tmem, a_hi + kk * ksa, hiw, b_hi + kk * ksb, hiw, idesc, acc); acc = 1; }
-  for (int kk = 0; kk < nk; ++kk) tc::mma_bf16_lohi(d_tmem, a_lo + kk * ksa, hiw, b_hi + kk * ksb, hiw, idesc, 1u);
-  for (int kk = 0; kk < nk; ++kk) tc::mma_bf16_lohi(d_tmem, a_hi + kk * ksa, hiw, b_lo + kk * ksb, hiw, idesc, 1u);
+// D (+)= A_hi B_hi + A_lo B_hi + A_hi B_lo over nk K-chunks of 16 (A and B K-major panels)
+template <int N>
+__device__ __forceinline__ void ra_mma3(float (&d)[N / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, int nk,
+                                        uint64_t ksa, uint64_t ksb) {
+#pragma unroll 1
+  for (int kk = 0; kk < nk; ++kk) {
+    tc::Wg<N, 0>::ss(d, a_hi + kk * ksa, b_hi + kk * ksb, 1u);
+    tc::Wg<N, 0>::ss(d, a_lo + kk * ksa, b_hi + kk * ksb, 1u);
+    tc::Wg<N, 0>::ss(d, a_hi + kk * ksa, b_lo + kk * ksb, 1u);
+  }
+}
+
+__device__ __forceinline__ void ra_split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+  const float2 f = __bfloat1622float2(h2);
+  const __nv_bfloat162 l2 = __floats2bfloat162_rn(a - f.x, b - f.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h2);
+  lo = *reinterpret_cast<const uint32_t*>(&l2);
 }
 
 __global__ void __launch_bounds__(ra::THREADS, 1)
@@ -129,10 +138,8 @@ rel_attn_tc_kernel(const uint8_t* __restrict__ qimg, const uint8_t* __restrict__
                    float* __restrict__ out, int H, int heads, int T, int nq, int nk) {
   using namespace ra;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t q_full, qe_full, k_full[2], k_empty[2], v_full[2], v_empty[2], s_full[2], s_empty[2],
-      p_full, p_empty, o_full;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  __shared__ __align__(8) uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int warp_u = tc::warp_uniform_idx();
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int bh = b * heads + h;
@@ -154,21 +161,14 @@ rel_attn_tc_kernel(const uint8_t* __restrict__ qimg, const uint8_t* __restrict__
   for (int i = tid; i < NREL * D; i += THREADS) ev_s[i] = __ldg(ev + i);
   for (int i = tid; i < TQ * 12; i += THREADS) pb_s[i] = 0.f;
   if (tid == 0) {
-    tc::mbar_init(&q_full, 1); tc::mbar_init(&qe_full, 1); tc::mbar_init(&p_full, SM_WARPS * 32); tc::mbar_init(&p_empty, 1);
-    tc::mbar_init(&o_full, 1);
+    tc::mbar_init(&q_full, 1);
     for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&k_full[i], 1); tc::mbar_init(&k_empty[i], 1); tc::mbar_init(&v_full[i], 1); tc::mbar_init(&v_empty[i], 1);
-      tc::mbar_init(&s_full[i], 1); tc::mbar_init(&s_empty[i], SM_WARPS * 32);
+      tc::mbar_init(&k_full[i], 1); tc::mbar_init(&k_empty[i], 2); tc::mbar_init(&v_full[i], 1); tc::mbar_init(&v_empty[i], 2);
     }
     tc::fence_barrier_init();
   }
   tc::fence_proxy_async_smem();     // the Ek panels were written through the generic proxy
-  __syncwarp();
-  if (warp == SM_WARPS) tc::tmem_alloc(&tmem_slot, TMEM_COLS);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = tmem_slot;
   const int ntile = 2 * nk;          // key tiles visited: pass 1 then pass 2
 
   if (warp_u == SM_WARPS) {
@@ -189,172 +189,151 @@ rel_attn_tc_kernel(const uint8_t* __restrict__ qimg, const uint8_t* __restrict__
         }
       }
     }
-  } else if (warp_u == SM_WARPS + 1) {
-    // ------------------------------------------------------------------------------------ MMA issuer
-    const uint32_t sb = tc::smem_u32(smem);
-    const uint64_t dq = tc::smem_desc(sb + OFF_Q, TQ * 16);
-    const uint32_t hiw = (uint32_t)(dq >> 32);
-    const uint32_t q_hi = (uint32_t)dq, q_lo = (uint32_t)tc::smem_desc(sb + OFF_Q + Q_PART, TQ * 16);
-    const uint32_t e_hi = (uint32_t)tc::smem_desc(sb + OFF_E, 16 * 16), e_lo = (uint32_t)tc::smem_desc(sb + OFF_E + E_PART, 16 * 16);
-    const uint32_t p_hi = (uint32_t)tc::smem_desc(sb + OFF_P, TQ * 16), p_lo = (uint32_t)tc::smem_desc(sb + OFF_P + P_PART, TQ * 16);
-    constexpr uint32_t KS_Q = (2 * TQ * 16) >> 4, KS_K = (2 * TK * 16) >> 4, KS_E = (2 * 16 * 16) >> 4, KS_V = (2 * D * 16) >> 4;
-    constexpr uint32_t id_s = tc::idesc_bf16(TQ, TK), id_e = tc::idesc_bf16(TQ, 16), id_o = tc::idesc_bf16(TQ, D);
-    tc::mbar_wait_parked(&q_full, 0);
-    tc::fence_after_sync();
-    if (tc::elect_one()) {
-      ra_mma3(tmem + COL_QE, q_hi, q_lo, e_hi, e_lo, hiw, id_e, D / 16, KS_Q, KS_E, 0u);
-      tc::mma_commit(&qe_full);
-    }
-    for (int i = 0; i <= ntile; ++i) {
-      if (i < ntile) {   // S[i & 1] = Q K_i^T
-        const int buf = i & 1;
-        tc::mbar_wait_parked(&k_full[buf], (uint32_t)((i >> 1) & 1));
-        if (i >= 2) tc::mbar_wait_parked(&s_empty[buf], (uint32_t)(((i >> 1) - 1) & 1));
-        tc::fence_after_sync();
-        const uint32_t k_hi = (uint32_t)tc::smem_desc(sb + OFF_K + buf * K_TILE, TK * 16);
-        const uint32_t k_lo = (uint32_t)tc::smem_desc(sb + OFF_K + buf * K_TILE + K_PART, TK * 16);
-        if (tc::elect_one()) {
-          ra_mma3(tmem + COL_S + (uint32_t)buf * TK, q_hi, q_lo, k_hi, k_lo, hiw, id_s, D / 16, KS_Q, KS_K, 0u);
-          tc::mma_commit(&k_empty[buf]);
-          tc::mma_commit(&s_full[buf]);
-        }
-      }
-      if (i > nk) {      // O += P V of pass-2 tile kt = i - nk - 1 (its P was written while S of tile i was computed)
-        const int kt = i - nk - 1, vb = kt & 1;
-        tc::mbar_wait_parked(&p_full, (uint32_t)(kt & 1));
-        tc::mbar_wait_parked(&v_full[vb], (uint32_t)((kt >> 1) & 1));
-        tc::fence_after_sync();
-        const uint32_t v_hi = (uint32_t)tc::smem_desc(sb + OFF_V + vb * V_TILE, D * 16);
-        const uint32_t v_lo = (uint32_t)tc::smem_desc(sb + OFF_V + vb * V_TILE + V_PART, D * 16);
-        if (tc::elect_one()) {
-          ra_mma3(tmem + COL_O, p_hi, p_lo, v_hi, v_lo, hiw, id_o, TK / 16, KS_Q, KS_V, kt > 0 ? 1u : 0u);
-          tc::mma_commit(&p_empty);
-          tc::mma_commit(&v_empty[vb]);
-          if (kt == nk - 1) tc::mma_commit(&o_full);
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------------------------ softmax (warps 0-7)
-    // thread = (query row, half): warps w and w+4 share TMEM lane quadrant w & 3; half = 32 of the 64 key columns
-    const int row = tid & (TQ - 1), half = tid >> 7;
-    const int gi = qt * TQ + row;
-    const long long len = lengths ? lengths[b] : (long long)T;
-    const bool row_masked = gi >= len;
-    const uint32_t lane_base = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    float* ml_s = reinterpret_cast<float*>(smem + OFF_ML);   // [2 halves][128][m, l]
-    tc::mbar_wait_parked(&qe_full, 0);
-    tc::fence_after_sync();
-    if (half == 0) {
-      uint32_t u[16];
-      tc::tmem_ld16(lane_base + COL_QE, u);
-      tc::tmem_ld_wait();
+    return;
+  }
+  // ------------------------------------------------------------------------------------ two warpgroups of 64 rows
+  const int wg = warp >> 2, t = tid & 127, w = t >> 5, g = lane >> 2, c = lane & 3;
+  const uint32_t sb = tc::smem_u32(smem);
+  const uint32_t qrow = (uint32_t)wg * 64u * 16u;
+  const uint64_t q_hi = tc::smem_desc(sb + OFF_Q + qrow, TQ * 16), q_lo = tc::smem_desc(sb + OFF_Q + Q_PART + qrow, TQ * 16);
+  const uint64_t e_hi = tc::smem_desc(sb + OFF_E, 16 * 16), e_lo = tc::smem_desc(sb + OFF_E + E_PART, 16 * 16);
+  constexpr uint64_t KS_Q = (2 * TQ * 16) >> 4, KS_K = (2 * TK * 16) >> 4, KS_E = (2 * 16 * 16) >> 4, KS_V = (2 * D * 16) >> 4;
+  const long long len = lengths ? lengths[b] : (long long)T;
+  int lrow[2], gi[2];
+  bool row_masked[2];
 #pragma unroll
-      for (int r = 0; r < NREL; ++r) qe_s[row * 12 + r] = __uint_as_float(u[r]);
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");          // qe_s of the row is read by both halves
-    float m = -1e30f, l = 0.f, inv_l = 0.f;
-    for (int i = 0; i < ntile; ++i) {
-      const bool pass2 = i >= nk;
-      const int kt = pass2 ? i - nk : i, buf = i & 1;
-      if (i == nk) {   // combine the two halves' (max, sum) of pass 1
-        ml_s[(half * TQ + row) * 2] = m; ml_s[(half * TQ + row) * 2 + 1] = l;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        const float mo = ml_s[((half ^ 1) * TQ + row) * 2], lo_ = ml_s[((half ^ 1) * TQ + row) * 2 + 1];
-        const float mn = fmaxf(m, mo);
-        l = l * __expf(m - mn) + lo_ * __expf(mo - mn);
-        m = mn;
-        inv_l = 1.f / l;
-      }
-      tc::mbar_wait_parked(&s_full[buf], (uint32_t)((i >> 1) & 1));
-      tc::fence_after_sync();
-      const int j0 = kt * TK + half * 32;      // first key column of this thread's half
-      const int dlo = j0 - gi + W;             // band index of that column: r = dlo + jj
-      const bool band = dlo + 31 >= 0 && dlo < NREL;
-      uint32_t u[32];
-      tc::tmem_ld16(lane_base + COL_S + (uint32_t)(buf * TK + half * 32), reinterpret_cast<uint32_t(&)[16]>(u[0]));
-      tc::tmem_ld16(lane_base + COL_S + (uint32_t)(buf * TK + half * 32 + 16), reinterpret_cast<uint32_t(&)[16]>(u[16]));
-      tc::tmem_ld_wait();
-      float sc[32];
+  for (int hh = 0; hh < 2; ++hh) {
+    lrow[hh] = wg * 64 + 16 * w + g + 8 * hh;     // row of the CTA tile
+    gi[hh] = qt * TQ + lrow[hh];
+    row_masked[hh] = gi[hh] >= len;
+  }
+  tc::mbar_wait_parked(&q_full, 0);
+  {   // relative-key logits q_i . Ek[r], r < 9
+    float qe[8];
 #pragma unroll
-      for (int jj = 0; jj < 32; ++jj) {
-        const int j = j0 + jj;
-        float sv = __uint_as_float(u[jj]);
-        if (band) {
-          const int r = dlo + jj;
-          if ((unsigned)r < (unsigned)NREL) sv += qe_s[row * 12 + r];
+    for (int i = 0; i < 8; ++i) qe[i] = 0.f;
+    tc::wg_fence();
+    ra_mma3<16>(qe, q_hi, q_lo, e_hi, e_lo, D / 16, KS_Q, KS_E);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::wg_hold(qe);
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int col = 8 * i + 2 * c + (e & 1);
+        if (col < NREL) qe_s[lrow[e >> 1] * 12 + col] = qe[4 * i + e];
+      }
+    __syncwarp();                                           // a row's entries are read by the four threads that wrote them
+  }
+  float m[2] = {-1e30f, -1e30f}, l[2] = {0.f, 0.f}, inv_l[2] = {0.f, 0.f};
+  float o[48];
+#pragma unroll
+  for (int i = 0; i < 48; ++i) o[i] = 0.f;
+  for (int i = 0; i < ntile; ++i) {
+    const bool pass2 = i >= nk;
+    const int kt = pass2 ? i - nk : i, buf = i & 1;
+    if (i == nk) {   // combine the four threads' (max, sum) of each row
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int x = 1; x <= 2; x <<= 1) {
+          const float mo = __shfl_xor_sync(0xffffffffu, m[hh], x), lo_ = __shfl_xor_sync(0xffffffffu, l[hh], x);
+          const float mn = fmaxf(m[hh], mo);
+          l[hh] = l[hh] * __expf(m[hh] - mn) + lo_ * __expf(mo - mn);
+          m[hh] = mn;
         }
-        if (row_masked || j >= len) sv = -1e4f;
+        inv_l[hh] = 1.f / l[hh];
+      }
+    }
+    float sc[32];
+    {
+      tc::mbar_wait_parked(&k_full[buf], (uint32_t)((i >> 1) & 1));
+      const uint64_t k_hi = tc::smem_desc(sb + OFF_K + buf * K_TILE, TK * 16), k_lo = tc::smem_desc(sb + OFF_K + buf * K_TILE + K_PART, TK * 16);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) sc[j] = 0.f;
+      tc::wg_fence();
+      ra_mma3<64>(sc, q_hi, q_lo, k_hi, k_lo, D / 16, KS_Q, KS_K);
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_hold(sc);
+      if (t == 0) tc::mbar_arrive(&k_empty[buf]);
+    }
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int hh = e >> 1, j = kt * TK + 8 * q + 2 * c + (e & 1);
+        const int r = j - gi[hh] + W;
+        float sv = sc[4 * q + e];
+        if ((unsigned)r < (unsigned)NREL) sv += qe_s[lrow[hh] * 12 + r];
+        if (row_masked[hh] || j >= len) sv = -1e4f;
         if (j >= T) sv = -INFINITY;
-        sc[jj] = sv;
+        sc[4 * q + e] = sv;
       }
-      // the accumulator is in registers now: hand it back before the arithmetic
-      tc::fence_before_sync();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(&s_empty[buf])) : "memory");
-      if (!pass2) {
-        float mx = sc[0];
+    if (!pass2) {
 #pragma unroll
-        for (int jj = 1; jj < 32; ++jj) mx = fmaxf(mx, sc[jj]);
-        const float m_new = fmaxf(m, mx);
+      for (int hh = 0; hh < 2; ++hh) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) mx = fmaxf(mx, fmaxf(sc[4 * q + 2 * hh], sc[4 * q + 2 * hh + 1]));
+        const float m_new = fmaxf(m[hh], mx);
         float sum = 0.f;
 #pragma unroll
-        for (int jj = 0; jj < 32; ++jj) sum += __expf(sc[jj] - m_new);
-        l = l * __expf(m - m_new) + sum;
-        m = m_new;
-      } else {
-#pragma unroll
-        for (int jj = 0; jj < 32; ++jj) sc[jj] = __expf(sc[jj] - m) * inv_l;
-        if (band) {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) {
-            const int r = dlo + jj;
-            if ((unsigned)r < (unsigned)NREL) pb_s[row * 12 + r] = sc[jj];
-          }
-        }
-        if (kt >= 1) tc::mbar_wait_parked(&p_empty, (uint32_t)((kt - 1) & 1));   // P of tile kt-1 consumed by its MMAs
-#pragma unroll
-        for (int oc = 0; oc < 4; ++oc) {       // 4 octets of 8 keys = K-chunks of the P operand
-          float p8[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) p8[e] = sc[oc * 8 + e];
-          uint4 hi, lo;
-          ra_split8(p8, hi, lo);
-          const int kc = half * 4 + oc;
-          *reinterpret_cast<uint4*>(smem + OFF_P + (size_t)(kc * TQ + row) * 16) = hi;
-          *reinterpret_cast<uint4*>(smem + OFF_P + P_PART + (size_t)(kc * TQ + row) * 16) = lo;
-        }
-        tc::fence_proxy_async_smem();          // P panels: generic-proxy stores -> visible to the MMA (async proxy)
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(&p_full)) : "memory");
+        for (int q = 0; q < 8; ++q) sum += __expf(sc[4 * q + 2 * hh] - m_new) + __expf(sc[4 * q + 2 * hh + 1] - m_new);
+        l[hh] = l[hh] * __expf(m[hh] - m_new) + sum;
+        m[hh] = m_new;
       }
-    }
-    // epilogue: O (+ relative-value band) -> out[b, h*96 + c, t]; each half writes 48 of the 96 head dims
-    tc::mbar_wait_parked(&o_full, 0);
-    tc::fence_after_sync();
-    asm volatile("bar.sync 1, 256;" ::: "memory");          // pb_s entries were written by either half
-    float pb[NREL];
+    } else {
+      uint32_t ph[4][4], pl[4][4];
 #pragma unroll
-    for (int r = 0; r < NREL; ++r) pb[r] = pb_s[row * 12 + r];
-    float* ob = out + ((long long)b * H + (long long)h * D) * T + gi;
+      for (int q = 0; q < 8; ++q) {
 #pragma unroll
-    for (int cc = 0; cc < 3; ++cc) {
-      const int c0 = half * 48 + cc * 16;
-      uint32_t u[16];
-      tc::tmem_ld16(lane_base + COL_O + (uint32_t)c0, u);
-      tc::tmem_ld_wait();
-      if (gi < T) {
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          float o = __uint_as_float(u[c]);
-#pragma unroll
-          for (int r = 0; r < NREL; ++r) o = fmaf(pb[r], ev_s[r * D + c0 + c], o);
-          ob[(long long)(c0 + c) * T] = o;
+        for (int e = 0; e < 4; ++e) {
+          const int hh = e >> 1;
+          sc[4 * q + e] = __expf(sc[4 * q + e] - m[hh]) * inv_l[hh];
+          const int r = kt * TK + 8 * q + 2 * c + (e & 1) - gi[hh] + W;
+          if ((unsigned)r < (unsigned)NREL) pb_s[lrow[hh] * 12 + r] = sc[4 * q + e];
         }
+        ra_split2(sc[4 * q], sc[4 * q + 1], ph[q >> 1][(q & 1) * 2], pl[q >> 1][(q & 1) * 2]);
+        ra_split2(sc[4 * q + 2], sc[4 * q + 3], ph[q >> 1][(q & 1) * 2 + 1], pl[q >> 1][(q & 1) * 2 + 1]);
       }
+      const int vb = kt & 1;
+      tc::mbar_wait_parked(&v_full[vb], (uint32_t)((kt >> 1) & 1));
+      const uint64_t v_hi = tc::smem_desc(sb + OFF_V + vb * V_TILE, D * 16), v_lo = tc::smem_desc(sb + OFF_V + vb * V_TILE + V_PART, D * 16);
+      tc::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < TK / 16; ++kk) {
+        tc::Wg<96, 0>::rs(o, ph[kk], v_hi + kk * KS_V, 1u);
+        tc::Wg<96, 0>::rs(o, pl[kk], v_hi + kk * KS_V, 1u);
+        tc::Wg<96, 0>::rs(o, ph[kk], v_lo + kk * KS_V, 1u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_hold(o);
+      if (t == 0) tc::mbar_arrive(&v_empty[vb]);
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == ra::SM_WARPS) tc::tmem_dealloc(tmem, ra::TMEM_COLS);
+  // epilogue: O (+ relative-value band) -> out[b, h*96 + col, t]
+  __syncwarp();                                             // pb_s entries of a row were written by its four threads
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    if (gi[hh] >= T) continue;
+    float pb[NREL];
+#pragma unroll
+    for (int r = 0; r < NREL; ++r) pb[r] = pb_s[lrow[hh] * 12 + r];
+    float* ob = out + ((long long)b * H + (long long)h * D) * T + gi[hh];
+#pragma unroll
+    for (int q = 0; q < 12; ++q)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = 8 * q + 2 * c + e;
+        float v = o[4 * q + 2 * hh + e];
+#pragma unroll
+        for (int r = 0; r < NREL; ++r) v = fmaf(pb[r], ev_s[r * D + col], v);
+        ob[(long long)col * T] = v;
+      }
+  }
 }
 
 int launch_rel_attention_tc(const float* qkv, const float* ek, const float* ev, const long long* lengths, float* out,

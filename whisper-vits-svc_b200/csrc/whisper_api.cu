@@ -1,7 +1,7 @@
 // C ABI for the PPG extractor: truncated Whisper AudioEncoder (whisper/model.py:132-163 after the
 // loader's surgery, whisper/inference.py:11-29).  Stage pipeline:
 //   conv1+GELU (GEMM over an im2col image of the log-mel; its epilogue scatters into conv2's im2col image) ->
-//   conv2(stride 2)+GELU+pos-emb (GEMM) -> n_layer x { LN -> QKV GEMM (head-major panels) -> tcgen05 attention
+//   conv2(stride 2)+GELU+pos-emb (GEMM) -> n_layer x { LN -> QKV GEMM (head-major panels) -> wgmma attention
 //   (whisper_attn_tc.cu) -> out-proj GEMM (+residual) -> LN -> MLP GEMM+GELU -> MLP GEMM (+residual) } -> ln_post
 #include <algorithm>
 #include <cstring>
@@ -79,7 +79,7 @@ int svcb_whisper_create(const void* dev_blob, size_t blob_bytes, const svcb_tens
   SVCB_CUDA_CHECK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   SVCB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) { set_error("libsvc_b200 is built for sm_100a only"); return SVCB_E_UNSUPPORTED; }
+  if (prop.major != 9 || prop.minor != 0) { set_error("libsvc_b200 is built for sm_90a only"); return SVCB_E_UNSUPPORTED; }
   svcb_whisper* w = new svcb_whisper();
   w->cfg = c;
   const char* blob = static_cast<const char*>(dev_blob);

@@ -6,8 +6,8 @@
 // bf16 mma.sync (m16n8k16) tiles, fp32 online softmax; one CTA = 64 queries of one head, 4 warps x
 // 16 rows; K/V tiles of 64 keys double-buffered with cp.async in an XOR-swizzled layout that keeps
 // ldmatrix conflict-free.  Round 1's encoder ran this kernel (247 TFLOP/s); since round 2 the encoder and HuBERT use the
-// tcgen05 kernel of whisper_attn_tc.cu and this one only backs the unit-test entry point `svcb_op_attention_bf16`
-// (an independent implementation the tcgen05 kernel is also compared with).
+// wgmma kernel of whisper_attn_tc.cu and this one only backs the unit-test entry point `svcb_op_attention_bf16`
+// (an independent implementation the wgmma kernel is also compared with).
 #include "common.cuh"
 #include "tc.cuh"
 

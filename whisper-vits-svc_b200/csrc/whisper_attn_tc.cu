@@ -1,27 +1,19 @@
-// Whisper encoder self-attention on the 5th-gen tensor cores (head dim 64, no mask).
+// Whisper encoder self-attention on the Hopper tensor cores (head dim 64, no mask).
 //
 // Replaces MultiHeadAttention.qkv_attention (whisper/model.py:88-101): q, k scaled by d^-1/4 each
-// (= scores / 8), softmax in fp32, w @ v — SURVEY.md §8a row a15.  Round 1 ran this on `mma.sync`
-// (HMMA) at 247 TFLOP/s, 18 of the encoder's 43.7 ms; here both products are tcgen05.mma with the
-// accumulators in tensor memory.
+// (= scores / 8), softmax in fp32, w @ v — SURVEY.md §8a row a15.  Both products are wgmma.
 //
 // Operands come straight from the QKV GEMM, whose epilogue 4 writes the head-major layout of
 // common.cuh qkv_heads_off: per (item, q|k|v, head) the positions are tiled ([.][8 octets][128 or 64 rows][8]
-// bf16, items padded to 128 positions), so every operand tile is one contiguous SWIZZLE_NONE panel and one
-// bulk copy (a first version read the flat [M/128][3D/64] tile image with 16 copies of <= 1 KB per tile: the
-// producer's issue rate, ~800 cycles per tile, bounded the kernel).
+// bf16, items padded to 128 positions), so every operand tile is one contiguous no-swizzle panel and one
+// bulk copy.
 //   S = Q K^T   A = Q panel [8][128][8] (shared memory), B = K tile [8][64 keys][8]   (K-major, 4 MMAs of K = 16)
-//   O += P V    A = P, bf16, written by the softmax warps into TENSOR MEMORY over the score columns it came
-//               from (lane = query, 32-bit column = two keys), B = V tile [8 d-octets][64 keys][8] read as an
-//               MN-major operand (no transpose pass)
-// One CTA = (item, head, 128 queries): 4 softmax warps (thread = query row), a producer warp (one 8 KB bulk copy
-// per K / V tile into a 4-slot ring) and an MMA warp; 128 TMEM columns (S / P 64, O 64), 48 KB of shared memory
-// and 192 threads, so FOUR CTAs share an SM and hide each other's MMA -> softmax -> MMA latency chain.
-// ONE pass over the keys: online softmax with a lazy reference maximum — the reference only moves when the tile
-// maximum exceeds it by more than 2^8 (then the O row in tensor memory and the running sum are rescaled), so
-// every score costs one exponential; the MUFU unit (16 / clock / SM) is the floor.  Scores and O are single-
-// buffered: tcgen05.mma executes in issue order, so S_{i+1} is issued right behind P_i V_i, and when a softmax
-// thread sees S_{i+1} complete no MMA is in flight on its O row.
+//   O += P V    A = P, bf16, straight from the S accumulator registers (the m64nN accumulator fragment is the
+//               m64k16 A fragment), B = V tile [8 d-octets][64 keys][8] read as an MN-major operand (no
+//               transpose pass): 8 keys x 16 B = one core matrix, key groups 128 B apart (LBO), d-octets
+//               TK * 16 B apart (SBO)
+// One CTA = (item, head, 128 queries): two warpgroups of 64 query rows (online softmax over the 64-key tiles,
+// four threads per row) and a producer warp (one 8 KB bulk copy per K / V tile into a 4-slot ring).
 // The output is written as the tile image the out-projection consumes.
 #include <cstdint>
 
@@ -35,43 +27,26 @@ constexpr int D = 64, TQ = 128, TK = 64, NS = 4;
 constexpr uint32_t Q_BYTES = (D / 8) * TQ * 16;    // 16,384
 constexpr uint32_t T_BYTES = (D / 8) * TK * 16;    //  8,192  (one ring slot: a K or a V tile)
 constexpr uint32_t OFF_Q = 0, OFF_R = OFF_Q + Q_BYTES, SMEM = OFF_R + NS * T_BYTES;
-constexpr uint32_t COL_S = 0, COL_O = 64, TMEM_COLS = 128;
-constexpr int SM_WARPS = 4, THREADS = (SM_WARPS + 2) * 32;
-constexpr int CTAS_PER_SM = 4;
-constexpr float LAZY = 8.f;                        // log2 of the largest p the reference maximum may lag by
-static_assert(CTAS_PER_SM * (SMEM + 1024 + 256) <= 228 * 1024, "four CTAs must share an SM");
+constexpr int THREADS = 288;
+constexpr int CTAS_PER_SM = 2;
 }  // namespace wa
 
-// kind::f16, bf16 A (K-major) x bf16 B (MN-major when b_mn), fp32 D
-__host__ __device__ constexpr uint32_t wa_idesc(int M, int N, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (b_mn ? (1u << 16) : 0u) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ uint64_t wa_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
 __device__ __forceinline__ float wa_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+__device__ __forceinline__ uint32_t wa_pack(float a, float b) {
+  const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h2);
+}
 
 __global__ void __launch_bounds__(wa::THREADS, wa::CTAS_PER_SM)
 whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out_img, int T, int Dm,
-                       int vswap, long long* trace) {
+                       int vswap) {
   using namespace wa;
-  const bool tr = trace != nullptr && blockIdx.x == 3 && blockIdx.y == 7 && blockIdx.z == (gridDim.z >> 1);
-#define WA_T0 const unsigned t0_ = tr ? (unsigned)clock() : 0u
-#define WA_T1(slot) if (tr) acc_[slot] += (unsigned)clock() - t0_
-  unsigned acc_[4] = {0, 0, 0, 0};
-  const unsigned tstart_ = tr ? (unsigned)clock() : 0u;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t q_full, r_full[NS], r_empty[NS], s_full, p_full, o_full;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t q_full, r_full[NS], r_empty[NS];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int warp_u = tc::warp_uniform_idx();
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
@@ -79,18 +54,13 @@ whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __r
   const int nk = (T + TK - 1) / TK;
   const int m_item = b * T;                       // first flat row of the item
   if (tid == 0) {
-    tc::mbar_init(&q_full, 1); tc::mbar_init(&o_full, 1); tc::mbar_init(&s_full, 1); tc::mbar_init(&p_full, SM_WARPS * 32);
-    for (int i = 0; i < NS; ++i) { tc::mbar_init(&r_full[i], 1); tc::mbar_init(&r_empty[i], 1); }
+    tc::mbar_init(&q_full, 1);
+    for (int i = 0; i < NS; ++i) { tc::mbar_init(&r_full[i], 1); tc::mbar_init(&r_empty[i], 2); }
     tc::fence_barrier_init();
   }
-  __syncwarp();
-  if (warp == SM_WARPS) tc::tmem_alloc(&tmem_slot, TMEM_COLS);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = tmem_slot;
 
-  if (warp_u == SM_WARPS) {
+  if (warp_u == 8) {
     // ---------------------------------------------------------------- producer: ring order K_0 V_0 K_1 V_1 ..
     if (tc::elect_one()) {
       const __nv_bfloat16* qb = qkv + qkv_heads_off(b, 0, h, 0, 0, heads, Tp);
@@ -108,153 +78,91 @@ whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __r
         if (++slot == NS) { slot = 0; ph ^= 1u; }
       }
     }
-  } else if (warp_u == SM_WARPS + 1) {
-    // ------------------------------------------------------------------------------------ MMA issuer
-    const uint32_t sb = tc::smem_u32(smem);
-    const uint64_t dq = wa_desc(sb + OFF_Q, TQ * 16, 128);
-    const uint32_t hiw = (uint32_t)(dq >> 32);     // SBO = 128 B: shared by the Q and K descriptors
-    const uint32_t q_lo = (uint32_t)dq;
-    constexpr uint32_t KS_Q = (2 * TQ * 16) >> 4, KS_K = (2 * TK * 16) >> 4;   // K = 16 steps of the Q panel, a K tile
-    constexpr uint32_t id_s = wa_idesc(TQ, TK, false), id_o = wa_idesc(TQ, D, true);
-    // V tile [8 d-octets][64 keys][8 d] as the MN-major B operand of O += P V: 8 keys x 16 B = one core matrix;
-    // groups of 8 keys 128 B apart (LBO), d-octets TK * 16 B apart (SBO)
-    const uint32_t v_lbo = vswap ? TK * 16 : 128, v_sbo = vswap ? 128 : TK * 16;
-    const uint32_t vhw = (uint32_t)(wa_desc(0, v_lbo, v_sbo) >> 32);   // the low word carries address and LBO
-    tc::mbar_wait_parked(&q_full, 0);
-    for (int kt = 0; kt < nk; ++kt) {
-      {   // S = Q K_kt^T  (issued right behind P_{kt-1} V_{kt-1}, which reads the columns it overwrites)
-        const int n = 2 * kt, slot = n % NS;
-        { WA_T0; tc::mbar_wait_parked(&r_full[slot], (uint32_t)((n / NS) & 1)); WA_T1(0); }
-        tc::fence_after_sync();
-        const uint32_t k_lo = (uint32_t)wa_desc(sb + OFF_R + slot * T_BYTES, TK * 16, 128);
-        if (tc::elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk)
-            tc::mma_bf16_lohi(tmem + COL_S, q_lo + kk * KS_Q, hiw, k_lo + kk * KS_K, hiw, id_s, kk ? 1u : 0u);
-          tc::mma_commit(&r_empty[slot]);
-          tc::mma_commit(&s_full);
-        }
-        __syncwarp();
-      }
-      {   // O += P_kt V_kt, P from tensor memory: keys 0-31 in columns 0-15, keys 32-63 in columns 32-47
-        const int n = 2 * kt + 1, slot = n % NS;
-        { WA_T0; tc::mbar_wait_parked(&p_full, (uint32_t)(kt & 1)); WA_T1(1); }
-        { WA_T0; tc::mbar_wait_parked(&r_full[slot], (uint32_t)((n / NS) & 1)); WA_T1(2); }
-        tc::fence_after_sync();
-        const uint32_t v_lo = (uint32_t)wa_desc(sb + OFF_R + slot * T_BYTES, v_lbo, v_sbo);
-        if (tc::elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < TK / 16; ++kk)   // 16 keys per MMA: 8 columns of P, two key groups = 256 B of the V tile
-            tc::mma_bf16_ts(tmem + COL_O, tmem + COL_S + (uint32_t)((kk >> 1) * 32 + (kk & 1) * 8), v_lo + kk * 16u, vhw, id_o,
-                            (kt > 0 || kk > 0) ? 1u : 0u);
-          tc::mma_commit(&r_empty[slot]);
-          if (kt == nk - 1) tc::mma_commit(&o_full);
-        }
-        __syncwarp();
-      }
-    }
-    if (tr && lane == 0) { for (int j = 0; j < 3; ++j) trace[8 + j] = acc_[j]; trace[13] = (unsigned)clock() - tstart_; }
-  } else {
-    // ------------------------------------------------------------------------------------ softmax (warps 0-3)
-    const int row = tid;                          // query row = TMEM lane
-    const int ti = qt * TQ + row;                 // position inside the item
-    const uint32_t lane_base = tmem + ((uint32_t)(warp * 32) << 16);
-    constexpr float kC = 0.125f * 1.4426950408889634f;   // d^-1/4 on q and on k, and log2(e)
-    float mref = -INFINITY;                        // reference maximum (log2 domain): p = 2^(s kC - mref) <= 2^LAZY
-    float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-    for (int kt = 0; kt < nk; ++kt) {
-      { WA_T0; tc::mbar_wait_parked(&s_full, (uint32_t)(kt & 1)); WA_T1(0); }
-      tc::fence_after_sync();
-      const unsigned tc0_ = tr ? (unsigned)clock() : 0u;
-      const int nvalid = T - kt * TK;              // >= 64 except in the item's last tile
-      // tile maximum of this row (the scores are read again below: 32 live registers instead of 64)
-      float a0 = -INFINITY, a1 = -INFINITY, a2 = -INFINITY, a3 = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t u[32];
-        tc::tmem_ld16(lane_base + COL_S + (uint32_t)(c * 32), reinterpret_cast<uint32_t(&)[16]>(u[0]));
-        tc::tmem_ld16(lane_base + COL_S + (uint32_t)(c * 32 + 16), reinterpret_cast<uint32_t(&)[16]>(u[16]));
-        tc::tmem_ld_wait();
-        if (nvalid - c * 32 >= 32) {
-#pragma unroll
-          for (int jj = 0; jj < 32; jj += 4) {
-            a0 = fmaxf(a0, __uint_as_float(u[jj])); a1 = fmaxf(a1, __uint_as_float(u[jj + 1]));
-            a2 = fmaxf(a2, __uint_as_float(u[jj + 2])); a3 = fmaxf(a3, __uint_as_float(u[jj + 3]));
-          }
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) a0 = fmaxf(a0, c * 32 + jj < nvalid ? __uint_as_float(u[jj]) : -INFINITY);
-        }
-      }
-      const float tmax = fmaxf(fmaxf(a0, a1), fmaxf(a2, a3)) * kC;
-      const bool move = tmax > mref + LAZY;
-      if (__any_sync(0xffffffffu, move)) {   // tcgen05.ld / st are warp-collective: the whole warp rescales, by 1 where !move
-        const float alpha = move ? wa_ex2(mref - tmax) : 1.f;
-        if (move) { mref = tmax; l0 *= alpha; l1 *= alpha; l2 *= alpha; l3 *= alpha; }
-        if (kt > 0) {   // no MMA is in flight on O here (see the file header); tile 0 finds O unwritten
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[16];
-            tc::tmem_ld16(lane_base + COL_O + (uint32_t)(c * 16), o);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-            tc::tmem_st16(lane_base + COL_O + (uint32_t)(c * 16), o);
-          }
-        }
-        if (tr) acc_[3] += 1;
-      }
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t u[32];
-        tc::tmem_ld16(lane_base + COL_S + (uint32_t)(c * 32), reinterpret_cast<uint32_t(&)[16]>(u[0]));
-        tc::tmem_ld16(lane_base + COL_S + (uint32_t)(c * 32 + 16), reinterpret_cast<uint32_t(&)[16]>(u[16]));
-        tc::tmem_ld_wait();
-        uint32_t pk[16];   // P over this chunk's own score columns: 32 bf16 = 16 columns at c * 32
-        const int nv = nvalid - c * 32;
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          float p0 = wa_ex2(fmaf(__uint_as_float(u[2 * e]), kC, -mref)), p1 = wa_ex2(fmaf(__uint_as_float(u[2 * e + 1]), kC, -mref));
-          if (nv < 32) { p0 = 2 * e < nv ? p0 : 0.f; p1 = 2 * e + 1 < nv ? p1 : 0.f; }
-          if (e & 1) { l2 += p0; l3 += p1; } else { l0 += p0; l1 += p1; }
-          const __nv_bfloat162 h2 = __floats2bfloat162_rn(p0, p1);
-          pk[e] = *reinterpret_cast<const uint32_t*>(&h2);
-        }
-        tc::tmem_st16(lane_base + COL_S + (uint32_t)(c * 32), pk);
-      }
-      tc::tmem_st_wait();
-      tc::fence_before_sync();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(&p_full)) : "memory");
-      if (tr) acc_[1] += (unsigned)clock() - tc0_;
-    }
-    // epilogue: O / sum(p) -> bf16, written as the A tile image of the out-projection ([M/128][D/64][8][128][8])
-    const float inv_l = 1.f / ((l0 + l1) + (l2 + l3));
-    tc::mbar_wait_parked(&o_full, 0);
-    tc::fence_after_sync();
-    const int mrow = m_item + ti;
-    __nv_bfloat16* dst = out_img + ((size_t)(mrow >> 7) * heads + h) * 8192 + (size_t)(mrow & 127) * 8;
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t u[32];
-      tc::tmem_ld16(lane_base + COL_O + (uint32_t)(c * 32), reinterpret_cast<uint32_t(&)[16]>(u[0]));
-      tc::tmem_ld16(lane_base + COL_O + (uint32_t)(c * 32 + 16), reinterpret_cast<uint32_t(&)[16]>(u[16]));
-      tc::tmem_ld_wait();
-      if (ti < T) {
-#pragma unroll
-        for (int oc = 0; oc < 4; ++oc) {
-          __align__(16) __nv_bfloat162 h2[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            h2[e] = __floats2bfloat162_rn(__uint_as_float(u[oc * 8 + 2 * e]) * inv_l, __uint_as_float(u[oc * 8 + 2 * e + 1]) * inv_l);
-          *reinterpret_cast<uint4*>(dst + (size_t)(c * 4 + oc) * 1024) = *reinterpret_cast<const uint4*>(h2);
-        }
-      }
-    }
-    if (tr && tid == 0) { for (int j = 0; j < 4; ++j) trace[j] = acc_[j]; trace[6] = (unsigned)clock() - tstart_; }
+    return;
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == wa::SM_WARPS) tc::tmem_dealloc(tmem, wa::TMEM_COLS);
+  // ------------------------------------------------------------------ two warpgroups of 64 query rows
+  const int wg = warp >> 2, t = tid & 127, w = t >> 5, g = lane >> 2, c = lane & 3;
+  const uint32_t sb = tc::smem_u32(smem);
+  const uint64_t dq = tc::smem_desc(sb + OFF_Q + (uint32_t)wg * 64u * 16u, TQ * 16);
+  constexpr uint64_t KS_Q = (2 * TQ * 16) >> 4, KS_K = (2 * TK * 16) >> 4;
+  // V as the MN-major B operand: LBO between 8-key groups, SBO between d-octets (vswap exchanges them)
+  const uint32_t v_lbo = vswap ? TK * 16 : 128, v_sbo = vswap ? 128 : TK * 16;
+  constexpr float kC = 0.125f * 1.4426950408889634f;   // d^-1/4 on q and on k, and log2(e)
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows g and g + 8 of this warp's 16
+  tc::mbar_wait_parked(&q_full, 0);
+  for (int kt = 0; kt < nk; ++kt) {
+    float sc[32];
+    {   // S = Q K_kt^T
+      const int n = 2 * kt, slot = n % NS;
+      tc::mbar_wait_parked(&r_full[slot], (uint32_t)((n / NS) & 1));
+      const uint64_t dk = tc::smem_desc(sb + OFF_R + slot * T_BYTES, TK * 16);
+      tc::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < D / 16; ++kk) tc::Wg<64, 0>::ss(sc, dq + kk * KS_Q, dk + kk * KS_K, kk ? 1u : 0u);
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_hold(sc);
+      if (t == 0) tc::mbar_arrive(&r_empty[slot]);
+    }
+    const int nvalid = T - kt * TK;              // >= 64 except in the item's last tile
+    if (nvalid < TK) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (8 * i + 2 * c + (e & 1) >= nvalid) sc[4 * i + e] = -INFINITY;
+    }
+    float a0 = -INFINITY, a1 = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { a0 = fmaxf(a0, fmaxf(sc[4 * i], sc[4 * i + 1])); a1 = fmaxf(a1, fmaxf(sc[4 * i + 2], sc[4 * i + 3])); }
+    a0 = fmaxf(a0, __shfl_xor_sync(0xffffffffu, a0, 1)); a0 = fmaxf(a0, __shfl_xor_sync(0xffffffffu, a0, 2));
+    a1 = fmaxf(a1, __shfl_xor_sync(0xffffffffu, a1, 1)); a1 = fmaxf(a1, __shfl_xor_sync(0xffffffffu, a1, 2));
+    const float n0 = fmaxf(m0, a0 * kC), n1 = fmaxf(m1, a1 * kC);
+    const float al0 = wa_ex2(m0 - n0), al1 = wa_ex2(m1 - n1);
+    m0 = n0; m1 = n1; l0 *= al0; l1 *= al1;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { o[4 * i] *= al0; o[4 * i + 1] *= al0; o[4 * i + 2] *= al1; o[4 * i + 3] *= al1; }
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float p0 = wa_ex2(fmaf(sc[4 * i], kC, -m0)), p1 = wa_ex2(fmaf(sc[4 * i + 1], kC, -m0));
+      const float p2 = wa_ex2(fmaf(sc[4 * i + 2], kC, -m1)), p3 = wa_ex2(fmaf(sc[4 * i + 3], kC, -m1));
+      l0 += p0 + p1; l1 += p2 + p3;
+      pa[i >> 1][(i & 1) * 2] = wa_pack(p0, p1);
+      pa[i >> 1][(i & 1) * 2 + 1] = wa_pack(p2, p3);
+    }
+    {   // O += P_kt V_kt
+      const int n = 2 * kt + 1, slot = n % NS;
+      tc::mbar_wait_parked(&r_full[slot], (uint32_t)((n / NS) & 1));
+      const uint64_t dv = tc::smem_desc(sb + OFF_R + slot * T_BYTES, v_lbo, v_sbo);
+      tc::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < TK / 16; ++kk) tc::Wg<64, 1>::rs(o, pa[kk], dv + (uint64_t)kk * 16u, 1u);   // 16 keys = 256 B
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_hold(o);
+      if (t == 0) tc::mbar_arrive(&r_empty[slot]);
+    }
+  }
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float i0 = 1.f / l0, i1 = 1.f / l1;
+  // O / sum(p) -> bf16, written as the A tile image of the out-projection ([M/128][D/64][8][128][8])
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int ti = qt * TQ + wg * 64 + 16 * w + g + 8 * half;
+    if (ti < T) {
+      const int mrow = m_item + ti;
+      __nv_bfloat16* dst = out_img + ((size_t)(mrow >> 7) * heads + h) * 8192 + (size_t)(mrow & 127) * 8 + 2 * c;
+      const float inv = half ? i1 : i0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        *reinterpret_cast<uint32_t*>(dst + (size_t)i * 1024) = wa_pack(o[4 * i + 2 * half] * inv, o[4 * i + 2 * half + 1] * inv);
+    }
+  }
 }
 
 // qkv: head-major layout of common.cuh (B x 3 x heads blocks of Tp x 64, pad rows finite);
@@ -267,7 +175,7 @@ int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T
   SVCB_CUDA_CHECK(ensure_dyn_smem(whisper_attn_tc_kernel, wa::SMEM, attr_cache));
   KernelScope ks("whisper_attn_tc", s, 4.0 * B * (double)T * T * D, 2.0 * 4 * B * (double)T * D);
   whisper_attn_tc_kernel<<<dim3((T + wa::TQ - 1) / wa::TQ, heads, B), wa::THREADS, wa::SMEM, s>>>(
-      static_cast<const __nv_bfloat16*>(qkv_img), static_cast<__nv_bfloat16*>(out_img), T, D, vswap, s2d_get_trace());
+      static_cast<const __nv_bfloat16*>(qkv_img), static_cast<__nv_bfloat16*>(out_img), T, D, vswap);
   SVCB_LAUNCH_CHECK("whisper_attn_tc");
   return SVCB_OK;
 }

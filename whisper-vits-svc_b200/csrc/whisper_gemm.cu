@@ -1,4 +1,4 @@
-// Dense bf16 GEMM on tcgen05/TMEM for the Whisper encoder's linear layers, with fused epilogues.
+// Dense bf16 GEMM on wgmma for the Whisper encoder's linear layers, with fused epilogues.
 //
 //   C[M,N] = A[M,K] . W[N,K]^T + bias        replaces the F.linear calls of whisper/model.py:66-82
 //                                            (query/key/value/out) and :116 (Linear -> GELU -> Linear)
@@ -8,14 +8,14 @@
 // (packed by the host) are stored tile by tile — [row-tile][k-tile] blocks of 128 (or BN) rows x 64
 // k, each block already in the K-major panel order of tc.cuh ([k/8][row][8]).  A k-tile of either
 // operand is therefore ONE contiguous bulk copy (TMA engine) signalled on an mbarrier: no tensor
-// maps, no swizzle bookkeeping, no LSU traffic (a first version gathered 16-byte chunks with
-// cp.async from row-major operands and reached 199 TFLOP/s; profiles/r01_notes.md).
+// maps, no swizzle bookkeeping, no LSU traffic.
 //
-// Persistent CTAs walk (m-tile, n-tile) pairs; three roles pipeline across tiles:
-//   producer thread   4-deep ring of (A 16 KB + W BN*128 B) k-tiles
-//   MMA thread        tcgen05.mma M=128, N=BN, K=16 x4 per k-tile into TMEM accumulator (tile & 1)
-//   8 epilogue warps  previous tile: tcgen05.ld -> bias / GELU / residual -> stores (row-major bf16,
-//                     tile-image bf16 for the next GEMM, or fp32 residual stream)
+// Persistent CTAs walk (m-tile, n-tile) pairs:
+//   producer thread   3-deep ring of (A 16 KB + W BN*128 B) k-tiles, running ahead across tiles
+//   2 warpgroups      64 rows each: wgmma m64nBNk16 x4 per k-tile into register accumulators, then the
+//                     epilogue through a per-warpgroup shared-memory strip (64 columns at a time):
+//                     bias / GELU / residual -> stores (row-major bf16, tile-image bf16 for the next
+//                     GEMM, or fp32 residual stream)
 #include <algorithm>
 
 #include "common.cuh"
@@ -38,7 +38,9 @@ namespace svcb {
 enum GemmEpi : int { EPI_BF16_ROWMAJOR = 0, EPI_GELU_BF16_IMAGE = 1, EPI_RESID_F32 = 2, EPI_GELU_ADD_F32 = 3, EPI_QKV_HEADS = 4,
                      EPI_GELU_CONV2_IMG = 5, EPI_GELU_VALID_S2_IMG = 6, EPI_GELU_ADD_F32_LD = 7 };
 
-constexpr int GM_BM = 128, GM_BK = 64, GM_STAGES = 4;
+constexpr int GM_BM = 128, GM_BK = 64, GM_STAGES = 3;
+constexpr int GM_EPI_LD = 72;   // floats per row of an epilogue strip (64 columns + 8: conflict-free fragment stores)
+constexpr int GM_THREADS = 288;
 
 // element offset of (m, k) inside a tile image with KT k-tiles per row-tile
 __host__ __device__ inline size_t img_off(int m, int k, int KT) {
@@ -46,28 +48,21 @@ __host__ __device__ inline size_t img_off(int m, int k, int KT) {
 }
 
 template <int BN, int EPI>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(GM_THREADS, 1)
 gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __restrict__ Wimg,
                const float* __restrict__ bias, void* out, const float* res, int M, int N, int K, int res_mod, int aux) {
   constexpr uint32_t A_BYTES = GM_BM * GM_BK * 2, B_BYTES = BN * GM_BK * 2, ST_BYTES = A_BYTES + B_BYTES;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_full[GM_STAGES], bar_empty[GM_STAGES], t_full[2], t_empty[2];
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  __shared__ __align__(8) uint64_t bar_full[GM_STAGES], bar_empty[GM_STAGES];
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int KT = K / GM_BK, NT = N / BN, MT = (M + GM_BM - 1) / GM_BM;
   const int ntiles = MT * NT;
 
   if (tid == 0) {
-    for (int s = 0; s < GM_STAGES; ++s) { tc::mbar_init(&bar_full[s], 1); tc::mbar_init(&bar_empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&t_full[i], 1); tc::mbar_init(&t_empty[i], 256); }
+    for (int s = 0; s < GM_STAGES; ++s) { tc::mbar_init(&bar_full[s], 1); tc::mbar_init(&bar_empty[s], 2); }
     tc::fence_barrier_init();
   }
-  __syncwarp();
-  if (warp == 8) tc::tmem_alloc(&tmem_slot, 2 * BN <= 256 ? 256 : 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = tmem_slot;
 
   if (tid == 256) {
     // ------------------------------------------------------------------ producer
@@ -85,62 +80,66 @@ gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __re
         tc::bulk_g2s(As + A_BYTES, w_src + (size_t)kt * (BN * GM_BK), B_BYTES, &bar_full[st]);
       }
     }
-  } else if (tid == 288) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = tc::idesc_bf16(GM_BM, BN);
+  } else if (warp < 8) {
+    // ------------------------------------------------------------------ MMA + epilogue (warpgroup wg: rows 64 wg ..)
+    const int wg = warp >> 2, t = tid & 127;
+    float* strip = reinterpret_cast<float*>(smem + (size_t)GM_STAGES * ST_BYTES) + wg * 64 * GM_EPI_LD;
     const uint32_t s0 = tc::smem_u32(smem);
     const uint32_t lbo_a = GM_BM * 16u, lbo_b = BN * 16u;
-    const uint32_t kstep_a = (2u * lbo_a) >> 4, kstep_b = (2u * lbo_b) >> 4;
-    int kc = 0, it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      if (it >= 2) tc::mbar_wait(&t_empty[acc], (uint32_t)(((it >> 1) - 1) & 1));
-      tc::fence_after_sync();
-      const uint32_t d_tmem = tmem + (uint32_t)(acc * BN);
+    const uint64_t ks_a = (2u * lbo_a) >> 4, ks_b = (2u * lbo_b) >> 4;
+    int kc = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      const int mt = tile / NT, nt = tile - mt * NT;
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       for (int kt = 0; kt < KT; ++kt, ++kc) {
         const int st = kc % GM_STAGES;
         tc::mbar_wait(&bar_full[st], (uint32_t)((kc / GM_STAGES) & 1));
-        tc::fence_after_sync();
         const uint32_t a0 = s0 + (uint32_t)st * ST_BYTES;
-        uint64_t ad = tc::smem_desc(a0, lbo_a), bd = tc::smem_desc(a0 + A_BYTES, lbo_b);
+        const uint64_t ad = tc::smem_desc(a0 + (uint32_t)wg * 64u * 16u, lbo_a), bd = tc::smem_desc(a0 + A_BYTES, lbo_b);
+        tc::wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < GM_BK / 16; ++kk) {
-          tc::mma_bf16(d_tmem, ad, bd, idesc, (kt | kk) ? 1u : 0u);
-          ad += kstep_a; bd += kstep_b;
-        }
-        tc::mma_commit(&bar_empty[st]);
+        for (int kk = 0; kk < GM_BK / 16; ++kk) tc::Wg<BN, 0>::ss(acc, ad + kk * ks_a, bd + kk * ks_b, 1u);
+        tc::wg_commit();
+        tc::wg_wait<1>();                   // the previous k-tile's MMAs are done: release its stage
+        if (kt > 0 && t == 0) tc::mbar_arrive(&bar_empty[(kc - 1) % GM_STAGES]);
       }
-      tc::mma_commit(&t_full[acc]);
-    }
-  } else if (warp < 8) {
-    // ------------------------------------------------------------------ epilogue
-    const int grp = warp >> 2, wq = warp & 3;  // two warp groups split the columns
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const int mt = tile / NT, nt = tile - mt * NT;
-      tc::mbar_wait(&t_full[acc], (uint32_t)((it >> 1) & 1));
-      tc::fence_after_sync();
-      const int m = mt * GM_BM + wq * 32 + lane;
+      tc::wg_wait<0>();
+      tc::wg_hold(acc);
+      if (t == 0) tc::mbar_arrive(&bar_empty[(kc - 1) % GM_STAGES]);
+
+      // epilogue: 64-column chunks through the strip; thread = (row t % 64, 32-column half t / 64)
+      const int m = mt * GM_BM + wg * 64 + (t & 63);
       const int n0 = nt * BN;
-      const uint32_t tbase = tmem + ((uint32_t)(wq * 32) << 16) + (uint32_t)(acc * BN);
-      for (int c0 = grp * (BN / 2); c0 < (grp + 1) * (BN / 2); c0 += 16) {
-        uint32_t v[16];
-        tc::tmem_ld16(tbase + (uint32_t)c0, v);
-        float r16[16];
+#pragma unroll 1
+      for (int ch = 0; ch < BN / 64; ++ch) {
+        tc::named_sync(1 + wg, 128);        // the previous chunk has been read
+        tc::acc_to_smem<BN>(acc, strip, GM_EPI_LD, 8 * ch, 8 * ch + 8);
+        tc::named_sync(1 + wg, 128);
+#pragma unroll 1
+        for (int sub = 0; sub < 2; ++sub) {
+          const int cl = (t >> 6) * 32 + sub * 16;   // column inside the chunk
+          const int c0 = ch * 64 + cl;              // column inside the tile
+          float v[16];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) r16[j] = 0.f;
-        if ((EPI == EPI_RESID_F32 || EPI == EPI_GELU_ADD_F32) && m < M && res) {   // (EPI_RESID_F32 without res: plain fp32 output)
-          const int mr = (EPI == EPI_GELU_ADD_F32 && res_mod > 0) ? m % res_mod : m;
-          const float4* rr = reinterpret_cast<const float4*>(res + (size_t)mr * N + n0 + c0);
+          for (int j = 0; j < 16; j += 4) {
+            const float4 q = *reinterpret_cast<const float4*>(strip + (t & 63) * GM_EPI_LD + cl + j);
+            v[j] = q.x; v[j + 1] = q.y; v[j + 2] = q.z; v[j + 3] = q.w;
+          }
+          float r16[16];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) { const float4 q = rr[j]; r16[4 * j] = q.x; r16[4 * j + 1] = q.y; r16[4 * j + 2] = q.z; r16[4 * j + 3] = q.w; }
-        }
-        tc::tmem_ld_wait();
-        if (m < M) {
-          float f[16];
+          for (int j = 0; j < 16; ++j) r16[j] = 0.f;
+          if ((EPI == EPI_RESID_F32 || EPI == EPI_GELU_ADD_F32) && m < M && res) {   // (EPI_RESID_F32 without res: plain fp32 output)
+            const int mr = (EPI == EPI_GELU_ADD_F32 && res_mod > 0) ? m % res_mod : m;
+            const float4* rr = reinterpret_cast<const float4*>(res + (size_t)mr * N + n0 + c0);
 #pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) + (bias ? __ldg(bias + n0 + c0 + j) : 0.f);
+            for (int j = 0; j < 4; ++j) { const float4 q = rr[j]; r16[4 * j] = q.x; r16[4 * j + 1] = q.y; r16[4 * j + 2] = q.z; r16[4 * j + 3] = q.w; }
+          }
+          if (m < M) {
+            float f[16];
+#pragma unroll
+            for (int j = 0; j < 16; ++j) f[j] = v[j] + (bias ? __ldg(bias + n0 + c0 + j) : 0.f);
           if (EPI == EPI_GELU_ADD_F32 || EPI == EPI_GELU_CONV2_IMG || EPI == EPI_GELU_VALID_S2_IMG || EPI == EPI_GELU_ADD_F32_LD) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) f[j] = 0.5f * f[j] * (1.f + erff(f[j] * 0.70710678118654752440f));
@@ -216,19 +215,15 @@ gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __re
           }
         }
       }
-      tc::fence_before_sync();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(&t_empty[acc])) : "memory");
+      }
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 8) tc::tmem_dealloc(tmem, 2 * BN <= 256 ? 256 : 512);
 }
 
 template <int BN, int EPI>
 static int launch_gemm_t(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, void* out,
                          const float* res, int M, int N, int K, int res_mod, cudaStream_t s, int aux = 0) {
-  constexpr size_t smem = (size_t)GM_STAGES * (GM_BM * GM_BK * 2 + BN * GM_BK * 2);
+  constexpr size_t smem = (size_t)GM_STAGES * (GM_BM * GM_BK * 2 + BN * GM_BK * 2) + 2 * 64 * GM_EPI_LD * 4;
   static DevSmemCache attr_cache;
   SVCB_CUDA_CHECK(ensure_dyn_smem(gemm_tc_kernel<BN, EPI>, smem, attr_cache));
   const int n_sm = device_sm_count();
@@ -237,7 +232,7 @@ static int launch_gemm_t(const __nv_bfloat16* A, const __nv_bfloat16* W, const f
   const int grid = std::min(ntiles, n_sm);
   KernelScope ks("whisper_gemm_tc", s, 2.0 * M * (double)N * K,
                  2.0 * ((double)M * K + (double)N * K) + (EPI == EPI_RESID_F32 ? 8.0 : EPI == EPI_GELU_ADD_F32 ? 4.0 : 2.0) * M * (double)N);
-  gemm_tc_kernel<BN, EPI><<<grid, 320, smem, s>>>(A, W, bias, out, res, M, N, K, res_mod, aux);
+  gemm_tc_kernel<BN, EPI><<<grid, GM_THREADS, smem, s>>>(A, W, bias, out, res, M, N, K, res_mod, aux);
   SVCB_LAUNCH_CHECK("gemm_tc");
   return SVCB_OK;
 }

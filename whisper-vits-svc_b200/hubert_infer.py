@@ -1,6 +1,6 @@
-"""HuBERT-Soft content encoder on the B200 path — host-side mirror of the reference's `hubert/inference.py`
+"""HuBERT-Soft content encoder on the H100 path — host-side mirror of the reference's `hubert/inference.py`
 (`load_model`, `pred_vec`) and `hubert/hubert_model.py` (`hubert_soft`, `HubertSoft.units`) behind the C ABI
-(`svcb_hubert_*`, csrc/hubert_api.cu).  SURVEY.md §8f-2.  No CPU fallback: a CUDA (sm_100a) device is required."""
+(`svcb_hubert_*`, csrc/hubert_api.cu).  SURVEY.md §8f-2.  No CPU fallback: a CUDA (sm_90a) device is required."""
 from __future__ import annotations
 
 import ctypes
@@ -86,7 +86,7 @@ class HubertSoftB200:
     def __init__(self, state_dict: Dict[str, torch.Tensor], device):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise _lib.SvcbError("HuBERT-Soft runs only on a CUDA (sm_100a) device; no CPU fallback")
+            raise _lib.SvcbError("HuBERT-Soft runs only on a CUDA (sm_90a) device; no CPU fallback")
         items, self.n_layer = pack_hubert(state_dict)
         blob_cpu, table = pack.build_blob(items)
         blob = blob_cpu.to(self.device)

@@ -8,7 +8,7 @@ and streams here.  There is no CPU path: calling a compute method without a CUDA
 without the built library, raises.
 
 `precision` selects how the dense convolutions are computed (DESIGN.md §3): 3 (default) =
-bf16x3-split tcgen05 MMAs + fused fp32 narrow stages (meets the 1e-3 waveform gate, ~1e-5 measured),
+bf16x3-split wgmma MMAs + fused fp32 narrow stages (meets the 1e-3 waveform gate, ~1e-5 measured),
 1 = plain bf16 MMAs (faster, ~4e-3), 0 = all-fp32 CUDA-core kernels (device-side reference).
 
 The reference draws three random tensors internally (vits/models.py:51,
@@ -93,7 +93,7 @@ class SynthesizerInfer(torch.nn.Module):
     def _ensure(self):
         dev = self._device()
         if dev.type != "cuda":
-            raise _lib.SvcbError("SynthesizerInfer computes only on a CUDA device (sm_100a); "
+            raise _lib.SvcbError("SynthesizerInfer computes only on a CUDA device (sm_90a); "
                                  "call .to('cuda') first. There is no CPU fallback.")
         if self._handle is not None and self._packed_device == dev:
             return

@@ -1,4 +1,4 @@
-"""Host-side mirror of whisper/inference.py (`load_model`, `pred_ppg`) over the B200 encoder.
+"""Host-side mirror of whisper/inference.py (`load_model`, `pred_ppg`) over the H100 encoder.
 
 `load_model(path, device)` reads the reference checkpoint format {"dims", "model_state_dict"}
 (whisper/inference.py:12-20), applies the loader's surgery (decoder dropped, last quarter of the
@@ -109,7 +109,7 @@ class WhisperEncoderB200:
     def __init__(self, ckpt: dict, device):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise _lib.SvcbError("the Whisper encoder runs only on a CUDA (sm_100a) device; no CPU fallback")
+            raise _lib.SvcbError("the Whisper encoder runs only on a CUDA (sm_90a) device; no CPU fallback")
         self.dims = dict(ckpt["dims"])
         items, self.cfg = pack_whisper(ckpt)
         blob_cpu, table = pack.build_blob(items)
