@@ -13,7 +13,8 @@
  *   - return 0 on success, <0 = svcb_status; svcb_last_error() gives a thread-local message;
  *   - a model handle is immutable after creation: concurrent calls on different streams
  *     are fine when their workspaces differ;
- *   - sm_90a only, no fallback: svcb_model_create fails with SVCB_E_UNSUPPORTED elsewhere.
+ *   - sm_90a only, no fallback: svcb_model_create, svcb_whisper_create and svcb_hubert_create fail
+ *     with SVCB_E_UNSUPPORTED elsewhere.
  */
 #ifndef SVCB_H_
 #define SVCB_H_
@@ -206,11 +207,9 @@ size_t svcb_op_gemm_bf16_scratch_bytes(int32_t M, int32_t N, int32_t K);
 int svcb_op_gemm_bf16(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
                       int32_t M, int32_t N, int32_t K, int32_t epilogue, void* scratch, size_t scratch_bytes,
                       svcb_stream stream);
-/* softmax(q k^T / sqrt(64)) v per head: qkv bf16 [B*T, 3*D] rows (q|k|v), out bf16 [B*T, D]. */
-int svcb_op_attention_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, int32_t T, int32_t D, int32_t heads,
-                           svcb_stream stream);
-/* The same attention as the encoder runs it (csrc/whisper_attn_tc.cu): q k^T and p v as wgmma MMAs with S and
- * O in registers, operands taken from the head-major layout the QKV GEMM writes (built here from the row-major input).
+/* softmax(q k^T / sqrt(64)) v per head as the encoder runs it (csrc/whisper_attn_tc.cu): qkv bf16 [B*T, 3*D] rows
+ * (q|k|v), out bf16 [B*T, D].  q k^T and p v as wgmma MMAs with S and O in registers, operands taken from the
+ * head-major layout the QKV GEMM writes (built here from the row-major input).
  * v_layout: 0 = the V panel read as an MN-major operand with LBO = 128 B between 8-key groups (what the encoder
  * uses), 1 = LBO / SBO exchanged (kept for the descriptor unit test).  scratch: 256-byte aligned. */
 size_t svcb_op_attention_tc_bf16_scratch_bytes(int32_t B, int32_t T, int32_t D);
@@ -284,9 +283,6 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
  * and — when y_act != NULL — SnakeAlias_out(result) as the next link's bf16 hi/lo operand image, returned
  * here decoded to fp32 [B,C,L].  w_s2d = pack.py:pack_conv_s2d image; L % (160/C) == 0. */
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L);
-/* Debugging hook (profiling scripts): when dev_buf != NULL, CTA 0 of every following amp_s2d link launch
- * writes clock64() stamps of its first 32 tiles into dev_buf ([32][16] int64); NULL switches it off. */
-void svcb_debug_s2d_trace(void* dev_buf);
 int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                          const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                          const float* fd, const void* w_s2d, const float* bias, int32_t B, int32_t C, int32_t L,

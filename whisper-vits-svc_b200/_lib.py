@@ -87,7 +87,6 @@ SIGNATURES = {
     "svcb_whisper_log_mel": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
     "svcb_op_gemm_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_gemm_bf16": (c_int, [c_void_p] * 5 + [c_int32] * 4 + [c_void_p, c_size_t, c_void_p]),
-    "svcb_op_attention_bf16": (c_int, [c_void_p, c_void_p] + [c_int32] * 4 + [c_void_p]),
     "svcb_op_attention_tc_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_attention_tc_bf16": (c_int, [c_void_p, c_void_p] + [c_int32] * 5 + [c_void_p, c_size_t, c_void_p]),
     "svcb_timing_enable": (None, [c_int32]),
@@ -111,7 +110,6 @@ SIGNATURES = {
     "svcb_op_conv_tc": (c_int, [c_void_p] * 6 + [c_int32] * 9 + [c_void_p]),
     "svcb_op_amp_conv_tc_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_amp_conv_tc": (c_int, [c_void_p] * 9 + [c_int32] * 6 + [c_void_p, c_size_t, c_void_p]),
-    "svcb_debug_s2d_trace": (None, [c_void_p]),
     "svcb_op_amp_s2d_link_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_amp_s2d_link": (c_int, [c_void_p] * 12 + [c_int32] * 5 + [c_void_p, c_size_t, c_void_p]),
     "svcb_op_tc_gemm_selftest": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int32] * 4 + [c_void_p]),

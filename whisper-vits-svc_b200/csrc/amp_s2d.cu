@@ -396,7 +396,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
               for (int i = 0; i < 6; ++i) {
                 const int j = a + 1 + i;
                 const float2 pr = (j & 1) ? XO[(j - 1) / 2] : XE[j / 2];
-                U = i == 0 ? f2_mul(pr, p.fup[0]) : f2_fma(pr, p.fup[i], U);
+                U = i == 0 ? f2_mul(pr, p.taps.fup[0]) : f2_fma(pr, p.taps.fup[i], U);
               }
               // u + sin^2(a u) / (e^beta + 1e-9) = (u + b/2) - (b/2) cos(2 a u); a u = k pi + r, |r| <= pi/2
               const float2 t = f2_mul(U, make_float2(a_, a_));
@@ -449,12 +449,12 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
 #pragma unroll
             for (int n = 0; n < R; ++n) {
               // out[n] = v[2n-5] f0 + sum_i (v[2n-4+2i], v[2n-3+2i]) . (f[2i+1], f[2i+2]) + v[2n+6] f11
-              float2 acc2 = f2_mul(V[k][n + 1], p.fdp[0]);
+              float2 acc2 = f2_mul(V[k][n + 1], p.taps.fdp[0]);
 #pragma unroll
-              for (int i = 1; i < 5; ++i) acc2 = f2_fma(V[k][n + 1 + i], p.fdp[i], acc2);
+              for (int i = 1; i < 5; ++i) acc2 = f2_fma(V[k][n + 1 + i], p.taps.fdp[i], acc2);
               float o1 = acc2.x + acc2.y;
-              o1 = fmaf(V[k][n].y, p.fd0, o1);
-              out[k * R + n] = fmaf(V[k][n + 6].x, p.fd11, o1);
+              o1 = fmaf(V[k][n].y, p.taps.fd0, o1);
+              out[k * R + n] = fmaf(V[k][n + 6].x, p.taps.fd11, o1);
             }
           }
           if (useful) {
@@ -477,13 +477,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
   }
 }
 
-static long long* g_s2d_trace = nullptr;
-void s2d_set_trace(long long* dev_buf) { g_s2d_trace = dev_buf; }
-long long* s2d_get_trace() { return g_s2d_trace; }
-
-int launch_amp_s2d_link(const AmpS2dParams& p_in, cudaStream_t s) {
-  AmpS2dParams p = p_in;
-  p.trace = g_s2d_trace;
+int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s) {
   const int r = p.C > 0 ? s2d::N / p.C : 0;
   if (p.B <= 0 || p.L <= 0 || p.C * r != s2d::N || (r != 4 && r != 8 && r != 16) || p.L % r) {
     set_error("amp_s2d_link: unsupported shape (need C * r = 160 with r in {4, 8, 16} and L % r == 0)");

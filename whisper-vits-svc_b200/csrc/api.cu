@@ -3,6 +3,7 @@
 #include <algorithm>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -68,12 +69,6 @@ struct SnakeW {
   float fu_h[12] = {0}, fd_h[12] = {0};   // host copies of the 12 + 12 alias-filter taps (read back once at model creation)
   SnakeTapsV tapsv() const { return snake_taps_pack(fu_h, fd_h); }
 };
-static void snake_taps_to(const SnakeW& w, AmpS2dParams& q) {
-  for (int k = 0; k < 12; ++k) { q.fu2[k] = 2.f * w.fu_h[k]; q.fdn[k] = w.fd_h[k]; }
-  for (int i = 0; i < 6; ++i) q.fup[i] = make_float2(q.fu2[11 - 2 * i], q.fu2[10 - 2 * i]);
-  for (int i = 0; i < 5; ++i) q.fdp[i] = make_float2(q.fdn[2 * i + 1], q.fdn[2 * i + 2]);
-  q.fd0 = q.fdn[0]; q.fd11 = q.fdn[11];
-}
 
 struct EncLayer {
   ConvW qkv, o, ffn1, ffn2;
@@ -84,6 +79,12 @@ struct FlowLayer {
   std::vector<ConvW> in, rs;
   const float *snac_w, *snac_b;
 };
+// Which kernels run each generator stage.  They depend only on the config, the precision and the blob's images,
+// so resolve() chooses them once at model creation.
+enum UpsForm { UPS_POLYPHASE, UPS_COMB, UPS_FUSED };      // `rate` phase convs + ups_finalize | `comb` | ups_fused
+enum NoiseForm { NOISE_IN_UPS, NOISE_TC, NOISE_CONV1D };  // inside the upsampler's kernel | `noise_tc` | conv1d
+enum AmpForm { AMP_S2D, AMP_BLOCK_FUSED, AMP_TC, AMP_FP32 };
+
 struct UpStage {
   std::vector<ConvW> phase;  // one sub-convolution per output phase
   const float* bias;
@@ -92,6 +93,10 @@ struct UpStage {
   int comb_cin1 = 0, comb_cin2 = 0;   // comb's input channels: [0, comb_cin1) the stage input (zero padded), then windows of the source
   ConvW comb;                // all phases as ONE conv with rate * Cout channels, taps + 1 taps (pack.py:ups_combined) or tc == null
   int rate, k, pad, taps;
+  int sf = 1;                // source samples per output sample: the product of the later stages' rates
+  UpsForm form = UPS_POLYPHASE;
+  std::vector<bool> phase_tc;   // UPS_POLYPHASE: phase r runs as conv_tc, else conv1d
+  NoiseForm noise_form = NOISE_IN_UPS;
 };
 struct ResBlock {
   ConvW c1[3], c2[3];
@@ -101,6 +106,9 @@ struct ResBlock {
   int s2d_r = 0, s2d_ml1[3], s2d_nt1[3], s2d_ml2[3], s2d_nt2[3];
   SnakeW act[6];
   int k, dil[3];
+  AmpForm form = AMP_FP32;
+  AmpForm fallback = AMP_FP32;   // the form when the stage runs without s2d images (= form unless that is AMP_S2D):
+                                 // AMP_S2D needs L % s2d_r == 0 and L % 8 == 0
 };
 
 // must match pack.py:S2D_LINK_FACTORS / s2d_taps
@@ -116,9 +124,6 @@ static void s2d_taps(int k, int dil, int r, int& mlo, int& ntaps) {
 struct svcb_model {
   svcb_config cfg;
   int hop = 1;
-  const char* blob = nullptr;
-  size_t blob_bytes = 0;
-  std::map<std::string, std::pair<const float*, uint64_t>> tensors;
   // resolved views
   svcb::ConvW pre, hub, proj;
   const float* pit_emb = nullptr;
@@ -190,6 +195,18 @@ static ConvParams std_conv(const ConvW& w, const float* x, float* y, int B, int 
   return p;
 }
 
+// A stride-1 tensor-core convolution of w over x[b, ci, t] = x[b * sxb + ci * sxc + t * sxt] into y[B, Cout, Tout].
+static ConvTcParams conv_tc_params(const ConvW& w, const float* x, long long sxb, long long sxc, long long sxt, float* y,
+                                   int B, int Tin, int Tout, int dil, int pad, int nsplit) {
+  ConvTcParams q;
+  q.x = x; q.sxb = sxb; q.sxc = sxc; q.sxt = sxt;
+  q.wpk = w.tc; q.bias = w.b; q.y = y;
+  q.B = B; q.Cin = w.cin; q.cin_pad = w.cin_pad; q.Cout = w.cout; q.Tin = Tin; q.Tout = Tout;
+  q.K = w.k; q.dil = dil; q.pad = pad; q.kch = w.kch; q.bn = w.bn; q.ntiles = w.ntiles;
+  q.nsplit = nsplit;
+  return q;
+}
+
 // Route a stride-1 "same" convolution to the tensor cores when the model runs in a tensor-core
 // precision mode and the conv has a tile image; otherwise the fp32 CUDA-core kernel.
 static int run_conv(const svcb_model* m, const ConvW& w, const ConvParams& p, cudaStream_t s) {
@@ -197,12 +214,9 @@ static int run_conv(const svcb_model* m, const ConvW& w, const ConvParams& p, cu
   if (prec == 0 || !w.tc || p.stride != 1 || p.out_mul != 1 || p.out_off != 0 || p.q0 != 0 ||
       p.syt != 1 || p.addvec || p.out_div != 0.f || p.nq != p.Tin)
     return launch_conv1d(p, s);
-  ConvTcParams q;
-  q.x = p.x; q.sxb = p.sxb; q.sxc = p.sxc; q.sxt = p.sxt;
-  q.wpk = w.tc; q.bias = p.bias; q.y = p.y; q.res = p.res; q.lengths = p.lengths;
-  q.B = p.B; q.Cin = p.Cin; q.cin_pad = w.cin_pad; q.Cout = p.Cout; q.Tin = p.Tin; q.Tout = p.nq;
-  q.K = p.K; q.dil = p.dil; q.pad = p.pad; q.kch = w.kch; q.bn = w.bn; q.ntiles = w.ntiles;
-  q.nsplit = prec == 1 ? 1 : 3; q.flags = p.flags; q.act = p.act;
+  // (every caller builds p with std_conv from w: p.bias, Cin, Cout and K are w's)
+  ConvTcParams q = conv_tc_params(w, p.x, p.sxb, p.sxc, p.sxt, p.y, p.B, p.Tin, p.nq, p.dil, p.pad, prec == 1 ? 1 : 3);
+  q.res = p.res; q.lengths = p.lengths; q.flags = p.flags; q.act = p.act;
   return launch_conv_tc(q, s);
 }
 
@@ -378,105 +392,105 @@ static int run_flow(const svcb_model* m, Ctx& ctx, const float* z_p, const long 
 }
 
 // ----------------------------------------------------------------------------- generator
-static int run_amp_stage(const svcb_model* m, Ctx& ctx, int stage, const float* X, float* ACC,
-                         float* T1, float* T2, float* RA, float* RB, void* IMG_HI, void* IMG_LO, void* const* S2D,
-                         int B, int ch, int L) {
-  cudaStream_t s = ctx.stream;
-  const int nres = m->cfg.n_res;
-  const int prec = m->cfg.precision;
-  for (int j = 0; j < nres; ++j) {
-    const ResBlock& R = m->res[stage * nres + j];
-    if (prec == 3 && R.s2d_r && S2D[0] && L % R.s2d_r == 0 && L % 8 == 0) {
-      // narrow stages: every link = block-Toeplitz wgmma conv with the next SnakeAlias in its epilogue
-      const int Rp = s2d_rows(L, R.s2d_r);
-      void *ia_hi = S2D[0], *ia_lo = S2D[1], *ib_hi = S2D[2], *ib_lo = S2D[3];
-      const SnakeTapsV tv0 = R.act[0].tapsv();
-      RUN(launch_snake_pack_s2d(X, ia_hi, ia_lo, R.act[0].ea, R.act[0].ib, R.act[0].fu, R.act[0].fd, B, ch, L, s, &tv0));
-      const float* cur = X;
-      for (int d = 0; d < 3; ++d) {
-        AmpS2dParams q;
-        q.B = B; q.C = ch; q.L = L; q.K = R.k; q.Rp = Rp;
-        q.a_hi = ia_hi; q.a_lo = ia_lo; q.o_hi = ib_hi; q.o_lo = ib_lo;
-        q.wpk = R.c1_s2d[d]; q.bias = R.c1[d].b; q.ntaps = R.s2d_nt1[d]; q.mlo = R.s2d_ml1[d];
-        const SnakeW& a2 = R.act[2 * d + 1];
-        q.ea = a2.ea; q.ib = a2.ib; q.fu = a2.fu; q.fd = a2.fd;
-        snake_taps_to(a2, q);
-        RUN(launch_amp_s2d_link(q, s));
-        AmpS2dParams q2;
-        q2.B = B; q2.C = ch; q2.L = L; q2.K = R.k; q2.Rp = Rp;
-        q2.a_hi = ib_hi; q2.a_lo = ib_lo;
-        q2.wpk = R.c2_s2d[d]; q2.bias = R.c2[d].b; q2.ntaps = R.s2d_nt2[d]; q2.mlo = R.s2d_ml2[d];
-        q2.res = cur;
-        if (d < 2) {
-          q2.y = (d == 0) ? RA : RB;
-          const SnakeW& a3 = R.act[2 * d + 2];
-          q2.o_hi = ia_hi; q2.o_lo = ia_lo; q2.ea = a3.ea; q2.ib = a3.ib; q2.fu = a3.fu; q2.fd = a3.fd;
-          snake_taps_to(a3, q2);
-        } else {  // last unit of the block: fold into the stage mean (generator.py:188-194)
-          q2.y = ACC; q2.accum = j > 0;
-          if (j == nres - 1) q2.out_div = (float)nres;
-        }
-        RUN(launch_amp_s2d_link(q2, s));
-        cur = q2.y;
-      }
-      continue;
-    }
-    if (prec != 0 && amp_block_fused_supported(ch, R.k, R.dil)) {
-      // narrow stages: the whole block (6 convs + 6 SnakeAlias + residuals) in one fp32 kernel
-      AmpBlockParams q;
-      q.x = X; q.y = ACC; q.B = B; q.C = ch; q.L = L; q.K = R.k;
-      for (int d = 0; d < 3; ++d) {
-        q.dil[d] = R.dil[d];
-        q.w1[d] = R.c1[d].w; q.b1[d] = R.c1[d].b; q.w2[d] = R.c2[d].w; q.b2[d] = R.c2[d].b;
-      }
-      q.cout_pad = R.c1[0].cout_pad;
-      for (int a = 0; a < 6; ++a) { q.ea[a] = R.act[a].ea; q.ib[a] = R.act[a].ib; q.fu[a] = R.act[a].fu; q.fd[a] = R.act[a].fd; }
-      q.accum = j > 0;
-      if (j == nres - 1) q.out_div = (float)nres;
-      RUN(launch_amp_block_fused(q, s));
-      continue;
-    }
-    const float* cur = X;
-    for (int d = 0; d < 3; ++d) {
-      const SnakeW& a1 = R.act[2 * d];
-      const SnakeW& a2 = R.act[2 * d + 1];
-      if (prec != 0) {  // tensor-core path: snake_pack -> amp_conv_tc, twice per unit
-        AmpConvParams q;
-        q.B = B; q.C = ch; q.Cp = (ch + 15) / 16 * 16; q.L = L; q.K = R.k; q.nsplit = prec == 1 ? 1 : 3;
-        q.Lp = p8_rows(L); q.a_hi = IMG_HI; q.a_lo = q.nsplit == 3 ? IMG_LO : nullptr;
-        void* lo = q.nsplit == 3 ? IMG_LO : nullptr;
-        const SnakeTapsV tv1 = a1.tapsv(), tv2 = a2.tapsv();
-        RUN(launch_snake_pack(cur, IMG_HI, lo, a1.ea, a1.ib, a1.fu, a1.fd, B, ch, L, s, &tv1));
-        q.y = T2; q.wpk = R.c1_tc[d]; q.bias = R.c1[d].b; q.dil = R.dil[d];
-        RUN(launch_amp_conv_tc(q, s));
-        RUN(launch_snake_pack(T2, IMG_HI, lo, a2.ea, a2.ib, a2.fu, a2.fd, B, ch, L, s, &tv2));
-        q.wpk = R.c2_tc[d]; q.bias = R.c2[d].b; q.dil = 1; q.res = cur;
-        if (d < 2) {
-          q.y = (d == 0) ? RA : RB;
-        } else {
-          q.y = ACC;
-          q.accum = j > 0;
-          if (j == nres - 1) q.out_div = (float)nres;
-        }
-        RUN(launch_amp_conv_tc(q, s));
-        cur = q.y;
-        continue;
-      }
-      RUN(launch_snake_alias(cur, T1, a1.ea, a1.ib, a1.fu, a1.fd, B, ch, L, s));
-      RUN(launch_conv1d(std_conv(R.c1[d], T1, T2, B, L, L, R.dil[d] * (R.k - 1) / 2, R.dil[d]), s));
-      RUN(launch_snake_alias(T2, T1, a2.ea, a2.ib, a2.fu, a2.fd, B, ch, L, s));
-      ConvParams p = std_conv(R.c2[d], T1, nullptr, B, L, L, (R.k - 1) / 2);
-      p.res = cur;
-      if (d < 2) {
-        p.y = (d == 0) ? RA : RB;
-      } else {  // last unit of the block: fold into the stage mean (generator.py:188-194)
-        p.y = ACC;
-        if (j > 0) p.flags |= CONV_ACCUM;
-        if (j == nres - 1) p.out_div = (float)nres;
-      }
-      RUN(launch_conv1d(p, s));
-      cur = p.y;
-    }
+// The buffers of one stage's AMP blocks.  Unit d of block j writes RA, RB, then ACC: each block adds its output to
+// the stage mean there (generator.py:188-194), the first block writes it, the others accumulate, the last divides.
+struct AmpStage {
+  const float* X;             // stage input [B, C, L]
+  float* ACC;
+  float *T1, *T2, *RA, *RB;   // fp32 temporaries [B, C, L]
+  void *img_hi, *img_lo;      // snake_pack operand images (AMP_TC)
+  void* s2d[4];               // two ping-pong S2D images, hi and lo each (AMP_S2D)
+  int B, C, L, nres, nsplit;
+  float* out(int d) const { return d == 0 ? RA : d == 1 ? RB : ACC; }
+  bool accum(int d, int j) const { return d == 2 && j > 0; }
+  float out_div(int d, int j) const { return d == 2 && j == nres - 1 ? (float)nres : 0.f; }
+};
+
+// Link `half` of unit d: c1[d] from S2D image 0 to image 1, or c2[d] from image 1 to image 0 (a.s2d = hi, lo of each);
+// the output image is the SnakeAlias that follows the conv, none after the block's last one.
+static AmpS2dParams s2d_link(const AmpStage& a, const ResBlock& R, int d, int half) {
+  void* const* in = a.s2d + 2 * half;
+  void* const* out = a.s2d + 2 - 2 * half;
+  const int next = 2 * d + 1 + half;   // the SnakeAlias after this conv
+  AmpS2dParams q;
+  q.B = a.B; q.C = a.C; q.L = a.L; q.K = R.k; q.Rp = s2d_rows(a.L, R.s2d_r);
+  q.a_hi = in[0]; q.a_lo = in[1];
+  q.wpk = half ? R.c2_s2d[d] : R.c1_s2d[d]; q.bias = half ? R.c2[d].b : R.c1[d].b;
+  q.ntaps = half ? R.s2d_nt2[d] : R.s2d_nt1[d]; q.mlo = half ? R.s2d_ml2[d] : R.s2d_ml1[d];
+  if (next < 6) {
+    const SnakeW& act = R.act[next];
+    q.o_hi = out[0]; q.o_lo = out[1];
+    q.ea = act.ea; q.ib = act.ib; q.fu = act.fu; q.fd = act.fd; q.taps = act.tapsv();
+  }
+  return q;
+}
+
+// narrow stages: every link = block-Toeplitz wgmma conv with the next SnakeAlias in its epilogue
+static int run_amp_s2d(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+  const SnakeW& s0 = R.act[0];
+  const SnakeTapsV tv0 = s0.tapsv();
+  RUN(launch_snake_pack_s2d(a.X, a.s2d[0], a.s2d[1], s0.ea, s0.ib, s0.fu, s0.fd, a.B, a.C, a.L, ctx.stream, &tv0));
+  const float* cur = a.X;
+  for (int d = 0; d < 3; ++d) {
+    RUN(launch_amp_s2d_link(s2d_link(a, R, d, 0), ctx.stream));
+    AmpS2dParams q = s2d_link(a, R, d, 1);
+    q.res = cur; q.y = a.out(d); q.accum = a.accum(d, j); q.out_div = a.out_div(d, j);
+    RUN(launch_amp_s2d_link(q, ctx.stream));
+    cur = q.y;
+  }
+  return SVCB_OK;
+}
+
+// narrow stages: the whole block (6 convs + 6 SnakeAlias + residuals) in one fp32 kernel
+static int run_amp_block_fused(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+  AmpBlockParams q;
+  q.x = a.X; q.y = a.ACC; q.B = a.B; q.C = a.C; q.L = a.L; q.K = R.k;
+  for (int d = 0; d < 3; ++d) {
+    q.dil[d] = R.dil[d];
+    q.w1[d] = R.c1[d].w; q.b1[d] = R.c1[d].b; q.w2[d] = R.c2[d].w; q.b2[d] = R.c2[d].b;
+  }
+  q.cout_pad = R.c1[0].cout_pad;
+  for (int k = 0; k < 6; ++k) { q.ea[k] = R.act[k].ea; q.ib[k] = R.act[k].ib; q.fu[k] = R.act[k].fu; q.fd[k] = R.act[k].fd; }
+  q.accum = a.accum(2, j); q.out_div = a.out_div(2, j);   // (the block's last unit writes the stage mean)
+  RUN(launch_amp_block_fused(q, ctx.stream));
+  return SVCB_OK;
+}
+
+// tensor-core path: snake_pack -> amp_conv_tc, twice per unit
+static int run_amp_tc(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+  void* lo = a.nsplit == 3 ? a.img_lo : nullptr;
+  const float* cur = a.X;
+  for (int d = 0; d < 3; ++d) {
+    const SnakeW& s1 = R.act[2 * d];
+    const SnakeW& s2 = R.act[2 * d + 1];
+    AmpConvParams q;
+    q.B = a.B; q.C = a.C; q.Cp = (a.C + 15) / 16 * 16; q.L = a.L; q.K = R.k; q.nsplit = a.nsplit;
+    q.Lp = p8_rows(a.L); q.a_hi = a.img_hi; q.a_lo = lo;
+    const SnakeTapsV tv1 = s1.tapsv(), tv2 = s2.tapsv();
+    RUN(launch_snake_pack(cur, a.img_hi, lo, s1.ea, s1.ib, s1.fu, s1.fd, a.B, a.C, a.L, ctx.stream, &tv1));
+    q.y = a.T2; q.wpk = R.c1_tc[d]; q.bias = R.c1[d].b; q.dil = R.dil[d];
+    RUN(launch_amp_conv_tc(q, ctx.stream));
+    RUN(launch_snake_pack(a.T2, a.img_hi, lo, s2.ea, s2.ib, s2.fu, s2.fd, a.B, a.C, a.L, ctx.stream, &tv2));
+    q.wpk = R.c2_tc[d]; q.bias = R.c2[d].b; q.dil = 1; q.res = cur;
+    q.y = a.out(d); q.accum = a.accum(d, j); q.out_div = a.out_div(d, j);
+    RUN(launch_amp_conv_tc(q, ctx.stream));
+    cur = q.y;
+  }
+  return SVCB_OK;
+}
+
+static int run_amp_fp32(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+  const float* cur = a.X;
+  for (int d = 0; d < 3; ++d) {
+    const SnakeW& s1 = R.act[2 * d];
+    const SnakeW& s2 = R.act[2 * d + 1];
+    RUN(launch_snake_alias(cur, a.T1, s1.ea, s1.ib, s1.fu, s1.fd, a.B, a.C, a.L, ctx.stream));
+    RUN(launch_conv1d(std_conv(R.c1[d], a.T1, a.T2, a.B, a.L, a.L, R.dil[d] * (R.k - 1) / 2, R.dil[d]), ctx.stream));
+    RUN(launch_snake_alias(a.T2, a.T1, s2.ea, s2.ib, s2.fu, s2.fd, a.B, a.C, a.L, ctx.stream));
+    ConvParams p = std_conv(R.c2[d], a.T1, a.out(d), a.B, a.L, a.L, (R.k - 1) / 2);
+    p.res = cur; p.flags = a.accum(d, j) ? CONV_ACCUM : 0; p.out_div = a.out_div(d, j);
+    RUN(launch_conv1d(p, ctx.stream));
+    cur = p.y;
   }
   return SVCB_OK;
 }
@@ -486,26 +500,26 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
   const svcb_config& c = m->cfg;
   cudaStream_t s = ctx.stream;
   const int U = c.gen_input;
+  const int nsplit = c.precision == 1 ? 1 : 3;
   const long long Ltot = (long long)T * m->hop;
   float* sc = ctx.alloc<float>((size_t)B * U);
   float* bi = ctx.alloc<float>((size_t)B * U);
   float* xa = ctx.alloc<float>((size_t)B * U * T);
   float* x0 = ctx.alloc<float>((size_t)B * c.gen_initial_channel * T);
-  // temporaries sized for the largest stage
-  size_t max_stage = 0;
+  // temporaries and operand images sized for the largest stage
+  size_t max_stage = 0, img_bytes = 0;
   {
     int ch = c.gen_initial_channel; long long L = T;
-    for (int i = 0; i < c.n_ups; ++i) { ch /= 2; L *= c.up_rates[i]; max_stage = std::max<size_t>(max_stage, (size_t)B * ch * L); }
+    for (int i = 0; i < c.n_ups; ++i) {
+      ch /= 2; L *= c.up_rates[i];
+      max_stage = std::max<size_t>(max_stage, (size_t)B * ch * L);
+      if (c.precision != 0) img_bytes = std::max<size_t>(img_bytes, p8_image_bytes(B, ch, (int)L));
+    }
   }
   float* T1 = ctx.alloc<float>(max_stage);
   float* T2 = ctx.alloc<float>(max_stage);
   float* RA = ctx.alloc<float>(max_stage);
   float* RB = ctx.alloc<float>(max_stage);
-  size_t img_bytes = 0;
-  if (c.precision != 0) {
-    int ch = c.gen_initial_channel; long long L = T;
-    for (int i = 0; i < c.n_ups; ++i) { ch /= 2; L *= c.up_rates[i]; img_bytes = std::max<size_t>(img_bytes, p8_image_bytes(B, ch, (int)L)); }
-  }
   const long long Lpad = (SRC_PADF + Ltot + 128 + 3) / 4 * 4;
   float* SRCP = c.precision != 0 ? ctx.alloc<float>((size_t)B * Lpad) : nullptr;
   void* IMG_HI = img_bytes ? ctx.alloc<uint8_t>(img_bytes) : nullptr;
@@ -533,118 +547,95 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
   int L = T;
   for (int i = 0; i < c.n_ups; ++i) {
     const UpStage& us = m->ups[i];
-    const int chn = ch / 2, Ln = L * us.rate;
+    const int chn = ch / 2, Ln = L * us.rate, sf = us.sf;
     float* X = ctx.alloc<float>((size_t)B * chn * Ln);
     float* ACC = ctx.alloc<float>((size_t)B * chn * Ln);
     SVCB_TRY(check_ws(ctx));
-    // ConvTranspose1d as `rate` polyphase sub-convolutions (generator.py:183), each into its own
-    // contiguous slab of T1 (coalesced), interleaved + biased + (short) noise conv by ups_finalize
-    int sf = 1;
-    for (int k2 = i + 1; k2 < c.n_ups; ++k2) sf *= c.up_rates[k2];
-    const bool last = (i + 1 == c.n_ups);
-    const int Kn = us.noise.k;
-    const bool fuse_noise = Kn <= 8;
-    UpsFinalizeParams fp;
-    fp.bias = us.bias; fp.y = X; fp.C = chn; fp.Ln = Ln; fp.rate = us.rate; fp.pad = us.pad;
-    fp.src = fuse_noise ? source : nullptr; fp.wn = us.noise.w; fp.bn = us.noise.b; fp.Kn = Kn;
-    fp.sf = last ? 1 : sf; fp.padn = last ? 0 : sf / 2; fp.cout_pad = us.noise.cout_pad; fp.Ltot = Ltot;
-    size_t slab = 0;
-    const bool fused_up = c.precision != 0 && fuse_noise && ups_fused_supported(ch, chn, us.rate, us.taps, Kn);
-    // wide stages: every phase AND the stage's noise conv in one tensor-core conv whose epilogue stores the
-    // interleaved samples — the stage input is read once, X is written once
-    const bool comb_up = c.precision != 0 && !fused_up && us.comb.tc != nullptr && !last && Kn == 2 * sf && sf / 2 <= SRC_PADF;
-    if (comb_up) {
-      fp.src = nullptr;
-      const ConvW& w = us.comb;
-      ConvTcParams q;
-      q.x = x; q.sxb = (long long)ch * L; q.sxc = L; q.sxt = 1;
-      q.wpk = w.tc; q.bias = w.b; q.y = X;
-      q.B = B; q.Cin = ch; q.cin_pad = w.cin_pad; q.Cout = w.cout; q.Tin = L; q.Tout = L;
-      q.K = w.k; q.dil = 1; q.pad = us.taps - 1; q.kch = w.kch; q.bn = w.bn; q.ntiles = w.ntiles;
-      q.nsplit = c.precision == 1 ? 1 : 3; q.ilv = us.rate;
+    // ups[i](x) (ConvTranspose1d, generator.py:183) + noise_convs[i](source) (generator.py:185-186)
+    if (us.form == UPS_COMB) {
+      // wide stages: every phase AND the stage's noise conv in one tensor-core conv whose epilogue stores the
+      // interleaved samples — the stage input is read once, X is written once
+      ConvTcParams q = conv_tc_params(us.comb, x, (long long)ch * L, L, 1, X, B, L, L, 1, us.taps - 1, nsplit);
+      q.Cin = ch; q.ilv = us.rate;
       q.x2 = SRCP + (SRC_PADF - sf / 2); q.sx2b = Lpad; q.sx2t = (long long)sf * us.rate;
       q.cin1 = us.comb_cin1; q.cin2 = us.comb_cin2;
       RUN(launch_conv_tc(q, s));
-    }
-    if (fused_up) {  // narrow stages: transposed conv + noise conv + biases in one fp32 pass
+    } else if (us.form == UPS_FUSED) {  // narrow stages: transposed conv + noise conv + biases in one fp32 pass
       UpsFusedParams q;
       q.x = x; q.wph[0] = us.phase[0].w; q.wph[1] = us.phase[1].w; q.bias = us.bias;
       q.src = source; q.wn = us.noise.w; q.bn = us.noise.b; q.y = X;
       q.B = B; q.Cin = ch; q.Cout = chn; q.L = L; q.Ln = Ln; q.rate = us.rate; q.M = us.taps; q.pad = us.pad;
-      q.cout_pad = us.phase[0].cout_pad; q.Kn = Kn; q.sf = fp.sf; q.padn = fp.padn;
+      q.cout_pad = us.phase[0].cout_pad; q.Kn = us.noise.k; q.sf = sf; q.padn = sf / 2;
       q.cout_pad_n = us.noise.cout_pad; q.Ltot = Ltot;
       RUN(launch_ups_fused(q, s));
-    }
-    for (int r = 0; r < us.rate && !fused_up && !comb_up; ++r) {
-      ConvParams p = std_conv(us.phase[r], x, nullptr, B, L, Ln, us.taps - 1);
-      p.bias = nullptr;
-      const int pr = us.pad - r;
-      p.q0 = pr > 0 ? (pr + us.rate - 1) / us.rate : 0;
-      const int qmax = (Ln - 1 + us.pad - r) / us.rate;
-      p.nq = qmax - p.q0 + 1;
-      p.y = T1 + slab;
-      p.syb = (long long)chn * p.nq; p.syc = p.nq; p.syt = 1;
-      p.out_mul = 1; p.out_off = -p.q0;
-      fp.tmp[r] = p.y; fp.nq[r] = p.nq; fp.q0[r] = p.q0;
-      slab += (size_t)B * chn * p.nq;
-      if (c.precision != 0 && us.phase[r].tc && p.nq == L && us.taps - 1 - p.q0 >= 0) {
-        // phase r is a stride-1 convolution with nq == L outputs: x index = t + j - (taps-1-q0)
-        ConvTcParams q;
-        const ConvW& w = us.phase[r];
-        q.x = x; q.sxb = (long long)ch * L; q.sxc = L; q.sxt = 1;
-        q.wpk = w.tc; q.bias = nullptr; q.y = p.y;
-        q.B = B; q.Cin = ch; q.cin_pad = w.cin_pad; q.Cout = chn; q.Tin = L; q.Tout = L;
-        q.K = us.taps; q.dil = 1; q.pad = us.taps - 1 - p.q0; q.kch = w.kch; q.bn = w.bn; q.ntiles = w.ntiles;
-        q.nsplit = c.precision == 1 ? 1 : 3;
-        RUN(launch_conv_tc(q, s));
-      } else {
-        RUN(launch_conv1d(p, s));
+    } else {
+      // `rate` polyphase sub-convolutions, each into its own contiguous slab of T1 (coalesced), interleaved + biased
+      // + (short) noise conv by ups_finalize
+      UpsFinalizeParams fp;
+      fp.bias = us.bias; fp.y = X; fp.C = chn; fp.Ln = Ln; fp.rate = us.rate; fp.pad = us.pad;
+      fp.src = us.noise_form == NOISE_IN_UPS ? source : nullptr; fp.wn = us.noise.w; fp.bn = us.noise.b;
+      fp.Kn = us.noise.k; fp.sf = sf; fp.padn = sf / 2; fp.cout_pad = us.noise.cout_pad; fp.Ltot = Ltot;
+      size_t slab = 0;
+      for (int r = 0; r < us.rate; ++r) {
+        ConvParams p = std_conv(us.phase[r], x, nullptr, B, L, Ln, us.taps - 1);
+        const int pr = us.pad - r;
+        p.q0 = pr > 0 ? (pr + us.rate - 1) / us.rate : 0;
+        const int qmax = (Ln - 1 + us.pad - r) / us.rate;
+        p.nq = qmax - p.q0 + 1;
+        p.y = T1 + slab;
+        p.syb = (long long)chn * p.nq; p.syc = p.nq; p.syt = 1;
+        p.out_mul = 1; p.out_off = -p.q0;
+        fp.tmp[r] = p.y; fp.nq[r] = p.nq; fp.q0[r] = p.q0;
+        slab += (size_t)B * chn * p.nq;
+        if (us.phase_tc[r]) {
+          // phase r is a stride-1 convolution with nq == L outputs: x index = t + j - (taps-1-q0)
+          RUN(launch_conv_tc(conv_tc_params(us.phase[r], x, (long long)ch * L, L, 1, p.y, B, L, L, 1, us.taps - 1 - p.q0, nsplit), s));
+        } else {
+          RUN(launch_conv1d(p, s));
+        }
       }
+      if (!ctx.dry) SVCB_TRY(launch_ups_finalize(fp, B, s));
     }
-    if (!ctx.dry && !fused_up && !comb_up) SVCB_TRY(launch_ups_finalize(fp, B, s));
-    if (comb_up) {
-      // (noise conv already inside the combined convolution)
-    } else if (!fuse_noise && c.precision != 0 && us.noise_tc.tc && sf <= 2 * SRC_PADF && !last) {
+    if (us.noise_form == NOISE_TC) {
       // long noise filter as Conv1d(sf -> C, K=2) over the space-to-depth view of the padded source:
       // x[b, ci, t] = srcp[b][32 - sf/2 + sf*t + ci]
-      const ConvW& w = us.noise_tc;
-      ConvTcParams q;
-      q.x = SRCP + (SRC_PADF - sf / 2); q.sxb = Lpad; q.sxc = 1; q.sxt = sf;
-      q.wpk = w.tc; q.bias = w.b; q.y = X;
-      q.B = B; q.Cin = sf; q.cin_pad = w.cin_pad; q.Cout = chn; q.Tin = Ln + 1; q.Tout = Ln;
-      q.K = 2; q.dil = 1; q.pad = 0; q.kch = w.kch; q.bn = w.bn; q.ntiles = w.ntiles;
-      q.nsplit = c.precision == 1 ? 1 : 3; q.flags = CONV_ACCUM;
+      ConvTcParams q = conv_tc_params(us.noise_tc, SRCP + (SRC_PADF - sf / 2), Lpad, 1, sf, X, B, Ln + 1, Ln, 1, 0, nsplit);
+      q.flags = CONV_ACCUM;
       RUN(launch_conv_tc(q, s));
-    } else if (!fuse_noise) {  // long noise filters (K = 2*prod(later rates)): separate accumulate pass
-      ConvParams p;
-      p.x = source; p.sxb = Ltot; p.sxc = Ltot; p.sxt = 1;
-      p.w = us.noise.w; p.cout_pad = us.noise.cout_pad; p.bias = us.noise.b;
-      p.y = X; p.syb = (long long)chn * Ln; p.syc = Ln; p.syt = 1;
-      p.B = B; p.Cin = 1; p.Cout = chn; p.Tin = (int)Ltot;
-      p.K = us.noise.k; p.stride = last ? 1 : sf; p.dil = 1; p.pad = last ? 0 : sf / 2;
-      p.q0 = 0; p.nq = Ln; p.flags = CONV_ACCUM;
+    } else if (us.noise_form == NOISE_CONV1D) {  // long noise filters (K = 2*prod(later rates)): separate accumulate pass
+      ConvParams p = std_conv(us.noise, source, X, B, (int)Ltot, Ln, sf / 2, 1, sf);
+      p.flags = CONV_ACCUM;
       RUN(launch_conv1d(p, s));
     }
     SVCB_TRY(tap(ctx, SVCB_TAP_GEN_UP0 + i, X, (size_t)B * chn * Ln));
-    void* S2D[4] = {nullptr, nullptr, nullptr, nullptr};
-    const int s2r = c.precision == 3 ? s2d_link_factor(chn) : 0;
-    if (s2r && Ln % s2r == 0 && Ln % 8 == 0) {
+
+    const ResBlock* rb = &m->res[(size_t)i * c.n_res];
+    AmpStage a{X, ACC, T1, T2, RA, RB, IMG_HI, IMG_LO, {nullptr, nullptr, nullptr, nullptr}, B, chn, Ln, c.n_res, nsplit};
+    // every block of a stage has the same channel count, so either all or none take the s2d form
+    const bool s2d = rb[0].form == AMP_S2D && Ln % rb[0].s2d_r == 0 && Ln % 8 == 0;
+    const size_t mark = ctx.off;
+    if (s2d) {
       // two ping-pong S2D images (hi, lo each), cleared once per stage: rows outside the sequences are the
       // convolutions' zero padding and are never written by the link kernels
-      const size_t ib = s2d_image_bytes(B, Ln, s2r);
-      const size_t mark = ctx.off;
+      const size_t ib = s2d_image_bytes(B, Ln, rb[0].s2d_r);
       uint8_t* base = ctx.alloc<uint8_t>(4 * ib);
       SVCB_TRY(check_ws(ctx));
-      for (int q = 0; q < 4; ++q) S2D[q] = base + (size_t)q * ib;
+      for (int q = 0; q < 4; ++q) a.s2d[q] = base + (size_t)q * ib;
       if (!ctx.dry) {
         KernelScope ks("s2d_image_clear", s, 0.0, 4.0 * ib);
         SVCB_CUDA_CHECK(cudaMemsetAsync(base, 0, 4 * ib, s));
       }
-      SVCB_TRY(run_amp_stage(m, ctx, i, X, ACC, T1, T2, RA, RB, IMG_HI, IMG_LO, S2D, B, chn, Ln));
-      ctx.off = mark;
-    } else {
-      SVCB_TRY(run_amp_stage(m, ctx, i, X, ACC, T1, T2, RA, RB, IMG_HI, IMG_LO, S2D, B, chn, Ln));
     }
+    for (int j = 0; j < c.n_res; ++j) {
+      const ResBlock& R = rb[j];
+      switch (s2d ? R.form : R.fallback) {
+        case AMP_S2D: SVCB_TRY(run_amp_s2d(ctx, a, R, j)); break;
+        case AMP_BLOCK_FUSED: SVCB_TRY(run_amp_block_fused(ctx, a, R, j)); break;
+        case AMP_TC: SVCB_TRY(run_amp_tc(ctx, a, R, j)); break;
+        case AMP_FP32: SVCB_TRY(run_amp_fp32(ctx, a, R, j)); break;
+      }
+    }
+    ctx.off = mark;
     SVCB_TRY(tap(ctx, SVCB_TAP_GEN_STAGE0 + i, ACC, (size_t)B * chn * Ln));
     x = ACC; ch = chn; L = Ln;
   }
@@ -663,19 +654,35 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
 }
 
 // ----------------------------------------------------------------------------- model creation
-struct Resolver {
-  const svcb_model* m;
-  bool ok = true;
-  std::string missing;
-  const float* get(const std::string& name, uint64_t min_numel = 0) {
-    auto it = m->tensors.find(name);
-    if (it == m->tensors.end() || it->second.second < min_numel) {
-      if (ok) missing = name;
-      ok = false;
-      return nullptr;
-    }
-    return it->second.first;
+int check_blob_device(const void* dev_blob) {
+  if (((uintptr_t)dev_blob & 255) != 0) { set_error("weight blob must be 256-byte aligned"); return SVCB_E_BAD_ALIGN; }
+  int dev = 0;
+  SVCB_CUDA_CHECK(cudaGetDevice(&dev));
+  cudaDeviceProp prop;
+  SVCB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("libsvc_b200 is built for sm_90a only; device is sm_" + std::to_string(prop.major) +
+              std::to_string(prop.minor));
+    return SVCB_E_UNSUPPORTED;
   }
+  return SVCB_OK;
+}
+
+int BlobTensors::read(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table, int32_t n) {
+  const char* blob = static_cast<const char*>(dev_blob);
+  for (int i = 0; i < n; ++i) {
+    const svcb_tensor_entry& e = table[i];
+    const std::string name(e.name, strnlen(e.name, sizeof(e.name)));
+    if (e.offset_bytes % 256 != 0 || e.offset_bytes + e.numel * sizeof(float) > blob_bytes) {
+      set_error("bad table entry: " + name);
+      return SVCB_E_BAD_ALIGN;
+    }
+    map[name] = {reinterpret_cast<const float*>(blob + e.offset_bytes), e.numel};
+  }
+  return SVCB_OK;
+}
+
+struct Resolver : BlobTensors {
   ConvW conv(const std::string& prefix, int cin, int cout, int k, bool bias = true, bool tc = false) {
     ConvW w;
     w.cin = cin; w.cout = cout; w.k = k; w.cout_pad = (cout + 7) / 8 * 8;
@@ -694,16 +701,15 @@ struct Resolver {
     s.fu = get(prefix + ".fu", 12); s.fd = get(prefix + ".fd", 12);
     if (s.fu && s.fd && (cudaMemcpy(s.fu_h, s.fu, 12 * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
                          cudaMemcpy(s.fd_h, s.fd, 12 * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)) {
-      if (ok) missing = prefix + ".fu/.fd (device read-back failed)";
-      ok = false;
+      fail(prefix + ".fu/.fd (device read-back failed)");
     }
     return s;
   }
 };
 
-static int resolve(svcb_model* m) {
+static int resolve(svcb_model* m, Resolver& R) {
   const svcb_config& c = m->cfg;
-  Resolver R{m};
+  const bool tc = c.precision != 0;
   const int H = c.hidden_channels, C = c.inter_channels;
   m->pre = R.conv("enc_p.pre", c.ppg_dim, H, 5, true, true);
   m->hub = R.conv("enc_p.hub", c.vec_dim, H, 5, true, true);
@@ -751,17 +757,16 @@ static int resolve(svcb_model* m) {
     us.rate = c.up_rates[i]; us.k = c.up_kernels[i];
     us.pad = (us.k - us.rate) / 2;
     us.taps = (us.k + us.rate - 1) / us.rate;
+    for (int k2 = i + 1; k2 < c.n_ups; ++k2) us.sf *= c.up_rates[k2];
     m->hop *= us.rate;
     const std::string p = "dec.ups." + std::to_string(i);
     for (int r = 0; r < us.rate; ++r)
       us.phase.push_back(R.conv(p + ".ph" + std::to_string(r), ch, ch / 2, us.taps, false, true));
     us.bias = R.get(p + ".b", ch / 2);
     if (us.rate == 4 && us.taps == 2 && i + 1 < c.n_ups) {   // pack.py:UPS_COMBINED_RATES (+ the stage's noise conv)
-      int sfc = 1;
-      for (int k2 = i + 1; k2 < c.n_ups; ++k2) sfc *= c.up_rates[k2];
       ConvW& w = us.comb;
       us.comb_cin1 = (ch + 31) / 32 * 32;
-      us.comb_cin2 = us.rate * sfc + sfc;             // source samples a frame's rate outputs reach (filter 2 sf, stride sf)
+      us.comb_cin2 = us.rate * us.sf + us.sf;         // source samples a frame's rate outputs reach (filter 2 sf, stride sf)
       w.cin = us.comb_cin1 + us.comb_cin2; w.cout = us.rate * (ch / 2); w.k = us.taps + 1; w.cout_pad = (w.cout + 7) / 8 * 8;
       tc_tiling(w);
       w.tc = reinterpret_cast<const uint8_t*>(R.get(p + ".comb.tc", (uint64_t)w.k * 2 * w.cin_pad * w.ntiles * w.bn / 2));
@@ -771,18 +776,30 @@ static int resolve(svcb_model* m) {
   }
   ch = c.gen_initial_channel;
   for (int i = 0; i < c.n_ups; ++i) {
-    int sf = 1;
-    for (int k2 = i + 1; k2 < c.n_ups; ++k2) sf *= c.up_rates[k2];
+    UpStage& us = m->ups[i];
+    const int sf = us.sf;
     const int nk = (i + 1 == c.n_ups) ? 1 : 2 * sf;
-    m->ups[i].noise = R.conv("dec.noise." + std::to_string(i), 1, ch / 2, nk);
+    us.noise = R.conv("dec.noise." + std::to_string(i), 1, ch / 2, nk);
     if (nk > 8) {
-      ConvW& w = m->ups[i].noise_tc;
+      ConvW& w = us.noise_tc;
       w.cin = sf; w.cout = ch / 2; w.k = 2; w.cout_pad = (w.cout + 7) / 8 * 8;
       tc_tiling(w);
       w.tc = reinterpret_cast<const uint8_t*>(
           R.get("dec.noise." + std::to_string(i) + ".tc", (uint64_t)2 * 2 * w.cin_pad * w.ntiles * w.bn / 2));
-      w.b = m->ups[i].noise.b;
+      w.b = us.noise.b;
     }
+    // the stage's kernels (comb and noise_tc exist only for stages before the last)
+    if (tc && nk <= 8 && ups_fused_supported(ch, ch / 2, us.rate, us.taps, nk)) us.form = UPS_FUSED;
+    else if (tc && us.comb.tc && sf / 2 <= SRC_PADF) us.form = UPS_COMB;
+    else us.form = UPS_POLYPHASE;
+    // phase r's outputs start at q0 (independent of L); with pad >= 0 it has exactly L of them, a stride-1 conv
+    for (int r = 0; r < us.rate; ++r) {
+      const int q0 = us.pad - r > 0 ? (us.pad - r + us.rate - 1) / us.rate : 0;
+      us.phase_tc.push_back(tc && us.phase[r].tc && us.pad >= 0 && us.taps - 1 - q0 >= 0);
+    }
+    if (us.form != UPS_POLYPHASE || nk <= 8) us.noise_form = NOISE_IN_UPS;
+    else if (tc && us.noise_tc.tc && sf <= 2 * SRC_PADF) us.noise_form = NOISE_TC;
+    else us.noise_form = NOISE_CONV1D;
     ch /= 2;
   }
   m->res.resize((size_t)c.n_ups * c.n_res);
@@ -811,14 +828,13 @@ static int resolve(svcb_model* m) {
         rb.c2_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c2." + std::to_string(d) + ".s2d", per_tap * rb.s2d_nt2[d]));
       }
       for (int a = 0; a < 6; ++a) rb.act[a] = R.snake(p + ".act." + std::to_string(a), ch);
+      rb.fallback = !tc ? AMP_FP32 : amp_block_fused_supported(ch, rb.k, rb.dil) ? AMP_BLOCK_FUSED : AMP_TC;
+      rb.form = c.precision == 3 && rb.s2d_r ? AMP_S2D : rb.fallback;
     }
   }
   m->post_act = R.snake("dec.post.act", ch);
   m->conv_post = R.conv("dec.conv_post", ch, 1, 7, false);
-  if (!R.ok) {
-    set_error("tensor missing or too small in packed blob: " + R.missing);
-    return SVCB_E_MISSING_TENSOR;
-  }
+  SVCB_TRY(R.status("packed blob"));
   {  // packed [cin][k][cout_pad]: keep output channel 0 of every tap on the host
     const ConvW& w = m->conv_post;
     std::vector<float> packed((size_t)w.cin * w.k * w.cout_pad);
@@ -899,34 +915,14 @@ const char* svcb_timing_report(void) {
 int svcb_model_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table_host,
                       int32_t n_entries, const svcb_config* cfg_host, svcb_model** out) {
   if (!dev_blob || !table_host || !cfg_host || !out) { set_error("null argument"); return SVCB_E_BAD_SHAPE; }
-  if (((uintptr_t)dev_blob & 255) != 0) { set_error("weight blob must be 256-byte aligned"); return SVCB_E_BAD_ALIGN; }
-  int dev = 0;
-  SVCB_CUDA_CHECK(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  SVCB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 9 || prop.minor != 0) {
-    set_error("libsvc_b200 is built for sm_90a only; device is sm_" + std::to_string(prop.major) +
-              std::to_string(prop.minor));
-    return SVCB_E_UNSUPPORTED;
-  }
+  SVCB_TRY(check_blob_device(dev_blob));
   SVCB_TRY(validate_cfg(*cfg_host));
-  svcb_model* m = new svcb_model();
+  Resolver R;
+  SVCB_TRY(R.read(dev_blob, blob_bytes, table_host, n_entries));
+  auto m = std::make_unique<svcb_model>();
   m->cfg = *cfg_host;
-  m->blob = static_cast<const char*>(dev_blob);
-  m->blob_bytes = blob_bytes;
-  for (int i = 0; i < n_entries; ++i) {
-    const svcb_tensor_entry& e = table_host[i];
-    if (e.offset_bytes % 256 != 0 || e.offset_bytes + e.numel * sizeof(float) > blob_bytes) {
-      set_error(std::string("bad table entry: ") + e.name);
-      delete m;
-      return SVCB_E_BAD_ALIGN;
-    }
-    std::string nm(e.name, strnlen(e.name, sizeof(e.name)));
-    m->tensors[nm] = {reinterpret_cast<const float*>(m->blob + e.offset_bytes), e.numel};
-  }
-  const int st = resolve(m);
-  if (st != SVCB_OK) { delete m; return st; }
-  *out = m;
+  SVCB_TRY(resolve(m.get(), R));
+  *out = m.release();
   return SVCB_OK;
 }
 
@@ -1047,15 +1043,10 @@ int svcb_op_conv_tc(const float* x, const void* w_tc, const float* bias, float* 
                     const int64_t* lengths, int32_t B, int32_t Cin, int32_t Cout, int32_t T, int32_t K,
                     int32_t dilation, int32_t nsplit, int32_t flags, int32_t act, svcb_stream stream) {
   g_launches = 0;
-  ConvW w; w.cin = Cin; w.cout = Cout; w.k = K;
+  ConvW w; w.cin = Cin; w.cout = Cout; w.k = K; w.tc = static_cast<const uint8_t*>(w_tc); w.b = bias;
   tc_tiling(w);
-  ConvTcParams q;
-  q.x = x; q.sxb = (long long)Cin * T; q.sxc = T; q.sxt = 1;
-  q.wpk = static_cast<const uint8_t*>(w_tc); q.bias = bias; q.y = y; q.res = res;
-  q.lengths = reinterpret_cast<const long long*>(lengths);
-  q.B = B; q.Cin = Cin; q.cin_pad = w.cin_pad; q.Cout = Cout; q.Tin = T; q.Tout = T;
-  q.K = K; q.dil = dilation; q.pad = dilation * (K - 1) / 2; q.kch = w.kch; q.bn = w.bn; q.ntiles = w.ntiles;
-  q.nsplit = nsplit; q.flags = flags; q.act = act;
+  ConvTcParams q = conv_tc_params(w, x, (long long)Cin * T, T, 1, y, B, T, T, dilation, dilation * (K - 1) / 2, nsplit);
+  q.res = res; q.lengths = reinterpret_cast<const long long*>(lengths); q.flags = flags; q.act = act;
   return launch_conv_tc(q, static_cast<cudaStream_t>(stream));
 }
 
@@ -1081,8 +1072,6 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
   q.B = B; q.C = C; q.Cp = (C + 15) / 16 * 16; q.L = L; q.K = K; q.dil = dilation; q.nsplit = nsplit;
   return launch_amp_conv_tc(q, s);
 }
-
-void svcb_debug_s2d_trace(void* dev_buf) { s2d_set_trace(static_cast<long long*>(dev_buf)); }
 
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L) {
   const int r = C > 0 ? 160 / C : 0;
@@ -1111,10 +1100,7 @@ int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_ac
   q.a_hi = b0; q.a_lo = b0 + img;
   if (y_act) {
     q.o_hi = b0 + 2 * img; q.o_lo = b0 + 3 * img; q.ea = ea_out; q.ib = ib_out; q.fu = fu; q.fd = fd;
-    SnakeW taps;   // (a unit-test entry point: a synchronous read-back of the 24 taps is fine here)
-    SVCB_CUDA_CHECK(cudaMemcpy(taps.fu_h, fu, 12 * sizeof(float), cudaMemcpyDeviceToHost));
-    SVCB_CUDA_CHECK(cudaMemcpy(taps.fd_h, fd, 12 * sizeof(float), cudaMemcpyDeviceToHost));
-    snake_taps_to(taps, q);
+    SVCB_TRY(snake_taps_from_device(fu, fd, &q.taps));
   }
   q.wpk = static_cast<const uint8_t*>(w_s2d); q.bias = bias; q.res = res; q.y = y;
   s2d_taps(K, dilation, r, q.mlo, q.ntaps);

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <atomic>
+#include <map>
 #include <string>
 
 #include "svcb.h"
@@ -11,6 +12,32 @@ namespace svcb {
 
 void set_error(const std::string& msg);
 void count_launch();
+
+// Handle creation (svcb_model_create, svcb_whisper_create, svcb_hubert_create).
+// SVCB_E_BAD_ALIGN unless the blob is 256-byte aligned, SVCB_E_UNSUPPORTED unless the current device is sm_90.
+int check_blob_device(const void* dev_blob);
+// The named tensors of a packed weight blob.
+struct BlobTensors {
+  std::map<std::string, std::pair<const float*, uint64_t>> map;
+  bool ok = true;
+  std::string missing;   // the first name get() failed on
+  // SVCB_E_BAD_ALIGN for an entry that is not 256-byte aligned or runs past the blob's end
+  int read(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table, int32_t n);
+  void fail(const std::string& what) { if (ok) missing = what; ok = false; }
+  // the tensor, or null when it is missing or has fewer than min_numel elements
+  const float* get(const std::string& name, uint64_t min_numel = 0) {
+    auto it = map.find(name);
+    if (it != map.end() && it->second.second >= min_numel) return it->second.first;
+    fail(name);
+    return nullptr;
+  }
+  // SVCB_E_MISSING_TENSOR (with the first missing name) after a failed get()
+  int status(const char* blob_kind) const {
+    if (ok) return SVCB_OK;
+    set_error(std::string("tensor missing or too small in ") + blob_kind + ": " + missing);
+    return SVCB_E_MISSING_TENSOR;
+  }
+};
 
 // Optional per-kernel CUDA-event timing (svcb_timing_enable): a KernelScope brackets one launch
 // with two events on the launching stream and books its algorithmic FLOPs / bytes under `name`.
@@ -229,17 +256,13 @@ struct AmpS2dParams {
   const float* res = nullptr;   // residual [B, C, L] fp32 or null
   float* y = nullptr;           // fp32 result [B, C, L] or null
   const float *ea = nullptr, *ib = nullptr, *fu = nullptr, *fd = nullptr;   // Snake of the output image
-  float2 fup[6] = {}, fdp[5] = {};      // ... as pairs for the packed f32x2 FIRs: fup[i] = (fu2[11-2i], fu2[10-2i]),
-  float fd0 = 0.f, fd11 = 0.f;          //     fdp[i] = (fdn[2i+1], fdn[2i+2]); the two end taps of the decimator apart
-  float fu2[12] = {0}, fdn[12] = {0};   // the same taps BY VALUE (fu2 = 2 * up taps: UpSample1d's ratio gain folded,
-                                        // exact): kernel parameters live in the constant bank, so the FIR FMAs
-                                        // take them as operands and no register holds a tap
+  SnakeTapsV taps = {};         // ... its filter taps BY VALUE: kernel parameters live in the constant bank, so the
+                                // FIR FMAs take them as operands and no register holds a tap
   int B = 0, C = 0, L = 0, K = 0;   // K = taps of the original conv (bookkeeping only)
   int Rp = 0;                   // image rows per (item, octet) = s2d_rows(L, r)
   int ntaps = 0, mlo = 0;       // Toeplitz row offsets -mlo .. ntaps-1-mlo (pack.py:s2d_taps)
   int accum = 0;                // y = y_old + v
   float out_div = 0.f;          // then / out_div when != 0
-  long long* trace = nullptr;   // debugging: CTA 0 writes clock64() stamps of its first 32 tiles ([tile][16]) or null
 };
 // Head-major QKV layout the Whisper attention kernel reads (written by the QKV GEMM's epilogue 4): per item
 // b, per w in {q, k, v}, per head h one block of Tp x 64 bf16 (Tp = T rounded up to 128 rows, pad rows zero);
@@ -251,8 +274,6 @@ __host__ __device__ inline size_t qkv_heads_off(int b, int w, int h, int t, int 
   return w == 0 ? base + (size_t)(t >> 7) * 8192 + (size_t)(d >> 3) * 1024 + (size_t)(t & 127) * 8 + (d & 7)
                 : base + (size_t)(t >> 6) * 4096 + (size_t)(d >> 3) * 512 + (size_t)(t & 63) * 8 + (d & 7);
 }
-long long* s2d_get_trace();               // (the Whisper attention kernel writes its wait counters to the same buffer)
-void s2d_set_trace(long long* dev_buf);   // test hook: trace buffer used by the next launches (null = off)
 int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s);
 int launch_snake_pack_s2d(const float* x, void* hi, void* lo, const float* ea, const float* inv_b, const float* fu,
                           const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps = nullptr);
@@ -359,5 +380,20 @@ int launch_source(const float* f0, const float* rand_ini, const float* noise, co
                   int n_harm, float sampling_rate, cudaStream_t s);
 size_t source_scan_ws_bytes(int B, int T, int n_harm);
 int launch_source2wav(const float* src, int16_t* out, size_t n, cudaStream_t s);
+
+// ----------------------------------------------------------------------------- Whisper / HuBERT transformer kernels
+// bf16 wgmma GEMM over tile images with the fused epilogues listed in whisper_gemm.cu (GemmEpi)
+int launch_gemm_tc(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
+                   int M, int N, int K, int epi, cudaStream_t s, int res_mod = 0, int aux = 0);
+int launch_im2col_s1_image(const float* mel, void* img, int B, int n_mels, int n, cudaStream_t s);
+int launch_im2col_s2_image(const float* h1, void* img, int B, int D, int n, int n2, cudaStream_t s, int taps = 3, int pad = 1);
+int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s);
+int launch_rowmajor_to_image(const void* src, void* dst, int R, int K, int rows, cudaStream_t s);
+int launch_image_to_rowmajor(const void* src, void* dst, int R, int K, cudaStream_t s);
+int launch_qkv_rowmajor_to_heads(const void* src, void* dst, int B, int T, int D, cudaStream_t s);
+int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T, int D, int heads, int vswap, cudaStream_t s);
+// row LayerNorm of fp32 [M, D]: bf16 tile image (A operand of the next GEMM; y32 also gets the fp32 rows) or fp32 rows
+int launch_ln_rows(const float* x, const float* gamma, const float* beta, void* y, int M, int D, bool out_bf16,
+                   cudaStream_t s, float* y32 = nullptr);
 
 }  // namespace svcb

@@ -20,21 +20,13 @@
 
 #include <algorithm>
 #include <cstdint>
-#include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "common.cuh"
 
 namespace svcb {
-int launch_gemm_tc(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
-                   int M, int N, int K, int epi, cudaStream_t s, int res_mod = 0, int aux = 0);
-int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s);
-int launch_im2col_s2_image(const float* h1, void* img, int B, int D, int n, int n2, cudaStream_t s, int taps = 3, int pad = 1);
-int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T, int D, int heads, int vswap, cudaStream_t s);
-int launch_ln_rows(const float* x, const float* gamma, const float* beta, void* y, int M, int D, bool out_bf16,
-                   cudaStream_t s, float* y32 = nullptr);
-
 constexpr int HB_C = 512, HB_D = 768, HB_H = 12, HB_FF = 3072, HB_OUT = 256, HB_PK = 128, HB_PG = 16, HB_PHALF = 24;
 static const int kHbKernels[6] = {3, 3, 3, 3, 2, 2};
 
@@ -210,7 +202,6 @@ using namespace svcb;
 
 struct svcb_hubert {
   int n_layer = 0;
-  std::map<std::string, std::pair<const float*, uint64_t>> tensors;
   const float *conv0_w, *gn_g, *gn_b, *conv_w[6], *conv_wimg[6], *fp_lng, *fp_lnb, *fp_w, *fp_b, *pos_w[HB_PG][2], *pos_b, *pos_wimg[HB_PG], *pos_bimg[HB_PG], *norm_g, *norm_b,
       *proj_w, *proj_b;
   std::vector<HLayer> layers;
@@ -221,63 +212,43 @@ extern "C" {
 int svcb_hubert_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table_host, int32_t n_entries,
                        int32_t n_layer, svcb_hubert** out) {
   if (!dev_blob || !table_host || !out || n_layer < 1 || n_layer > 64) { set_error("svcb_hubert_create: bad argument"); return SVCB_E_BAD_SHAPE; }
-  if (((uintptr_t)dev_blob & 255) != 0) { set_error("weight blob must be 256-byte aligned"); return SVCB_E_BAD_ALIGN; }
-  int dev = 0;
-  SVCB_CUDA_CHECK(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  SVCB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 9 || prop.minor != 0) { set_error("libsvc_b200 is built for sm_90a only"); return SVCB_E_UNSUPPORTED; }
-  svcb_hubert* h = new svcb_hubert();
+  SVCB_TRY(check_blob_device(dev_blob));
+  BlobTensors t;
+  SVCB_TRY(t.read(dev_blob, blob_bytes, table_host, n_entries));
+  auto h = std::make_unique<svcb_hubert>();
   h->n_layer = n_layer;
-  const char* blob = static_cast<const char*>(dev_blob);
-  for (int i = 0; i < n_entries; ++i) {
-    const svcb_tensor_entry& e = table_host[i];
-    if (e.offset_bytes % 256 != 0 || e.offset_bytes + e.numel * sizeof(float) > blob_bytes) {
-      set_error(std::string("bad table entry: ") + e.name);
-      delete h;
-      return SVCB_E_BAD_ALIGN;
-    }
-    h->tensors[std::string(e.name, strnlen(e.name, sizeof(e.name)))] = {reinterpret_cast<const float*>(blob + e.offset_bytes), e.numel};
-  }
-  bool ok = true;
-  std::string missing;
-  auto get = [&](const std::string& n, uint64_t min_numel) -> const float* {
-    auto it = h->tensors.find(n);
-    if (it == h->tensors.end() || it->second.second < min_numel) { if (ok) missing = n; ok = false; return nullptr; }
-    return it->second.first;
-  };
   const uint64_t C = HB_C, D = HB_D, FF = HB_FF;
-  h->conv0_w = get("fe.conv0.w", 10 * C);
-  h->gn_g = get("fe.gn.g", C); h->gn_b = get("fe.gn.b", C);
+  h->conv0_w = t.get("fe.conv0.w", 10 * C);
+  h->gn_g = t.get("fe.gn.g", C); h->gn_b = t.get("fe.gn.b", C);
   for (int i = 0; i < 6; ++i) {
-    h->conv_w[i] = get("fe.conv" + std::to_string(i + 1) + ".w", C * kHbKernels[i] * C);
-    h->conv_wimg[i] = get("fe.conv" + std::to_string(i + 1) + ".wimg", C * kHbKernels[i] * C / 2);
+    h->conv_w[i] = t.get("fe.conv" + std::to_string(i + 1) + ".w", C * kHbKernels[i] * C);
+    h->conv_wimg[i] = t.get("fe.conv" + std::to_string(i + 1) + ".wimg", C * kHbKernels[i] * C / 2);
   }
-  h->fp_lng = get("fp.ln.g", C); h->fp_lnb = get("fp.ln.b", C);
-  h->fp_w = get("fp.w", D * C / 2); h->fp_b = get("fp.b", D);
+  h->fp_lng = t.get("fp.ln.g", C); h->fp_lnb = t.get("fp.ln.b", C);
+  h->fp_w = t.get("fp.w", D * C / 2); h->fp_b = t.get("fp.b", D);
   for (int g = 0; g < HB_PG; ++g)
     for (int hf = 0; hf < 2; ++hf)
-      h->pos_w[g][hf] = get("pos." + std::to_string(g) + "." + std::to_string(hf) + ".w", (uint64_t)(D / HB_PG) * HB_PK * HB_PHALF);
+      h->pos_w[g][hf] = t.get("pos." + std::to_string(g) + "." + std::to_string(hf) + ".w", (uint64_t)(D / HB_PG) * HB_PK * HB_PHALF);
   for (int g = 0; g < HB_PG; ++g) {
-    h->pos_wimg[g] = get("pos." + std::to_string(g) + ".wimg", (uint64_t)256 * HB_PK * (D / HB_PG) / 2);
-    h->pos_bimg[g] = get("pos." + std::to_string(g) + ".bimg", 256);
+    h->pos_wimg[g] = t.get("pos." + std::to_string(g) + ".wimg", (uint64_t)256 * HB_PK * (D / HB_PG) / 2);
+    h->pos_bimg[g] = t.get("pos." + std::to_string(g) + ".bimg", 256);
   }
-  h->pos_b = get("pos.b", D);
-  h->norm_g = get("norm.g", D); h->norm_b = get("norm.b", D);
+  h->pos_b = t.get("pos.b", D);
+  h->norm_g = t.get("norm.g", D); h->norm_b = t.get("norm.b", D);
   h->layers.resize(n_layer);
   for (int i = 0; i < n_layer; ++i) {
     const std::string p = "L" + std::to_string(i);
     HLayer& l = h->layers[i];
-    l.wqkv = get(p + ".wqkv", 3 * D * D / 2); l.bqkv = get(p + ".bqkv", 3 * D);
-    l.wo = get(p + ".wo", D * D / 2); l.bo = get(p + ".bo", D);
-    l.w1 = get(p + ".w1", FF * D / 2); l.b1 = get(p + ".b1", FF);
-    l.w2 = get(p + ".w2", FF * D / 2); l.b2 = get(p + ".b2", D);
-    l.ln1g = get(p + ".ln1.g", D); l.ln1b = get(p + ".ln1.b", D);
-    l.ln2g = get(p + ".ln2.g", D); l.ln2b = get(p + ".ln2.b", D);
+    l.wqkv = t.get(p + ".wqkv", 3 * D * D / 2); l.bqkv = t.get(p + ".bqkv", 3 * D);
+    l.wo = t.get(p + ".wo", D * D / 2); l.bo = t.get(p + ".bo", D);
+    l.w1 = t.get(p + ".w1", FF * D / 2); l.b1 = t.get(p + ".b1", FF);
+    l.w2 = t.get(p + ".w2", FF * D / 2); l.b2 = t.get(p + ".b2", D);
+    l.ln1g = t.get(p + ".ln1.g", D); l.ln1b = t.get(p + ".ln1.b", D);
+    l.ln2g = t.get(p + ".ln2.g", D); l.ln2b = t.get(p + ".ln2.b", D);
   }
-  h->proj_w = get("proj.w", (uint64_t)HB_OUT * D / 2); h->proj_b = get("proj.b", HB_OUT);
-  if (!ok) { set_error("tensor missing or too small in hubert blob: " + missing); delete h; return SVCB_E_MISSING_TENSOR; }
-  *out = h;
+  h->proj_w = t.get("proj.w", (uint64_t)HB_OUT * D / 2); h->proj_b = t.get("proj.b", HB_OUT);
+  SVCB_TRY(t.status("hubert blob"));
+  *out = h.release();
   return SVCB_OK;
 }
 

@@ -3,27 +3,13 @@
 //   conv1+GELU (GEMM over an im2col image of the log-mel; its epilogue scatters into conv2's im2col image) ->
 //   conv2(stride 2)+GELU+pos-emb (GEMM) -> n_layer x { LN -> QKV GEMM (head-major panels) -> wgmma attention
 //   (whisper_attn_tc.cu) -> out-proj GEMM (+residual) -> LN -> MLP GEMM+GELU -> MLP GEMM (+residual) } -> ln_post
-#include <algorithm>
-#include <cstring>
-#include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "common.cuh"
 
 namespace svcb {
-int launch_gemm_tc(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
-                   int M, int N, int K, int epi, cudaStream_t s, int res_mod = 0, int aux = 0);
-int launch_im2col_s1_image(const float* mel, void* img, int B, int n_mels, int n, cudaStream_t s);
-int launch_im2col_s2_image(const float* h1, void* img, int B, int D, int n, int n2, cudaStream_t s, int taps = 3, int pad = 1);
-int launch_whisper_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int D, int heads, int img,
-                             cudaStream_t s);
-int launch_rowmajor_to_image(const void* src, void* dst, int R, int K, int rows, cudaStream_t s);
-int launch_image_to_rowmajor(const void* src, void* dst, int R, int K, cudaStream_t s);
-int launch_qkv_rowmajor_to_heads(const void* src, void* dst, int B, int T, int D, cudaStream_t s);
-int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T, int D, int heads, int vswap, cudaStream_t s);
-int launch_ln_rows(const float* x, const float* gamma, const float* beta, void* y, int M, int D, bool out_bf16,
-                   cudaStream_t s, float* y32 = nullptr);
 struct WBlock {
   const float *ln1g, *ln1b, *ln2g, *ln2b, *bqkv, *bo, *b1, *b2;
   const void *wqkv, *wo, *w1, *w2;
@@ -32,7 +18,6 @@ struct WBlock {
 
 struct svcb_whisper {
   svcb_whisper_config cfg;
-  std::map<std::string, std::pair<const float*, uint64_t>> tensors;
   const float *conv1_wimg, *conv1_b, *conv2_wimg, *conv2_b, *pos, *lnp_g, *lnp_b;
   std::vector<svcb::WBlock> blocks;
 };
@@ -69,55 +54,34 @@ extern "C" {
 int svcb_whisper_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table_host,
                         int32_t n_entries, const svcb_whisper_config* cfg_host, svcb_whisper** out) {
   if (!dev_blob || !table_host || !cfg_host || !out) { set_error("null argument"); return SVCB_E_BAD_SHAPE; }
-  if (((uintptr_t)dev_blob & 255) != 0) { set_error("weight blob must be 256-byte aligned"); return SVCB_E_BAD_ALIGN; }
+  SVCB_TRY(check_blob_device(dev_blob));
   const svcb_whisper_config& c = *cfg_host;
   if (c.n_state % 256 || c.n_state / c.n_head != 64 || c.n_layer < 1 || c.n_state > 2048) {
     set_error("whisper config: n_state must be a multiple of 256 (<= 2048) with 64-wide heads");
     return SVCB_E_UNSUPPORTED;
   }
-  int dev = 0;
-  SVCB_CUDA_CHECK(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  SVCB_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 9 || prop.minor != 0) { set_error("libsvc_b200 is built for sm_90a only"); return SVCB_E_UNSUPPORTED; }
-  svcb_whisper* w = new svcb_whisper();
+  BlobTensors t;
+  SVCB_TRY(t.read(dev_blob, blob_bytes, table_host, n_entries));
+  auto w = std::make_unique<svcb_whisper>();
   w->cfg = c;
-  const char* blob = static_cast<const char*>(dev_blob);
-  for (int i = 0; i < n_entries; ++i) {
-    const svcb_tensor_entry& e = table_host[i];
-    if (e.offset_bytes % 256 != 0 || e.offset_bytes + e.numel * sizeof(float) > blob_bytes) {
-      set_error(std::string("bad table entry: ") + e.name);
-      delete w;
-      return SVCB_E_BAD_ALIGN;
-    }
-    w->tensors[std::string(e.name, strnlen(e.name, sizeof(e.name)))] = {
-        reinterpret_cast<const float*>(blob + e.offset_bytes), e.numel};
-  }
-  bool ok = true;
-  std::string missing;
-  auto get = [&](const std::string& n, uint64_t min_numel) -> const float* {
-    auto it = w->tensors.find(n);
-    if (it == w->tensors.end() || it->second.second < min_numel) { if (ok) missing = n; ok = false; return nullptr; }
-    return it->second.first;
-  };
   const uint64_t D = c.n_state;
-  w->conv1_wimg = get("conv1.wimg", D * ((3 * (uint64_t)c.n_mels + 63) / 64 * 64) / 2); w->conv1_b = get("conv1.b", D);
-  w->conv2_wimg = get("conv2.wimg", D * 3 * D / 2); w->conv2_b = get("conv2.b", D);
-  w->pos = get("pos", (uint64_t)c.n_ctx * D);
-  w->lnp_g = get("ln_post.g", D); w->lnp_b = get("ln_post.b", D);
+  w->conv1_wimg = t.get("conv1.wimg", D * ((3 * (uint64_t)c.n_mels + 63) / 64 * 64) / 2); w->conv1_b = t.get("conv1.b", D);
+  w->conv2_wimg = t.get("conv2.wimg", D * 3 * D / 2); w->conv2_b = t.get("conv2.b", D);
+  w->pos = t.get("pos", (uint64_t)c.n_ctx * D);
+  w->lnp_g = t.get("ln_post.g", D); w->lnp_b = t.get("ln_post.b", D);
   w->blocks.resize(c.n_layer);
   for (int i = 0; i < c.n_layer; ++i) {
     const std::string p = "blk." + std::to_string(i);
     WBlock& b = w->blocks[i];
-    b.ln1g = get(p + ".ln1.g", D); b.ln1b = get(p + ".ln1.b", D);
-    b.ln2g = get(p + ".ln2.g", D); b.ln2b = get(p + ".ln2.b", D);
-    b.wqkv = get(p + ".wqkv", 3 * D * D / 2); b.bqkv = get(p + ".bqkv", 3 * D);
-    b.wo = get(p + ".wo", D * D / 2); b.bo = get(p + ".bo", D);
-    b.w1 = get(p + ".w1", 4 * D * D / 2); b.b1 = get(p + ".b1", 4 * D);
-    b.w2 = get(p + ".w2", 4 * D * D / 2); b.b2 = get(p + ".b2", D);
+    b.ln1g = t.get(p + ".ln1.g", D); b.ln1b = t.get(p + ".ln1.b", D);
+    b.ln2g = t.get(p + ".ln2.g", D); b.ln2b = t.get(p + ".ln2.b", D);
+    b.wqkv = t.get(p + ".wqkv", 3 * D * D / 2); b.bqkv = t.get(p + ".bqkv", 3 * D);
+    b.wo = t.get(p + ".wo", D * D / 2); b.bo = t.get(p + ".bo", D);
+    b.w1 = t.get(p + ".w1", 4 * D * D / 2); b.b1 = t.get(p + ".b1", 4 * D);
+    b.w2 = t.get(p + ".w2", 4 * D * D / 2); b.b2 = t.get(p + ".b2", D);
   }
-  if (!ok) { set_error("tensor missing or too small in whisper blob: " + missing); delete w; return SVCB_E_MISSING_TENSOR; }
-  *out = w;
+  SVCB_TRY(t.status("whisper blob"));
+  *out = w.release();
   return SVCB_OK;
 }
 
@@ -214,11 +178,6 @@ int svcb_op_attention_tc_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, i
   SVCB_TRY(launch_qkv_rowmajor_to_heads(qkv_bf16, qimg, B, T, D, s));
   SVCB_TRY(launch_whisper_attention_tc(qimg, oimg, B, T, D, heads, v_layout, s));
   return launch_image_to_rowmajor(oimg, out_bf16, (int)M, D, s);
-}
-
-int svcb_op_attention_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, int32_t T, int32_t D, int32_t heads,
-                           svcb_stream stream) {
-  return launch_whisper_attention(qkv_bf16, out_bf16, B, T, D, heads, 0, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -16,6 +16,7 @@
 //                     epilogue through a per-warpgroup shared-memory strip (64 columns at a time):
 //                     bias / GELU / residual -> stores (row-major bf16, tile-image bf16 for the next
 //                     GEMM, or fp32 residual stream)
+// The row LayerNorm that writes the GEMMs' A images (ln_rows) is at the end of this file.
 #include <algorithm>
 
 #include "common.cuh"
@@ -409,6 +410,92 @@ int launch_rowmajor_to_image(const void* src, void* dst, int R, int K, int rows,
   rowmajor_to_image_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(static_cast<const __nv_bfloat16*>(src),
                                                                        static_cast<__nv_bfloat16*>(dst), R, K, rows);
   SVCB_LAUNCH_CHECK("rowmajor_to_image");
+  return SVCB_OK;
+}
+
+__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+
+// Row LayerNorm over the last dim of fp32 [M, D] (nn.LayerNorm, eps 1e-5; whisper/model.py:28-31):
+// one warp per row, values held in registers, output bf16 (GEMM operand) or fp32 (ln_post).
+template <bool OUT_BF16>
+__global__ void __launch_bounds__(256)
+ln_rows_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+               void* __restrict__ y, float* __restrict__ y32, int M, int D, float eps) {
+  // bf16 output: the 8 rows of the block are staged in shared memory and leave as whole 128-byte lines of the tile
+  // image (8 rows x one 16-byte octet are contiguous there); lane-wise 8-byte stores into the image touched 16
+  // half-filled sectors per instruction and held the kernel at 2.2 TB/s
+  extern __shared__ __align__(16) uint8_t ln_stage[];
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const bool live = row < M;
+  if (!OUT_BF16 && !live) return;
+  const float* xr = x + (size_t)(live ? row : M - 1) * D;
+  const int srow = (D + 8) * 2;   // bytes per staged row (+16: conflict-free 16-byte reads down a column of rows)
+  constexpr int MAXV = 16;  // D <= 32*4*16 = 2048
+  float4 v[MAXV];
+  const int nv = D / 128;  // float4 per lane
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    if (i < nv) {
+      v[i] = *reinterpret_cast<const float4*>(xr + (size_t)(i * 32 + lane) * 4);
+      s += v[i].x + v[i].y + v[i].z + v[i].w;
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+  const float mean = s / (float)D;
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    if (i < nv) {
+      const float a = v[i].x - mean, b2 = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+      q += a * a + b2 * b2 + c * c + d * d;
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) q += __shfl_xor_sync(0xffffffffu, q, off);
+  const float rstd = 1.f / sqrtf(q / (float)D + eps);
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    if (i < nv) {
+      const int c0 = (i * 32 + lane) * 4;
+      const float4 gm = *reinterpret_cast<const float4*>(gamma + c0);
+      const float4 bt = *reinterpret_cast<const float4*>(beta + c0);
+      const float o0 = (v[i].x - mean) * rstd * gm.x + bt.x, o1 = (v[i].y - mean) * rstd * gm.y + bt.y;
+      const float o2 = (v[i].z - mean) * rstd * gm.z + bt.z, o3 = (v[i].w - mean) * rstd * gm.w + bt.w;
+      if (OUT_BF16) {  // GEMM tile image (A operand of the following linear layer), through the staging rows
+        // (+ the fp32 rows when the normalised values are also the residual stream: post-LN layers, HuBERT)
+        if (y32 && live) *reinterpret_cast<float4*>(y32 + (size_t)row * D + c0) = make_float4(o0, o1, o2, o3);
+        uint2 pk = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
+        *reinterpret_cast<uint2*>(ln_stage + (size_t)(threadIdx.x >> 5) * srow + (size_t)c0 * 2) = pk;
+      } else {
+        *reinterpret_cast<float4*>(static_cast<float*>(y) + (size_t)row * D + c0) = make_float4(o0, o1, o2, o3);
+      }
+    }
+  }
+  if (OUT_BF16) {
+    __syncthreads();
+    const int row0 = blockIdx.x * 8, noct = D / 8;
+    for (int idx = threadIdx.x; idx < noct * 8; idx += 256) {
+      const int o = idx >> 3, r = idx & 7;
+      if (row0 + r < M)
+        *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(y) + img_off(row0 + r, o * 8, D / 64)) =
+            *reinterpret_cast<const uint4*>(ln_stage + (size_t)r * srow + (size_t)o * 16);
+    }
+  }
+}
+
+// y32 (bf16 mode only, a buffer other than x): the same normalised rows in fp32 [M, D]
+int launch_ln_rows(const float* x, const float* gamma, const float* beta, void* y, int M, int D, bool out_bf16,
+                   cudaStream_t s, float* y32) {
+  if (D % 128 || D > 2048) { set_error("ln_rows: D must be a multiple of 128 and <= 2048"); return SVCB_E_UNSUPPORTED; }
+  KernelScope ks("ln_rows", s, 8.0 * M * (double)D, (out_bf16 ? (y32 ? 10.0 : 6.0) : 8.0) * M * (double)D);
+  if (out_bf16) ln_rows_kernel<true><<<(M + 7) / 8, 256, (size_t)8 * (D + 8) * 2, s>>>(x, gamma, beta, y, y32, M, D, 1e-5f);
+  else ln_rows_kernel<false><<<(M + 7) / 8, 256, 0, s>>>(x, gamma, beta, y, nullptr, M, D, 1e-5f);
+  SVCB_LAUNCH_CHECK("ln_rows");
   return SVCB_OK;
 }
 
