@@ -13,8 +13,8 @@
  *   - return 0 on success, <0 = svcb_status; svcb_last_error() gives a thread-local message;
  *   - a model handle is immutable after creation: concurrent calls on different streams
  *     are fine when their workspaces differ;
- *   - sm_90a only, no fallback: svcb_model_create, svcb_whisper_create and svcb_hubert_create fail
- *     with SVCB_E_UNSUPPORTED elsewhere.
+ *   - sm_90a only, no fallback: svcb_model_create, svcb_whisper_create, svcb_hubert_create and
+ *     svcb_ivf_create fail with SVCB_E_UNSUPPORTED elsewhere.
  */
 #ifndef SVCB_H_
 #define SVCB_H_
@@ -88,7 +88,7 @@ typedef struct {
 
 const char* svcb_last_error(void);
 int svcb_version(void);
-/* sizeof() of the ABI structs as compiled: 0 svcb_config, 1 svcb_tensor_entry, 2 svcb_taps
+/* sizeof() of the ABI structs as compiled: 0 svcb_config, 1 svcb_tensor_entry, 2 svcb_taps, 3 svcb_ivf_config
  * (lets a foreign-language binding verify its struct layout at load time). */
 size_t svcb_sizeof(int32_t which);
 
@@ -197,6 +197,32 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
 int svcb_whisper_log_mel(const float* audio, const float* mel_filters, const float* noise, float noise_gain,
                          float* mel, void* scratch, int32_t B, int32_t n_samples, int32_t n_mels,
                          svcb_stream stream);
+
+/* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
+/* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
+ * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */
+typedef struct {
+  int32_t d, nlist, nprobe, pad_;
+  int64_t ntotal;
+} svcb_ivf_config;   /* svcb_sizeof(3) */
+typedef struct svcb_ivf svcb_ivf;
+
+/* Replaces faiss.read_index of an IVF-Flat file (feature_retrieval/index.py:147-154).  Blob names/layouts:
+ * whisper-vits-svc_b200/retrieval.py:pack_ivf — "ivf.wimg" the centroids as a bf16 GEMM tile image
+ * [Np][3 d] = [-2 c_hi | -2 c_hi | -2 c_lo], Np = nlist rounded up to 256; "ivf.cnorm" [Np] |c|^2 (+inf past nlist);
+ * "ivf.vectors" [ntotal, d] fp32 in list order; "ivf.offsets" [nlist + 1] int32; "ivf.ids" [ntotal] int64. */
+int svcb_ivf_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table_host, int32_t n_entries,
+                    const svcb_ivf_config* cfg_host, svcb_ivf** out);
+void svcb_ivf_destroy(svcb_ivf* ix);
+size_t svcb_ivf_workspace_bytes(const svcb_ivf* ix, int32_t M, int32_t k);
+/* Replaces FaissRVCRetrievableFeatureIndex.retriv (feature_retrieval/index.py:57-62,75-94).
+ * x [M,d] fp32 row-major (16-byte aligned); out [M,d] (NULL = search only); dist [M,k] / ids [M,k] int64 optional
+ * (ascending; +inf / -1 where the probed lists hold fewer than k vectors).  1 <= k <= 32.
+ * out = (1 - ratio) x + ratio sum_i w_i v_i with w = (1/dist)^2 normalised, except: zero-distance neighbours share
+ * the weight equally; fewer than k found -> the blend runs over those found; none found -> out = x.
+ * Deterministic; a row's result does not depend on M or on its position. */
+int svcb_ivf_retrieve(const svcb_ivf* ix, const float* x, float* out, float* dist, int64_t* ids, int32_t M, int32_t k,
+                      float ratio, void* ws, size_t ws_bytes, svcb_stream stream);
 
 /* Operator entry points of the encoder (unit tests):
  * out[M,N] = A[M,K] . W[N,K]^T + bias with epilogue 0: bf16 row-major out, 1: GELU(erf) then bf16

@@ -7,9 +7,9 @@ Differences, by design (SURVEY.md §8 scope): the reference shells out to its Wh
 CREPE extractors when --ppg/--vec/--pit are missing (svc_inference.py:138-154).  Here --ppg and
 --vec are produced in-process by the H100 Whisper encoder / HuBERT-Soft encoder when their
 checkpoints are available (whisper_pretrain/large-v2.pt, hubert_pretrain/hubert-soft-0d54a1f4.pt);
-CREPE is out of scope (SURVEY.md §8f-4), so --pit must be given.  Feature retrieval
-(faiss, off by default in the reference) is not built; its flags are accepted and rejected with
-a clear message if enabled."""
+CREPE is out of scope (SURVEY.md §8f-4), so --pit must be given.  --enable-retrieval reads the
+reference's faiss IVF-Flat indexes without faiss and runs the search and blend on the device
+(whisper-vits-svc_b200/retrieval.py)."""
 import argparse
 import logging
 import os
@@ -20,14 +20,12 @@ import numpy as np
 import torch
 from scipy.io.wavfile import write
 
-from whisper_vits_svc_b200 import hostio, hparams, models
+from whisper_vits_svc_b200 import hostio, hparams, models, retrieval
 
 logger = logging.getLogger(__name__)
 
 
 def main(args):
-    if args.enable_retrieval:
-        raise SystemExit("feature retrieval (faiss) is outside the H100 hot path; run without --enable-retrieval")
     if args.pit is None:
         raise SystemExit("--pit is required: the CREPE pitch extractor is out of scope of this build "
                          "(use the reference's pitch/inference.py to produce it)")
@@ -51,12 +49,14 @@ def main(args):
     hp = hparams.load_hparams(args.config)
     model = models.SynthesizerInfer(hp.data.filter_length // 2 + 1, hp.data.segment_size // hp.data.hop_length, hp)
     hostio.load_svc_model(args.model, model)
+    retr = retrieval.create_retrival(args, hp, device)
     model.eval()
     model.to(device)
     spk = torch.FloatTensor(np.load(args.spk))
     print("pitch shift: ", args.shift)
     ppg, vec, pit = hostio.prepare_features(args.ppg, args.vec, args.pit, args.shift)
-    out_audio = hostio.svc_infer(model, spk, pit, ppg, vec, hp, device)
+    out_audio = hostio.svc_infer(model, spk, pit, ppg, vec, hp, device,
+                                 retrieval=None if isinstance(retr, retrieval.DummyRetrieval) else retr)
     write("svc_out.wav", hp.data.sampling_rate, out_audio)
 
 

@@ -61,6 +61,10 @@ class WhisperConfig(ctypes.Structure):
                 ("n_layer", c_int32)]
 
 
+class IvfConfig(ctypes.Structure):
+    _fields_ = [("d", c_int32), ("nlist", c_int32), ("nprobe", c_int32), ("pad_", c_int32), ("ntotal", c_int64)]
+
+
 class TensorEntry(ctypes.Structure):
     _fields_ = [("name", c_char * 96), ("offset_bytes", c_uint64), ("numel", c_uint64)]
 
@@ -85,6 +89,10 @@ SIGNATURES = {
     "svcb_hubert_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
     "svcb_hubert_units": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_int32, c_void_p]),
     "svcb_whisper_log_mel": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
+    "svcb_ivf_create": (c_int, [c_void_p, c_size_t, POINTER(TensorEntry), c_int32, POINTER(IvfConfig), POINTER(c_void_p)]),
+    "svcb_ivf_destroy": (None, [c_void_p]),
+    "svcb_ivf_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
+    "svcb_ivf_retrieve": (c_int, [c_void_p] * 5 + [c_int32, c_int32, c_float, c_void_p, c_size_t, c_void_p]),
     "svcb_op_gemm_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_gemm_bf16": (c_int, [c_void_p] * 5 + [c_int32] * 4 + [c_void_p, c_size_t, c_void_p]),
     "svcb_op_attention_tc_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
@@ -132,7 +140,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args
-    for which, st in enumerate((Config, TensorEntry, Taps)):
+    for which, st in enumerate((Config, TensorEntry, Taps, IvfConfig)):
         if lib.svcb_sizeof(which) != ctypes.sizeof(st):
             raise SvcbError(f"ABI struct {st.__name__} size mismatch: C {lib.svcb_sizeof(which)} vs ctypes {ctypes.sizeof(st)}")
     _lib = lib

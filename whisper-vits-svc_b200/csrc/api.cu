@@ -878,6 +878,7 @@ size_t svcb_sizeof(int32_t which) {
     case 0: return sizeof(svcb_config);
     case 1: return sizeof(svcb_tensor_entry);
     case 2: return sizeof(svcb_taps);
+    case 3: return sizeof(svcb_ivf_config);
     default: return 0;
   }
 }

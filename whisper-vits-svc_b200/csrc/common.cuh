@@ -396,4 +396,11 @@ int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T
 int launch_ln_rows(const float* x, const float* gamma, const float* beta, void* y, int M, int D, bool out_bf16,
                    cudaStream_t s, float* y32 = nullptr);
 
+// ----------------------------------------------------------------------------- IVF retrieval (csrc/retrieval_api.cu)
+// query rows x [M, d] fp32 -> the coarse search's A image [x_hi | x_lo | x_hi] ([ceil(M/128) * 128][3 d] bf16)
+int launch_ivf_pack(const float* x, void* img, int M, int d, cudaStream_t s);
+// gemm_tc epilogue 8 over that image and the centroid image: cand [M][N/16][nprobe] int2 {score bits, column}
+int launch_ivf_coarse_tc(const void* A_img, const void* W_img, const float* cnorm, void* cand, int M, int N, int K, int nprobe,
+                         cudaStream_t s);
+
 }  // namespace svcb

@@ -36,8 +36,11 @@ namespace svcb {
 //    A[b * Tn + t2][j * N + co] = h[b][co][2 t2 + j], Tn = (res_mod - aux) / 2 + 1 (every entry of the image is written)
 // 7: fp32 out[m * aux + col] = GELU(acc + bias) + res[m * aux + col] for the first res_mod columns only (aux = leading
 //    dimension of out / res): one group of HuBERT's grouped positional convolution, N padded from 48 to 256
+// 8: the IVF coarse search (csrc/retrieval_api.cu): f = acc + bias = |c|^2 - 2 x.c; each thread keeps the aux (= nprobe)
+//    smallest (score, column) pairs of its 16 columns, ties to the lower column, and writes them as int2 {score bits,
+//    column} to out[m][N / 16][aux] — the [M, N] score matrix is never stored
 enum GemmEpi : int { EPI_BF16_ROWMAJOR = 0, EPI_GELU_BF16_IMAGE = 1, EPI_RESID_F32 = 2, EPI_GELU_ADD_F32 = 3, EPI_QKV_HEADS = 4,
-                     EPI_GELU_CONV2_IMG = 5, EPI_GELU_VALID_S2_IMG = 6, EPI_GELU_ADD_F32_LD = 7 };
+                     EPI_GELU_CONV2_IMG = 5, EPI_GELU_VALID_S2_IMG = 6, EPI_GELU_ADD_F32_LD = 7, EPI_IVF_TOPK = 8 };
 
 constexpr int GM_BM = 128, GM_BK = 64, GM_STAGES = 3;
 constexpr int GM_EPI_LD = 72;   // floats per row of an epilogue strip (64 columns + 8: conflict-free fragment stores)
@@ -145,7 +148,25 @@ gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __re
 #pragma unroll
             for (int j = 0; j < 16; ++j) f[j] = 0.5f * f[j] * (1.f + erff(f[j] * 0.70710678118654752440f));
           }
-          if (EPI == EPI_GELU_ADD_F32_LD) {
+          if (EPI == EPI_IVF_TOPK) {
+            int2* o = static_cast<int2*>(out) + ((size_t)m * (N / 16) + (n0 + c0) / 16) * aux;
+            // aux passes of an arg-min over the columns not yet written, each re-reading the strip (f[] and v[] stay
+            // dead: the accumulators already hold most of the register file)
+            const float* sr = strip + (t & 63) * GM_EPI_LD + cl;
+            uint32_t taken = 0;
+#pragma unroll 1
+            for (int p = 0; p < aux; ++p) {
+              float bs = 0.f;
+              int bc = 16;
+#pragma unroll
+              for (int j = 0; j < 16; ++j) {
+                const float fj = sr[j] + __ldg(bias + n0 + c0 + j);
+                if (!((taken >> j) & 1u) && (bc == 16 || fj < bs)) { bs = fj; bc = j; }
+              }
+              taken |= 1u << bc;
+              o[p] = make_int2(__float_as_int(bs), n0 + c0 + bc);
+            }
+          } else if (EPI == EPI_GELU_ADD_F32_LD) {
             float* o = static_cast<float*>(out) + (size_t)m * aux;
             const float* rr = res + (size_t)m * aux;
 #pragma unroll
@@ -269,6 +290,69 @@ int launch_gemm_tc(const void* A_img, const void* W_img, const float* bias, void
   }
   set_error("gemm_tc: unknown epilogue");
   return SVCB_E_BAD_SHAPE;
+}
+
+// IVF coarse search (epilogue 8): cand[M][N/16][nprobe] int2 {score bits, column}, score = cnorm[col] - 2 x.c
+int launch_ivf_coarse_tc(const void* A_img, const void* W_img, const float* cnorm, void* cand, int M, int N, int K, int nprobe,
+                         cudaStream_t s) {
+  if (M <= 0) return SVCB_OK;
+  if (K % 64 || N % 256 || nprobe < 1 || nprobe > 8) { set_error("ivf_coarse_tc: need K % 64 == 0, N % 256 == 0, 1 <= nprobe <= 8"); return SVCB_E_BAD_SHAPE; }
+  constexpr size_t smem = (size_t)GM_STAGES * (GM_BM * GM_BK * 2 + 256 * GM_BK * 2) + 2 * 64 * GM_EPI_LD * 4;
+  static DevSmemCache attr_cache;
+  SVCB_CUDA_CHECK(ensure_dyn_smem(gemm_tc_kernel<256, EPI_IVF_TOPK>, smem, attr_cache));
+  const int n_sm = device_sm_count();
+  if (n_sm <= 0) { set_error("ivf_coarse_tc: cannot query the SM count"); return SVCB_E_CUDA; }
+  const int ntiles = ((M + GM_BM - 1) / GM_BM) * (N / 256);
+  // algorithmic FLOPs of the fp32 search (K = 3 d holds the three bf16 split products)
+  KernelScope ks("ivf_coarse_tc", s, 2.0 * M * (double)N * (K / 3),
+                 2.0 * ((double)M * K + (double)N * K) + 4.0 * N + 8.0 * M * (double)(N / 16) * nprobe);
+  gemm_tc_kernel<256, EPI_IVF_TOPK><<<std::min(ntiles, n_sm), GM_THREADS, smem, s>>>(
+      static_cast<const __nv_bfloat16*>(A_img), static_cast<const __nv_bfloat16*>(W_img), cnorm, cand, nullptr, M, N, K, 0, nprobe);
+  SVCB_LAUNCH_CHECK("ivf_coarse_tc");
+  return SVCB_OK;
+}
+
+// The coarse search's A operand: query rows x [M, d] fp32 -> bf16 tile image [ceil(M/128) * 128][3 d] holding
+// [x_hi | x_lo | x_hi] (x_hi = bf16(x), x_lo = bf16(x - x_hi)), rows past M zero.  With the centroid image
+// [-2 c_hi | -2 c_hi | -2 c_lo] one bf16 GEMM over K = 3 d gives -2 (x_hi c_hi + x_lo c_hi + x_hi c_lo): bf16x3.
+// Thread = one (row, octet of x), consecutive threads on consecutive rows: the image holds the octets of 128 rows
+// contiguously, so a warp's stores are 512 contiguous bytes (row-major threads spread them 2 KB apart).
+__global__ void __launch_bounds__(256)
+ivf_pack_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ img, int M, int Mp, int d) {
+  const int no = d / 8;
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)Mp * no) return;
+  const int o = (int)(idx / Mp), m = (int)(idx - (size_t)o * Mp), k = o * 8;
+  __align__(16) __nv_bfloat16 hi[8], lo[8];
+  if (m < M) {
+    const float4* s4 = reinterpret_cast<const float4*>(x + (size_t)m * d + k);
+    const float4 u0 = __ldg(s4), u1 = __ldg(s4 + 1);
+    const float v[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      hi[e] = __float2bfloat16_rn(v[e]);
+      lo[e] = __float2bfloat16_rn(v[e] - __bfloat162float(hi[e]));
+    }
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { hi[e] = __float2bfloat16_rn(0.f); lo[e] = hi[e]; }
+  }
+  const int KT = 3 * d / GM_BK;
+  const uint4 qh = *reinterpret_cast<const uint4*>(hi), ql = *reinterpret_cast<const uint4*>(lo);
+  *reinterpret_cast<uint4*>(img + img_off(m, k, KT)) = qh;
+  *reinterpret_cast<uint4*>(img + img_off(m, d + k, KT)) = ql;
+  *reinterpret_cast<uint4*>(img + img_off(m, 2 * d + k, KT)) = qh;
+}
+
+int launch_ivf_pack(const float* x, void* img, int M, int d, cudaStream_t s) {
+  if (M <= 0) return SVCB_OK;
+  if (d % 64) { set_error("ivf_pack: d must be a multiple of 64"); return SVCB_E_BAD_SHAPE; }
+  const int Mp = (M + GM_BM - 1) / GM_BM * GM_BM;
+  const size_t n = (size_t)Mp * (d / 8);
+  KernelScope ks("ivf_pack", s, 0.0, 4.0 * M * (double)d + 6.0 * Mp * (double)d);
+  ivf_pack_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, static_cast<__nv_bfloat16*>(img), M, Mp, d);
+  SVCB_LAUNCH_CHECK("ivf_pack");
+  return SVCB_OK;
 }
 
 // Stem conv2 (Conv1d(D, D, k=3, stride 2, pad 1), whisper/model.py:150) as a GEMM: this kernel builds

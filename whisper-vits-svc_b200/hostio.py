@@ -94,13 +94,17 @@ def chunk_plan(all_frame: int, hop_size: int, out_chunk: int = 2500, hop_frame: 
 
 
 def svc_infer(model, spk, pit, ppg, vec, hp, device, write_pit_wav: str | None = "svc_out_pit.wav",
-              rand_ini=None, noise=None, eps_fn=None, max_batch: int = 16):
+              rand_ini=None, noise=None, eps_fn=None, max_batch: int = 16, retrieval=None):
     """svc_inference.py:77-134.  Returns the float32 waveform as a numpy array of length
     n_frames*hop - 1 (the reference's last-chunk slice).  `rand_ini`/`noise` and
     `eps_fn(chunk_idx, 1, n_frames) -> [1, inter_channels, n_frames]` (one call per chunk) inject the
-    reference's random draws for parity tests."""
+    reference's random draws for parity tests.  `retrieval`: an object with `retriv_whisper` / `retriv_hubert`
+    (retrieval.py) or None.  The reference applies it per chunk (svc_inference.py:117-118); retrieval is row-wise,
+    so applying it once to the whole utterance gives the same rows."""
     len_min = min(pit.size(0), vec.size(0), ppg.size(0))
     pit, vec, ppg = pit[:len_min], vec[:len_min, :], ppg[:len_min, :]
+    if retrieval is not None:
+        ppg, vec = retrieval.retriv_whisper(ppg), retrieval.retriv_hubert(vec)
     hop = int(hp.data.hop_length)
     with torch.no_grad():
         spk = spk.unsqueeze(0).to(device)
