@@ -56,8 +56,8 @@ typedef struct {
   int32_t res_dilations[SVCB_MAX_RES][3];
   int32_t sampling_rate;
   int32_t n_harmonics;   /* 11 = fundamental + 10 overtones (vits_decoder/nsf.py:368) */
-  int32_t precision;     /* AMP-block convs: 0 = fp32 CUDA cores, 3 = bf16x3 split wgmma MMA
-                          * (parity grade), 1 = plain bf16 wgmma MMA */
+  int32_t precision;     /* convs and prior attention: 0 = fp32 CUDA cores, 3 = bf16x3 split wgmma MMA (parity
+                          * grade), 1 = plain bf16 wgmma MMA; other values: SVCB_E_UNSUPPORTED at create */
 } svcb_config;
 
 /* One named tensor inside the packed weight blob (host-side table, read at create time). */

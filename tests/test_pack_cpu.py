@@ -21,7 +21,7 @@ def test_pack_conv_roundtrip():
 @pytest.mark.parametrize("k,s", [(15, 5), (8, 4), (4, 2), (7, 3), (16, 8)])
 def test_polyphase_transposed_conv(k, s):
     """ConvTranspose1d == `rate` stride-1 sub-convolutions written with output stride `rate`
-    (csrc/api.cu run_generator uses exactly these q0 / nq / out_off formulas)."""
+    (csrc/api.cu run_generator uses exactly these q0 / nq formulas; phase r writes output q at q - q0)."""
     torch.manual_seed(k * 10 + s)
     cin, cout, T = 6, 4, 23
     w = torch.randn(cin, cout, k)
@@ -115,6 +115,17 @@ def test_packed_model_tensor_inventory(hp, sd):
     assert torch.equal(blob[off // 4: off // 4 + n], items[name].reshape(-1))
 
 
+def test_last_stage_of_rate_4_has_no_combined_image(hp):
+    """The combined up-sampler image (pack.ups_combined) carries the noise conv of a stage before the last; the last
+    stage's noise conv has kernel 1, so a last stage of rate 4 and kernel 8 packs without `comb` tensors."""
+    from whisper_vits_svc_b200 import hparams, synth
+    hpx = hparams.override(hp, gen__upsample_rates=[4, 4], gen__upsample_kernel_sizes=[8, 8],
+                           gen__upsample_initial_channel=64)
+    names = [n for n, _ in pack.pack_svc_state_dict(synth.svc_state_dict(hpx, 7), pack.config_from_hp(hpx))]
+    assert "dec.ups.0.comb.tc" in names and "dec.ups.0.comb.b" in names
+    assert not any(n.startswith("dec.ups.1.comb") for n in names)
+
+
 def test_whisper_conv2_weight_image_layout():
     """The stem's stride-2 conv runs as a GEMM over an im2col image (csrc/whisper_gemm.cu:
     im2col_s2_image): its weight must reach the kernel as W2[co][j*D + ci] = w[co][ci][j] in the bf16
@@ -160,8 +171,8 @@ def test_stem_conv2_im2col_equivalence():
     assert torch.allclose(got, ref, atol=1e-4)
 
 
-@pytest.mark.parametrize("C,k,dil", [(20, 3, 1), (20, 7, 3), (20, 11, 5), (10, 11, 5), (10, 3, 3), (40, 7, 5)])
-def test_conv_s2d_matrices_are_the_dilated_conv(C, k, dil):
+@pytest.mark.parametrize("C,k,dil", [(20, 3, 1), (20, 7, 3), (20, 11, 5), (10, 11, 5), (10, 3, 3), (40, 7, 5), (40, 11, 5)])
+def test_conv_s2d_image_is_the_dilated_conv(C, k, dil):
     """csrc/amp_s2d.cu multiplies rows of r consecutive samples (all channels) by block-Toeplitz matrices:
     sum over row offsets m of X'[tau + m] @ W_m^T must equal F.conv1d(x, w, dilation, 'same') — checked
     through the packed bf16 hi/lo image (hi + lo reproduces fp32 weights to ~2^-16 relative)."""
@@ -176,9 +187,7 @@ def test_conv_s2d_matrices_are_the_dilated_conv(C, k, dil):
     mlo, mhi = pack.s2d_taps(k, dil, r)
     P = dil * (k - 1) // 2
     assert mlo == -(-P // r) and mhi == (r - 1 + P) // r and mlo <= 8 and mhi <= 8   # fits the kernel's A panel
-    packed = pack.pack_conv_s2d(w, dil, r).view(pack.S2D_REPLICAS, -1)
-    assert all(torch.equal(packed[0], packed[i]) for i in range(1, pack.S2D_REPLICAS))   # replicas for L2 spreading
-    img = packed[0].contiguous().view(torch.bfloat16).view(mlo + mhi + 1, 2, 20, 160, 8).float()
+    img = pack.pack_conv_s2d(w, dil, r).view(torch.bfloat16).view(mlo + mhi + 1, 2, 20, 160, 8).float()
     W = (img[:, 0] + img[:, 1]).permute(0, 2, 1, 3).reshape(mlo + mhi + 1, 160, 160)      # [tap, n, k]
     assert (W - pack.conv_s2d_matrices(w, dil, r)).abs().max() <= 2e-5
     X = x.view(2, C, -1, r).permute(0, 2, 1, 3).reshape(2, -1, C * r)

@@ -140,7 +140,7 @@ def test_full_size_properties(model, hp, sd):
 
 
 def test_empty_and_bad_inputs(model, hp):
-    from whisper_vits_svc_b200 import _lib
+    from whisper_vits_svc_b200 import _lib, models
     d = make_inputs(9, 1, 8, hp)
     src = model.pitch2source(d["pit"], rand_ini=d["rand_ini"], noise=d["noise"])
     with pytest.raises(AssertionError):
@@ -150,6 +150,10 @@ def test_empty_and_bad_inputs(model, hp):
     src0 = model.pitch2source(pit0, rand_ini=d["rand_ini"], noise=d["noise"])
     w = model.inference(d["ppg"], d["vec"], pit0, d["spk"], torch.tensor([1]), src0, eps=d["eps"])
     assert torch.isfinite(w).all()
+    # precision is 0, 1 or 3: any other value fails model creation on first use instead of running a hybrid
+    bad = models.SynthesizerInfer(513, 25, hp, precision=2).to("cuda")
+    with pytest.raises(_lib.SvcbError, match="precision"):
+        bad.pitch2source(d["pit"], rand_ini=d["rand_ini"], noise=d["noise"])
 
 
 @pytest.mark.parametrize("precision,tol", [(3, WAVE_TOL), (1, 5e-2)])

@@ -203,8 +203,6 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
     // ------------------------------------------------------------------------------------ producer
     if (tc::elect_one()) {
       const uint8_t* img[2] = {reinterpret_cast<const uint8_t*>(p.a_hi), reinterpret_cast<const uint8_t*>(p.a_lo)};
-      // this CTA's copy of the matrices (identical replicas; spreads the hot L2 lines, see pack.py)
-      const uint8_t* wsrc = p.wpk + (size_t)(blockIdx.x % kS2dReplicas) * (size_t)(2 * p.ntaps) * W_SLOT;
       int it = 0, wi = 0;
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
         const int b = tile / tpi, t = tile - b * tpi;
@@ -221,7 +219,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
           tc::mbar_arrive_expect_tx(&w_full[st], W_SLOT);
 #pragma unroll
           for (int piece = 0; piece < 4; ++piece)    // four requests in flight per matrix instead of one long one
-            tc::bulk_g2s(Wbase + (size_t)st * W_SLOT + piece * (W_SLOT / 4), wsrc + (size_t)c * W_SLOT + piece * (W_SLOT / 4),
+            tc::bulk_g2s(Wbase + (size_t)st * W_SLOT + piece * (W_SLOT / 4), p.wpk + (size_t)c * W_SLOT + piece * (W_SLOT / 4),
                          W_SLOT / 4, &w_full[st]);
         }
       }

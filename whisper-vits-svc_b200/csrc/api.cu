@@ -53,13 +53,12 @@ struct ConvW {
   const float* b = nullptr;
   int cin = 0, cout = 0, cout_pad = 0, k = 1;
   const uint8_t* tc = nullptr;  // tensor-core tile image (pack.py:pack_conv_tc_general) or null
-  int kch = 0, cin_pad = 0, bn = 0, ntiles = 0;
+  int cin_pad = 0, bn = 0, ntiles = 0;
 };
 
 // must match pack.py:tc_tiling
 static void tc_tiling(ConvW& w) {
-  w.kch = 32;   // (64 when cin % 64 == 0 was the round-1 choice: one CTA per SM for the 192-channel convs)
-  w.cin_pad = (w.cin + w.kch - 1) / w.kch * w.kch;
+  w.cin_pad = (w.cin + kConvTcKch - 1) / kConvTcKch * kConvTcKch;
   const int cp16 = (w.cout + 15) / 16 * 16;
   w.ntiles = (cp16 + 255) / 256;
   w.bn = ((cp16 + w.ntiles - 1) / w.ntiles + 15) / 16 * 16;
@@ -111,7 +110,7 @@ struct ResBlock {
                                  // AMP_S2D needs L % s2d_r == 0 and L % 8 == 0
 };
 
-// must match pack.py:S2D_LINK_FACTORS / s2d_taps
+// must match pack.py:s2d_factor / s2d_taps
 static int s2d_link_factor(int ch) { return ch == 40 ? 4 : ch == 20 ? 8 : ch == 10 ? 16 : 0; }
 static void s2d_taps(int k, int dil, int r, int& mlo, int& ntaps) {
   const int P = dil * (k - 1) / 2;
@@ -124,6 +123,9 @@ static void s2d_taps(int k, int dil, int r, int& mlo, int& ntaps) {
 struct svcb_model {
   svcb_config cfg;
   int hop = 1;
+  // cfg.precision as the pipelines use it: the convs' operand split (0 = fp32 CUDA cores, 1, 3), prior attention on wgmma
+  int nsplit = 0;
+  bool attn_tc = false;
   // resolved views
   svcb::ConvW pre, hub, proj;
   const float* pit_emb = nullptr;
@@ -202,20 +204,16 @@ static ConvTcParams conv_tc_params(const ConvW& w, const float* x, long long sxb
   q.x = x; q.sxb = sxb; q.sxc = sxc; q.sxt = sxt;
   q.wpk = w.tc; q.bias = w.b; q.y = y;
   q.B = B; q.Cin = w.cin; q.cin_pad = w.cin_pad; q.Cout = w.cout; q.Tin = Tin; q.Tout = Tout;
-  q.K = w.k; q.dil = dil; q.pad = pad; q.kch = w.kch; q.bn = w.bn; q.ntiles = w.ntiles;
+  q.K = w.k; q.dil = dil; q.pad = pad; q.bn = w.bn; q.ntiles = w.ntiles;
   q.nsplit = nsplit;
   return q;
 }
 
-// Route a stride-1 "same" convolution to the tensor cores when the model runs in a tensor-core
-// precision mode and the conv has a tile image; otherwise the fp32 CUDA-core kernel.
+// A conv of the prior encoder, the flow or conv_pre, on the tensor cores unless all convs run on the CUDA cores.  Every
+// caller builds p with std_conv from w (a tile image, p.bias, Cin, Cout, K): a stride-1 'same' conv, contiguous y.
 static int run_conv(const svcb_model* m, const ConvW& w, const ConvParams& p, cudaStream_t s) {
-  const int prec = m->cfg.precision;
-  if (prec == 0 || !w.tc || p.stride != 1 || p.out_mul != 1 || p.out_off != 0 || p.q0 != 0 ||
-      p.syt != 1 || p.addvec || p.out_div != 0.f || p.nq != p.Tin)
-    return launch_conv1d(p, s);
-  // (every caller builds p with std_conv from w: p.bias, Cin, Cout and K are w's)
-  ConvTcParams q = conv_tc_params(w, p.x, p.sxb, p.sxc, p.sxt, p.y, p.B, p.Tin, p.nq, p.dil, p.pad, prec == 1 ? 1 : 3);
+  if (m->nsplit == 0) return launch_conv1d(p, s);
+  ConvTcParams q = conv_tc_params(w, p.x, p.sxb, p.sxc, p.sxt, p.y, p.B, p.Tin, p.nq, p.dil, p.pad, m->nsplit);
   q.res = p.res; q.lengths = p.lengths; q.flags = p.flags; q.act = p.act;
   return launch_conv_tc(q, s);
 }
@@ -305,9 +303,8 @@ static int run_prior(const svcb_model* m, Ctx& ctx, const float* ppg, const floa
   float* att = ctx.alloc<float>((size_t)B * H * T);
   float* hbuf = ctx.alloc<float>((size_t)B * Fc * T);
   float* stats = ctx.alloc<float>((size_t)B * 2 * C * T);
-  const bool attn_tc = c.precision != 0 && H / c.enc_heads == 96 && c.enc_window == 4;
-  const size_t attn_ws_bytes = attn_tc ? rel_attention_ws_bytes(B, c.enc_heads, T) : 0;
-  uint8_t* attn_ws = attn_tc ? ctx.alloc<uint8_t>(attn_ws_bytes) : nullptr;
+  const size_t attn_ws_bytes = m->attn_tc ? rel_attention_ws_bytes(B, c.enc_heads, T) : 0;
+  uint8_t* attn_ws = m->attn_tc ? ctx.alloc<uint8_t>(attn_ws_bytes) : nullptr;
   SVCB_TRY(check_ws(ctx));
   {  // pre / hub on time-major inputs (vits/models.py:40-46)
     ConvParams p = std_conv(m->pre, ppg, x, B, T, T, 2);
@@ -325,7 +322,7 @@ static int run_prior(const svcb_model* m, Ctx& ctx, const float* ppg, const floa
   for (int i = 0; i < c.enc_layers; ++i) {
     const EncLayer& L = m->enc[i];
     RUN(run_conv(m, L.qkv, std_conv(L.qkv, x, qkv, B, T, T, 0), s));
-    if (attn_tc) RUN(launch_rel_attention_tc(qkv, L.ek, L.ev, lengths, att, attn_ws, attn_ws_bytes, B, H, c.enc_heads, c.enc_window, T, s));
+    if (m->attn_tc) RUN(launch_rel_attention_tc(qkv, L.ek, L.ev, lengths, att, attn_ws, attn_ws_bytes, B, H, c.enc_heads, c.enc_window, T, s));
     else RUN(launch_rel_attention(qkv, L.ek, L.ev, lengths, att, B, H, c.enc_heads, c.enc_window, T, s));
     RUN(run_conv(m, L.o, std_conv(L.o, att, y, B, T, T, 0), s));
     RUN(launch_layernorm_c(x, y, L.ln1g, L.ln1b, x, B, H, T, 0, 1e-5f, s));
@@ -500,7 +497,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
   const svcb_config& c = m->cfg;
   cudaStream_t s = ctx.stream;
   const int U = c.gen_input;
-  const int nsplit = c.precision == 1 ? 1 : 3;
+  const int nsplit = m->nsplit;
   const long long Ltot = (long long)T * m->hop;
   float* sc = ctx.alloc<float>((size_t)B * U);
   float* bi = ctx.alloc<float>((size_t)B * U);
@@ -513,7 +510,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
     for (int i = 0; i < c.n_ups; ++i) {
       ch /= 2; L *= c.up_rates[i];
       max_stage = std::max<size_t>(max_stage, (size_t)B * ch * L);
-      if (c.precision != 0) img_bytes = std::max<size_t>(img_bytes, p8_image_bytes(B, ch, (int)L));
+      if (nsplit) img_bytes = std::max<size_t>(img_bytes, p8_image_bytes(B, ch, (int)L));
     }
   }
   float* T1 = ctx.alloc<float>(max_stage);
@@ -521,12 +518,12 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
   float* RA = ctx.alloc<float>(max_stage);
   float* RB = ctx.alloc<float>(max_stage);
   const long long Lpad = (SRC_PADF + Ltot + 128 + 3) / 4 * 4;
-  float* SRCP = c.precision != 0 ? ctx.alloc<float>((size_t)B * Lpad) : nullptr;
+  float* SRCP = nsplit ? ctx.alloc<float>((size_t)B * Lpad) : nullptr;
   void* IMG_HI = img_bytes ? ctx.alloc<uint8_t>(img_bytes) : nullptr;
-  void* IMG_LO = (img_bytes && c.precision != 1) ? ctx.alloc<uint8_t>(img_bytes) : nullptr;
+  void* IMG_LO = (img_bytes && nsplit == 3) ? ctx.alloc<uint8_t>(img_bytes) : nullptr;
   SVCB_TRY(check_ws(ctx));
 
-  if (c.precision != 0 && !ctx.dry) {
+  if (nsplit && !ctx.dry) {
     dim3 grid((unsigned)((Lpad + 255) / 256), B);
     KernelScope ks("pad_source", s, 0.0, 8.0 * B * (double)Lpad);
     pad_source_kernel<<<grid, 256, 0, s>>>(source, SRCP, Ltot, Lpad);
@@ -584,7 +581,6 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
         p.nq = qmax - p.q0 + 1;
         p.y = T1 + slab;
         p.syb = (long long)chn * p.nq; p.syc = p.nq; p.syt = 1;
-        p.out_mul = 1; p.out_off = -p.q0;
         fp.tmp[r] = p.y; fp.nq[r] = p.nq; fp.q0[r] = p.q0;
         slab += (size_t)B * chn * p.nq;
         if (us.phase_tc[r]) {
@@ -709,7 +705,9 @@ struct Resolver : BlobTensors {
 
 static int resolve(svcb_model* m, Resolver& R) {
   const svcb_config& c = m->cfg;
-  const bool tc = c.precision != 0;
+  m->nsplit = c.precision;   // validate_cfg admits 0, 1 and 3, which are the split counts
+  const bool tc = m->nsplit != 0;
+  m->attn_tc = tc && c.enc_window == 4;   // (and 96 channels per head, which validate_cfg requires)
   const int H = c.hidden_channels, C = c.inter_channels;
   m->pre = R.conv("enc_p.pre", c.ppg_dim, H, 5, true, true);
   m->hub = R.conv("enc_p.hub", c.vec_dim, H, 5, true, true);
@@ -763,7 +761,7 @@ static int resolve(svcb_model* m, Resolver& R) {
     for (int r = 0; r < us.rate; ++r)
       us.phase.push_back(R.conv(p + ".ph" + std::to_string(r), ch, ch / 2, us.taps, false, true));
     us.bias = R.get(p + ".b", ch / 2);
-    if (us.rate == 4 && us.taps == 2 && i + 1 < c.n_ups) {   // pack.py:UPS_COMBINED_RATES (+ the stage's noise conv)
+    if (us.rate == 4 && us.taps == 2 && i + 1 < c.n_ups) {   // must match pack.py:pack_svc_state_dict (+ the stage's noise conv)
       ConvW& w = us.comb;
       us.comb_cin1 = (ch + 31) / 32 * 32;
       us.comb_cin2 = us.rate * us.sf + us.sf;         // source samples a frame's rate outputs reach (filter 2 sf, stride sf)
@@ -823,13 +821,13 @@ static int resolve(svcb_model* m, Resolver& R) {
       for (int d = 0; d < 3 && rb.s2d_r; ++d) {
         s2d_taps(rb.k, rb.dil[d], rb.s2d_r, rb.s2d_ml1[d], rb.s2d_nt1[d]);
         s2d_taps(rb.k, 1, rb.s2d_r, rb.s2d_ml2[d], rb.s2d_nt2[d]);
-        const uint64_t per_tap = (uint64_t)kS2dReplicas * 2ull * 160 * 160 / 2;   // fp32-typed elements of one (hi, lo) pair, all replicas
+        const uint64_t per_tap = 2ull * 160 * 160 / 2;   // fp32-typed elements of one (hi, lo) pair
         rb.c1_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c1." + std::to_string(d) + ".s2d", per_tap * rb.s2d_nt1[d]));
         rb.c2_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c2." + std::to_string(d) + ".s2d", per_tap * rb.s2d_nt2[d]));
       }
       for (int a = 0; a < 6; ++a) rb.act[a] = R.snake(p + ".act." + std::to_string(a), ch);
       rb.fallback = !tc ? AMP_FP32 : amp_block_fused_supported(ch, rb.k, rb.dil) ? AMP_BLOCK_FUSED : AMP_TC;
-      rb.form = c.precision == 3 && rb.s2d_r ? AMP_S2D : rb.fallback;
+      rb.form = m->nsplit == 3 && rb.s2d_r ? AMP_S2D : rb.fallback;
     }
   }
   m->post_act = R.snake("dec.post.act", ch);
@@ -849,6 +847,7 @@ static int resolve(svcb_model* m, Resolver& R) {
 }
 
 static int validate_cfg(const svcb_config& c) {
+  if (c.precision != 0 && c.precision != 1 && c.precision != 3) { set_error("config: precision must be 0, 1 or 3"); return SVCB_E_UNSUPPORTED; }
   if (c.n_ups < 1 || c.n_ups > SVCB_MAX_UPS || c.n_res < 1 || c.n_res > SVCB_MAX_RES) {
     set_error("config: n_ups / n_res out of range");
     return SVCB_E_BAD_SHAPE;

@@ -208,13 +208,10 @@ struct ConvParams {
   float* y = nullptr;
   long long syb = 0, syc = 0, syt = 1;  // element strides of y[b, co, t]
   const float* res = nullptr;           // residual, indexed like y (same strides), or null
-  const float* addvec = nullptr;        // optional [Tout_total][Cout] row table added after act
-                                        // (Whisper positional embedding), or null
   const long long* lengths = nullptr;   // [B] int64 or null
   int B = 0, Cin = 0, Cout = 0, Tin = 0;
   int K = 1, stride = 1, dil = 1, pad = 0;
-  int q0 = 0, nq = 0;                   // outputs q = q0 .. q0+nq-1; x index = q*stride + j*dil - pad
-  int out_mul = 1, out_off = 0;         // y time index = q*out_mul + out_off
+  int q0 = 0, nq = 0;                   // outputs q = q0 .. q0+nq-1 at y time index q - q0; x index = q*stride + j*dil - pad
   int flags = 0;
   int act = ACT_NONE;
   float out_div = 0.f;                  // if != 0: v = v / out_div (after accumulate)
@@ -245,13 +242,12 @@ size_t p8_image_bytes(int B, int C, int L);
 int p8_rows(int L);
 
 // ----------------------------------------------------------------------------- space-to-depth AMP links (C = 20, 10)
-constexpr int kS2dReplicas = 1;   // copies of each matrix set in the blob (pack.py:S2D_REPLICAS)
 struct AmpS2dParams {
   const void* a_hi = nullptr;   // input S2D image (bf16 hi) [B][20][Rp][8] — SnakeAlias already applied
   const void* a_lo = nullptr;
   void* o_hi = nullptr;         // output S2D image = SnakeAlias_next(result), or null
   void* o_lo = nullptr;
-  const uint8_t* wpk = nullptr; // bf16 [kS2dReplicas][ntaps][2 (hi, lo)][20][160][8]  (pack.py:pack_conv_s2d)
+  const uint8_t* wpk = nullptr; // bf16 [ntaps][2 (hi, lo)][20][160][8]  (pack.py:pack_conv_s2d)
   const float* bias = nullptr;  // [C]
   const float* res = nullptr;   // residual [B, C, L] fp32 or null
   float* y = nullptr;           // fp32 result [B, C, L] or null
@@ -315,17 +311,18 @@ bool ups_fused_supported(int Cin, int Cout, int rate, int taps, int Kn);
 bool amp_block_fused_supported(int C, int K, const int* dil);
 
 // ----------------------------------------------------------------------------- general tensor-core conv
+constexpr int kConvTcKch = 32;   // input channels per chunk (the K of one A panel): 32 lets two CTAs share an SM
 struct ConvTcParams {
   const float* x = nullptr;
   long long sxb = 0, sxc = 0, sxt = 1;   // element strides of x[b, ci, t]
-  const uint8_t* wpk = nullptr;          // bf16 tiles [K][ncc][2][ntiles][kch/8][bn][8] (pack.py:pack_conv_tc_general)
+  const uint8_t* wpk = nullptr;          // bf16 tiles [K][ncc][2][ntiles][kConvTcKch/8][bn][8] (pack.py:pack_conv_tc_general)
   const float* bias = nullptr;           // [Cout] (packed order) or null
   float* y = nullptr;                    // [B, Cout(/2 if gated), Tout] contiguous
   const float* res = nullptr;            // indexed like y, or null
   const long long* lengths = nullptr;
   int B = 0, Cin = 0, cin_pad = 0, Cout = 0, Tin = 0, Tout = 0;
   int K = 1, dil = 1, pad = 0;
-  int kch = 64, bn = 128, ntiles = 1;
+  int bn = 128, ntiles = 1;
   int nsplit = 3;
   int flags = 0, act = 0;
   // optional second input (pack.py:ups_combined): packed input channels cin1 .. cin1 + cin2 are x2[b][t * sx2t + c]
@@ -382,9 +379,11 @@ size_t source_scan_ws_bytes(int B, int T, int n_harm);
 int launch_source2wav(const float* src, int16_t* out, size_t n, cudaStream_t s);
 
 // ----------------------------------------------------------------------------- Whisper / HuBERT transformer kernels
-// bf16 wgmma GEMM over tile images with the fused epilogues listed in whisper_gemm.cu (GemmEpi)
+// bf16 wgmma GEMM over tile images with fused epilogues (each one is described in whisper_gemm.cu)
+enum GemmEpi : int { EPI_BF16_ROWMAJOR = 0, EPI_GELU_BF16_IMAGE = 1, EPI_RESID_F32 = 2, EPI_GELU_ADD_F32 = 3, EPI_QKV_HEADS = 4,
+                     EPI_GELU_CONV2_IMG = 5, EPI_GELU_VALID_S2_IMG = 6, EPI_GELU_ADD_F32_LD = 7, EPI_IVF_TOPK = 8 };
 int launch_gemm_tc(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
-                   int M, int N, int K, int epi, cudaStream_t s, int res_mod = 0, int aux = 0);
+                   int M, int N, int K, GemmEpi epi, cudaStream_t s, int res_mod = 0, int aux = 0);
 int launch_im2col_s1_image(const float* mel, void* img, int B, int n_mels, int n, cudaStream_t s);
 int launch_im2col_s2_image(const float* h1, void* img, int B, int D, int n, int n2, cudaStream_t s, int taps = 3, int pad = 1);
 int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s);

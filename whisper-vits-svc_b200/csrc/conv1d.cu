@@ -121,13 +121,11 @@ conv1d_kernel(const ConvParams p, const int ci_tile, const int xspan) {
   for (int i = 0; i < TPT; ++i) {
     const int tq = tq0 + lane + 32 * i;
     if (tq >= p.nq) continue;
-    const long long to = (long long)(p.q0 + tq) * p.out_mul + p.out_off;
-    const bool keep = !(p.flags & CONV_OUT_MASK) || to < len;
-    auto finish = [&](float v, int co, int cout_real) {
+    const bool keep = !(p.flags & CONV_OUT_MASK) || tq < len;
+    auto finish = [&](float v, int co) {
       if (!keep) v = 0.f;
-      const long long off = (long long)co * p.syc + to * p.syt;
+      const long long off = (long long)co * p.syc + (long long)tq * p.syt;
       if (rb) v += rb[off];
-      if (p.addvec) v += __ldg(p.addvec + to * cout_real + co);
       if (p.flags & CONV_ACCUM) v += yb[off];
       if (p.out_div != 0.f) { asm volatile(""); v = v / p.out_div; }
       yb[off] = v;
@@ -140,7 +138,7 @@ conv1d_kernel(const ConvParams p, const int ci_tile, const int xspan) {
           float a = acc[i][2 * h], g = acc[i][2 * h + 1];
           if (p.bias) { a += __ldg(p.bias + cp); g += __ldg(p.bias + cp + 1); }
           const float v = tanhf(a) * (1.f / (1.f + expf(-g)));
-          finish(v, cp >> 1, p.Cout >> 1);
+          finish(v, cp >> 1);
         }
       }
     } else {
@@ -151,7 +149,7 @@ conv1d_kernel(const ConvParams p, const int ci_tile, const int xspan) {
           float v = acc[i][h];
           if (p.bias) v += __ldg(p.bias + co);
           v = act_apply(v, p.act);
-          finish(v, co, p.Cout);
+          finish(v, co);
         }
       }
     }
@@ -177,7 +175,7 @@ static int launch_t(const ConvParams& p, int cog, int ci_tile, int xspan, size_t
   dim3 grid((p.nq + 32 * TPT - 1) / (32 * TPT), (p.cout_pad / 8 + cog - 1) / cog, p.B);
   const int cout_real = (p.flags & CONV_GATE) ? p.Cout / 2 : p.Cout;
   char kname[64];
-  snprintf(kname, sizeof(kname), "conv1d_fp32_%dto%d_k%d_o%d", p.Cin, p.Cout, p.K, p.out_mul);
+  snprintf(kname, sizeof(kname), "conv1d_fp32_%dto%d_k%d_o1", p.Cin, p.Cout, p.K);
   KernelScope ks(kname, s, 2.0 * p.Cin * p.K * p.Cout * (double)p.nq * p.B,
                  4.0 * ((double)p.B * p.Cin * p.nq * p.stride + (double)p.B * cout_real * p.nq * (p.res ? 2 : 1) +
                         (double)p.Cin * p.K * p.Cout));

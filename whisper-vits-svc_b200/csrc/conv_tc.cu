@@ -5,8 +5,8 @@
 // vits_decoder/generator.py:177-178) — the F.conv1d call sites whose contraction is wide enough for
 // the tensor cores (SURVEY.md §8a rows a2-a7).
 //
-//   D[t, co] = sum_cc sum_tap  A_cc[t + tap*dil, :] . W[tap, cc][co, :]      M = 128, N = BN, K = KCH
-// * Input channels are processed in chunks of KCH (32 or 64).  Two warpgroups gather one chunk of x
+//   D[t, co] = sum_cc sum_tap  A_cc[t + tap*dil, :] . W[tap, cc][co, :]      M = 128, N = BN, K = 32
+// * Input channels are processed in chunks of 32 (kConvTcKch).  Two warpgroups gather one chunk of x
 //   (fp32, any strides — the time-major PPG input included), apply the optional input mask and the
 //   conv's zero padding, split to bf16 hi/lo and write the K-major panel layout of tc.cuh into a
 //   2-deep A ring; the gather of chunk cc+1 overlaps the MMAs of chunk cc still in flight.
@@ -48,16 +48,16 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
   const int t0 = blockIdx.x * CT_M;
   const int P = p.pad;
   const int R = CT_M + (p.K - 1) * p.dil;
-  const int KC = p.kch / 8;
+  constexpr int KC = kConvTcKch / 8;
   const int n0row = t0 - P;                       // sequence position of A row 0
   const uint32_t a_part = (uint32_t)KC * R * 16u; // one of hi / lo
   const int nparts = p.nsplit == 3 ? 2 : 1;
   const uint32_t a_buf = a_part * nparts;
-  const uint32_t w_tile = (uint32_t)p.kch * BN * 2u;
+  constexpr uint32_t w_tile = (uint32_t)kConvTcKch * BN * 2u;
   uint8_t* A0 = smem;
   uint8_t* W0 = smem + 2 * a_buf;
   float* Strips = reinterpret_cast<float*>(W0 + (size_t)wst * w_tile);
-  const int ncc = p.cin_pad / p.kch;
+  const int ncc = p.cin_pad / kConvTcKch;
   const long long len = p.lengths ? p.lengths[b] : (long long)1 << 60;
 
   if (tid == 0) {
@@ -89,7 +89,7 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
     auto fetch = [&](int item, int cc, float (&v)[8]) {
       const int r = item % R, kc = item / R;
       const int tau = n0row + r;
-      const int c0 = cc * p.kch + kc * 8;
+      const int c0 = cc * kConvTcKch + kc * 8;
       const bool row_ok = tau >= 0 && tau < p.Tin && (!(p.flags & CONV_IN_MASK) || tau < len);
       if (row_ok && x2b && c0 >= p.cin1) {   // second input: channel-contiguous windows (unaligned)
         const float* s2 = x2b + (long long)tau * p.sx2t + (c0 - p.cin1);
@@ -138,7 +138,7 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
   const uint32_t a_base = tc::smem_u32(A0) + (uint32_t)wg * 64u * 16u, w_base = tc::smem_u32(W0);
   const uint32_t lbo_a = (uint32_t)R * 16u, lbo_b = (uint32_t)BN * 16u;
   const uint64_t ks_a = (2u * lbo_a) >> 4, ks_b = (2u * lbo_b) >> 4;
-  const int nk = p.kch / 16;
+  constexpr int nk = kConvTcKch / 16;
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -261,13 +261,13 @@ conv_tc_kernel(const ConvTcParams p, const int wst) {
 
 static size_t conv_tc_smem_bytes(const ConvTcParams& p, int wst) {
   const int R = CT_M + (p.K - 1) * p.dil;
-  const size_t a_buf = (size_t)(p.kch / 8) * R * 16 * (p.nsplit == 3 ? 2 : 1);
-  return 2 * a_buf + (size_t)wst * p.kch * p.bn * 2 + CT_STRIP_BYTES + 128;
+  const size_t a_buf = (size_t)(kConvTcKch / 8) * R * 16 * (p.nsplit == 3 ? 2 : 1);
+  return 2 * a_buf + (size_t)wst * kConvTcKch * p.bn * 2 + CT_STRIP_BYTES + 128;
 }
 
 int launch_conv_tc(const ConvTcParams& p, cudaStream_t s) {
   if (p.B <= 0 || p.Tout <= 0) return SVCB_OK;
-  if ((p.kch != 32 && p.kch != 64) || p.cin_pad % p.kch || p.bn % 16 || p.bn < 16 || p.bn > 256 ||
+  if (p.cin_pad % kConvTcKch || p.bn % 16 || p.bn < 16 || p.bn > 256 ||
       p.ntiles * p.bn < p.Cout || (p.nsplit != 1 && p.nsplit != 3) || p.Tout > p.Tin) {
     set_error("conv_tc: unsupported tiling (stride-1 'same' convolutions only)");
     return SVCB_E_BAD_SHAPE;

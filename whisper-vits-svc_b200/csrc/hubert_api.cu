@@ -313,9 +313,9 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
     for (int i = 1; i <= 6; ++i) {
       const int K = kHbKernels[i - 1] * HB_C, Mi = B * L.T[i];
       if (i < 6)   // GELU, scattered into conv_{i+1}'s image
-        SVCB_TRY(launch_gemm_tc(img[(i - 1) & 1], h->conv_wimg[i - 1], nullptr, img[i & 1], nullptr, Mi, HB_C, K, 6, s, L.T[i], kHbKernels[i]));
+        SVCB_TRY(launch_gemm_tc(img[(i - 1) & 1], h->conv_wimg[i - 1], nullptr, img[i & 1], nullptr, Mi, HB_C, K, EPI_GELU_VALID_S2_IMG, s, L.T[i], kHbKernels[i]));
       else         // GELU -> fp32 rows [B * T, 512]
-        SVCB_TRY(launch_gemm_tc(img[(i - 1) & 1], h->conv_wimg[i - 1], nullptr, rows, nullptr, Mi, HB_C, K, 3, s));
+        SVCB_TRY(launch_gemm_tc(img[(i - 1) & 1], h->conv_wimg[i - 1], nullptr, rows, nullptr, Mi, HB_C, K, EPI_GELU_ADD_F32, s));
     }
   }
   const float* cur = bufa;
@@ -335,13 +335,13 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
   SVCB_TRY(tap(0, rows, (size_t)M * HB_C));
   // FeatureProjection: LayerNorm(512) -> Linear(512, 768)
   SVCB_TRY(launch_ln_rows(rows, h->fp_lng, h->fp_lnb, a512, M, HB_C, true, s));
-  SVCB_TRY(launch_gemm_tc(a512, h->fp_w, h->fp_b, x, nullptr, M, HB_D, HB_C, 2, s));
+  SVCB_TRY(launch_gemm_tc(a512, h->fp_w, h->fp_b, x, nullptr, M, HB_D, HB_C, EPI_RESID_F32, s));
   SVCB_TRY(tap(1, x, (size_t)M * HB_D));
   // y = x + GELU(pos_conv(x)[..., :-1]): 16 groups of 48 channels, 128 taps, two 24-channel halves per group
   for (int g = 0; g < HB_PG && !(flags & 2); ++g) {   // tensor cores: per group an im2col image (K = 128 x 48) x [256 (48 used), K]
     const int cg = HB_D / HB_PG, c0 = g * cg;
     SVCB_TRY(launch_im2col_rows_image(x, base + L.posimg, B, T, HB_D, c0, cg, HB_PK, HB_PK / 2, s));
-    SVCB_TRY(launch_gemm_tc(base + L.posimg, h->pos_wimg[g], h->pos_bimg[g], y + c0, x + c0, M, 256, HB_PK * cg, 7, s, cg, HB_D));
+    SVCB_TRY(launch_gemm_tc(base + L.posimg, h->pos_wimg[g], h->pos_bimg[g], y + c0, x + c0, M, 256, HB_PK * cg, EPI_GELU_ADD_F32_LD, s, cg, HB_D));
   }
   for (int g = 0; g < HB_PG && (flags & 2); ++g)       // flags bit 1: fp32 on the CUDA cores
     for (int hf = 0; hf < 2; ++hf) {
@@ -360,17 +360,17 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
   if (qkv_heads_tp(T) != T) SVCB_CUDA_CHECK(cudaMemsetAsync(qkv, 0, (size_t)B * qkv_heads_tp(T) * 3 * HB_D * 2, s));
   for (int i = 0; i < h->n_layer; ++i) {   // post-LN layers: x = LN1(x + SA(x)); x = LN2(x + W2 gelu(W1 x))
     const HLayer& l = h->layers[i];
-    SVCB_TRY(launch_gemm_tc(a, l.wqkv, l.bqkv, qkv, nullptr, M, 3 * HB_D, HB_D, 4, s, T));
+    SVCB_TRY(launch_gemm_tc(a, l.wqkv, l.bqkv, qkv, nullptr, M, 3 * HB_D, HB_D, EPI_QKV_HEADS, s, T));
     SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, T, HB_D, HB_H, 0, s));
-    SVCB_TRY(launch_gemm_tc(att, l.wo, l.bo, y, x, M, HB_D, HB_D, 2, s));
+    SVCB_TRY(launch_gemm_tc(att, l.wo, l.bo, y, x, M, HB_D, HB_D, EPI_RESID_F32, s));
     SVCB_TRY(launch_ln_rows(y, l.ln1g, l.ln1b, a, M, HB_D, true, s, x));
-    SVCB_TRY(launch_gemm_tc(a, l.w1, l.b1, mid, nullptr, M, HB_FF, HB_D, 1, s));
-    SVCB_TRY(launch_gemm_tc(mid, l.w2, l.b2, y, x, M, HB_D, HB_FF, 2, s));
+    SVCB_TRY(launch_gemm_tc(a, l.w1, l.b1, mid, nullptr, M, HB_FF, HB_D, EPI_GELU_BF16_IMAGE, s));
+    SVCB_TRY(launch_gemm_tc(mid, l.w2, l.b2, y, x, M, HB_D, HB_FF, EPI_RESID_F32, s));
     SVCB_TRY(launch_ln_rows(y, l.ln2g, l.ln2b, a, M, HB_D, true, s, x));
     if (i == 0) SVCB_TRY(tap(3, x, (size_t)M * HB_D));
   }
   SVCB_TRY(tap(4, x, (size_t)M * HB_D));
-  return launch_gemm_tc(a, h->proj_w, h->proj_b, out, nullptr, M, HB_OUT, HB_D, 2, s);
+  return launch_gemm_tc(a, h->proj_w, h->proj_b, out, nullptr, M, HB_OUT, HB_D, EPI_RESID_F32, s);
 }
 
 }  // extern "C"

@@ -111,20 +111,20 @@ int svcb_whisper_encode(const svcb_whisper* w, const float* mel, float* out, int
   // CUDA-core conv1 + the separate im2col pass were 2.0 of the encoder's 33.6 ms.)
   SVCB_CUDA_CHECK(cudaMemsetAsync(mid, 0, (size_t)(M + 127) / 128 * 128 * 3 * D * 2, s));
   SVCB_TRY(launch_im2col_s1_image(mel, a1, B, c.n_mels, n, s));
-  SVCB_TRY(launch_gemm_tc(a1, w->conv1_wimg, w->conv1_b, mid, nullptr, B * n, D, (3 * c.n_mels + 63) / 64 * 64, 5, s, n));
+  SVCB_TRY(launch_gemm_tc(a1, w->conv1_wimg, w->conv1_b, mid, nullptr, B * n, D, (3 * c.n_mels + 63) / 64 * 64, EPI_GELU_CONV2_IMG, s, n));
   // conv2 (k=3, stride 2) + GELU + positional embedding, time-major (:150-157): im2col image x the [D, 3D] weight image
-  SVCB_TRY(launch_gemm_tc(mid, w->conv2_wimg, w->conv2_b, x, w->pos, M, D, 3 * D, 3, s, n2));
+  SVCB_TRY(launch_gemm_tc(mid, w->conv2_wimg, w->conv2_b, x, w->pos, M, D, 3 * D, EPI_GELU_ADD_F32, s, n2));
   // pad positions of the head-major QKV buffer are read (times P = 0) but never written: keep them finite
   if (qkv_heads_tp(n2) != n2) SVCB_CUDA_CHECK(cudaMemsetAsync(qkv, 0, (size_t)B * qkv_heads_tp(n2) * 3 * D * 2, s));
   for (int i = 0; i < c.n_layer; ++i) {
     const WBlock& b = w->blocks[i];
     SVCB_TRY(launch_ln_rows(x, b.ln1g, b.ln1b, a, M, D, true, s));
-    SVCB_TRY(launch_gemm_tc(a, b.wqkv, b.bqkv, qkv, nullptr, M, 3 * D, D, 4, s, n2));
+    SVCB_TRY(launch_gemm_tc(a, b.wqkv, b.bqkv, qkv, nullptr, M, 3 * D, D, EPI_QKV_HEADS, s, n2));
     SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, n2, D, c.n_head, 0, s));
-    SVCB_TRY(launch_gemm_tc(att, b.wo, b.bo, x, x, M, D, D, 2, s));
+    SVCB_TRY(launch_gemm_tc(att, b.wo, b.bo, x, x, M, D, D, EPI_RESID_F32, s));
     SVCB_TRY(launch_ln_rows(x, b.ln2g, b.ln2b, a, M, D, true, s));
-    SVCB_TRY(launch_gemm_tc(a, b.w1, b.b1, mid, nullptr, M, 4 * D, D, 1, s));
-    SVCB_TRY(launch_gemm_tc(mid, b.w2, b.b2, x, x, M, D, 4 * D, 2, s));
+    SVCB_TRY(launch_gemm_tc(a, b.w1, b.b1, mid, nullptr, M, 4 * D, D, EPI_GELU_BF16_IMAGE, s));
+    SVCB_TRY(launch_gemm_tc(mid, b.w2, b.b2, x, x, M, D, 4 * D, EPI_RESID_F32, s));
   }
   return launch_ln_rows(x, w->lnp_g, w->lnp_b, out, M, D, false, s);
 }
@@ -153,7 +153,7 @@ int svcb_op_gemm_bf16(const void* A_bf16, const void* W_bf16, const float* bias,
   char* w_img = a_img + (((size_t)(M + 127) / 128 * 128 * K * 2 + 255) & ~(size_t)255);
   SVCB_TRY(launch_rowmajor_to_image(A_bf16, a_img, M, K, 128, s));
   SVCB_TRY(launch_rowmajor_to_image(W_bf16, w_img, N, K, 256, s));
-  return launch_gemm_tc(a_img, w_img, bias, out, res, M, N, K, epilogue, s);
+  return launch_gemm_tc(a_img, w_img, bias, out, res, M, N, K, static_cast<GemmEpi>(epilogue), s);
 }
 
 size_t svcb_op_attention_tc_bf16_scratch_bytes(int32_t B, int32_t T, int32_t D) {

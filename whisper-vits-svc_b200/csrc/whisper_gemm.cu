@@ -39,8 +39,6 @@ namespace svcb {
 // 8: the IVF coarse search (csrc/retrieval_api.cu): f = acc + bias = |c|^2 - 2 x.c; each thread keeps the aux (= nprobe)
 //    smallest (score, column) pairs of its 16 columns, ties to the lower column, and writes them as int2 {score bits,
 //    column} to out[m][N / 16][aux] — the [M, N] score matrix is never stored
-enum GemmEpi : int { EPI_BF16_ROWMAJOR = 0, EPI_GELU_BF16_IMAGE = 1, EPI_RESID_F32 = 2, EPI_GELU_ADD_F32 = 3, EPI_QKV_HEADS = 4,
-                     EPI_GELU_CONV2_IMG = 5, EPI_GELU_VALID_S2_IMG = 6, EPI_GELU_ADD_F32_LD = 7, EPI_IVF_TOPK = 8 };
 
 constexpr int GM_BM = 128, GM_BK = 64, GM_STAGES = 3;
 constexpr int GM_EPI_LD = 72;   // floats per row of an epilogue strip (64 columns + 8: conflict-free fragment stores)
@@ -261,7 +259,7 @@ static int launch_gemm_t(const __nv_bfloat16* A, const __nv_bfloat16* W, const f
 
 // A_img: tile image [ceil(M/128)][K/64][8][128][8]; W_img: tile image [N/256][K/64][8][256][8]
 int launch_gemm_tc(const void* A_img, const void* W_img, const float* bias, void* out, const float* res,
-                   int M, int N, int K, int epi, cudaStream_t s, int res_mod, int aux) {
+                   int M, int N, int K, GemmEpi epi, cudaStream_t s, int res_mod, int aux) {
   if (M <= 0) return SVCB_OK;
   if (K % 64 || N % 256) { set_error("gemm_tc: need K % 64 == 0 and N % 256 == 0"); return SVCB_E_BAD_SHAPE; }
   const __nv_bfloat16* A = static_cast<const __nv_bfloat16*>(A_img);
@@ -287,9 +285,10 @@ int launch_gemm_tc(const void* A_img, const void* W_img, const float* bias, void
       return launch_gemm_t<256, EPI_QKV_HEADS>(A, W, bias, out, res, M, N, K, res_mod, s);
     case EPI_GELU_ADD_F32:
       return launch_gemm_t<256, EPI_GELU_ADD_F32>(A, W, bias, out, res, M, N, K, res_mod, s);
+    default:   // (EPI_IVF_TOPK has its own launcher, launch_ivf_coarse_tc)
+      set_error("gemm_tc: unknown epilogue");
+      return SVCB_E_BAD_SHAPE;
   }
-  set_error("gemm_tc: unknown epilogue");
-  return SVCB_E_BAD_SHAPE;
 }
 
 // IVF coarse search (epilogue 8): cand[M][N/16][nprobe] int2 {score bits, column}, score = cnorm[col] - 2 x.c

@@ -64,8 +64,6 @@ def pack_conv_tc(w: torch.Tensor) -> torch.Tensor:
 
 
 S2D_WIDTH = 160   # K' = N' = C * r of the space-to-depth AMP links (csrc/amp_s2d.cu)
-S2D_REPLICAS = 1             # copies of every matrix set in the blob; must match csrc/common.cuh:kS2dReplicas
-S2D_LINK_FACTORS = (4, 8, 16)   # factors csrc/amp_s2d.cu implements (C = 40, 20, 10); must match api.cu:s2d_link_factor
 
 
 def s2d_factor(c: int) -> int:
@@ -110,18 +108,12 @@ def pack_conv_s2d(w: torch.Tensor, dil: int, r: int) -> torch.Tensor:
     lo = (W - hi.float()).bfloat16()
     st = torch.stack([hi, lo], 1)                              # [T, 2, n, k]
     img = st.view(T, 2, n, k // 8, 8).permute(0, 1, 3, 2, 4).contiguous()   # [T, 2, kc, n, 8]
-    # S2D_REPLICAS identical copies back to back (CTA i reads copy i % S2D_REPLICAS): a knob for spreading the
-    # hot L2 lines of the matrices every CTA streams per tile.  Measured with 4 copies: no change (the links
-    # are bound by their epilogue, not by weight delivery), so one copy is packed.
-    return img.view(torch.float32).reshape(-1).repeat(S2D_REPLICAS)
-
-
-TC_KCH64 = False   # input-channel chunk of csrc/conv_tc.cu: 32 everywhere lets two CTAs share an SM (api.cu:tc_tiling)
+    return img.view(torch.float32).reshape(-1)
 
 
 def tc_tiling(cout: int, cin: int):
     """(kch, cin_pad, bn, ntiles) — must match csrc/api.cu:tc_tiling."""
-    kch = 64 if (cin % 64 == 0 and TC_KCH64) else 32
+    kch = 32
     cin_pad = (cin + kch - 1) // kch * kch
     cp16 = (cout + 15) // 16 * 16
     ntiles = (cp16 + 255) // 256
@@ -144,9 +136,6 @@ def pack_conv_tc_general(w: torch.Tensor) -> torch.Tensor:
     st = st.view(k, 2, ntiles, bn, ncc, kch // 8, 8)            # K, part, nt, n, cc, kc, e
     img = st.permute(0, 4, 1, 2, 5, 3, 6).contiguous()          # K, cc, part, nt, kc, n, e
     return img.view(torch.float32).reshape(-1)
-
-
-UPS_COMBINED_RATES = (4,)   # stages whose polyphase sub-filters are also packed as ONE convolution (below)
 
 
 def ups_combined(subs, bias: torch.Tensor, rate: int, pad: int, wn: torch.Tensor = None, bn: torch.Tensor = None,
@@ -273,8 +262,8 @@ def pack_svc_state_dict(sd: Dict[str, torch.Tensor], cfg: dict) -> List[Tuple[st
             put(f"dec.ups.{i}.ph{r}.tc", pack_conv_tc_general(sub))
         put(f"dec.ups.{i}.b", sd[f"dec.ups.{i}.bias"])
         wn = sd[f"dec.noise_convs.{i}.weight"]
-        if rate in UPS_COMBINED_RATES and M == 2:
-            sf_c = int(np.prod(cfg["up_rates"][i + 1:])) if i + 1 < len(cfg["up_rates"]) else 1
+        if rate == 4 and M == 2 and i + 1 < cfg["n_ups"]:   # must match csrc/api.cu:resolve
+            sf_c = int(np.prod(cfg["up_rates"][i + 1:]))
             assert wn.shape[-1] == 2 * sf_c, "combined up-sampling stage: noise filter must be 2 * prod(later rates) long"
             wc, bc = ups_combined(subs, sd[f"dec.ups.{i}.bias"].float(), rate, (k - rate) // 2, wn.float(),
                                   sd[f"dec.noise_convs.{i}.bias"].float(), sf_c)
@@ -293,7 +282,7 @@ def pack_svc_state_dict(sd: Dict[str, torch.Tensor], cfg: dict) -> List[Tuple[st
         p = f"dec.resblocks.{n}"
         stage, j = divmod(n, cfg["n_res"])
         ch = cfg["gen_initial_channel"] >> (stage + 1)
-        r = s2d_factor(ch) if s2d_factor(ch) in S2D_LINK_FACTORS else 0
+        r = s2d_factor(ch)
         for d in range(3):
             w1 = fold_weight_norm(sd, f"{p}.convs1.{d}")
             w2 = fold_weight_norm(sd, f"{p}.convs2.{d}")
