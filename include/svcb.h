@@ -13,8 +13,8 @@
  *   - return 0 on success, <0 = svcb_status; svcb_last_error() gives a thread-local message;
  *   - a model handle is immutable after creation: concurrent calls on different streams
  *     are fine when their workspaces differ;
- *   - sm_90a only, no fallback: svcb_model_create, svcb_whisper_create, svcb_hubert_create and
- *     svcb_ivf_create fail with SVCB_E_UNSUPPORTED elsewhere.
+ *   - sm_90a only, no fallback: svcb_model_create, svcb_whisper_create, svcb_hubert_create,
+ *     svcb_ivf_create and svcb_speaker_create fail with SVCB_E_UNSUPPORTED elsewhere.
  */
 #ifndef SVCB_H_
 #define SVCB_H_
@@ -223,6 +223,36 @@ size_t svcb_ivf_workspace_bytes(const svcb_ivf* ix, int32_t M, int32_t k);
  * Deterministic; a row's result does not depend on M or on its position. */
 int svcb_ivf_retrieve(const svcb_ivf* ix, const float* x, float* out, float* dist, int64_t* ids, int32_t M, int32_t k,
                       float ratio, void* ws, size_t ws_bytes, svcb_stream stream);
+
+/* ------------------------------------------------------------------ speaker encoder (LSTM with projection) */
+typedef struct svcb_speaker svcb_speaker;
+/* Replaces LSTMSpeakerEncoder(80, 256, 768, 3) + load_checkpoint (speaker/models/lstm.py:35-60,124-131) and the
+ * AudioProcessor of speaker_pretrain/config.json.  Blob names/layouts: whisper-vits-svc_b200/speaker_infer.py:pack_speaker.
+ * Fails with SVCB_E_UNSUPPORTED unless the device is sm_90 and can hold the recurrence's 128 CTAs co-resident
+ * (cooperative launch, one CTA per SM). */
+int svcb_speaker_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table_host, int32_t n_entries,
+                        svcb_speaker** out);
+void svcb_speaker_destroy(svcb_speaker* s);
+/* mel frames of n_samples of 16 kHz audio: 1 + n_samples / 256 */
+int32_t svcb_speaker_frames(int64_t n_samples);
+/* scratch for svcb_speaker_embed on B items of total_samples samples (any split).  Items run in passes of up to 64,
+ * and a pass holds every window step's gate inputs in fp32 and the h image of a whole layer: about 0.6 GB for one
+ * utterance of 250 or more frames and about 3.1 GB for a pass of 64 (Lw x Mp rows of 19 KB, Lw = min(250, T),
+ * Mp = 10 items rounded up to 128). */
+size_t svcb_speaker_workspace_bytes(const svcb_speaker* s, int32_t B, int64_t total_samples);
+/* Replaces AudioProcessor.melspectrogram (speaker/utils/audio.py:561-571) for a ragged batch: item b is
+ * wav[sample_offsets_host[b] .. sample_offsets_host[b+1]) (more than 512 samples each) ->
+ * mel_out [sum_b T_b, 80] fp32 time-major, item b's T_b = svcb_speaker_frames(n_b) rows following item b-1's.
+ * Pre-emphasis, reflect-centred periodic-Hann STFT (1024 / 256), magnitude, Slaney mel, 20 log10 - ref_level_db,
+ * symmetric clipped normalisation, all in fp32.  ws may be NULL. */
+int svcb_speaker_mel(const svcb_speaker* s, const float* wav, const int64_t* sample_offsets_host, int32_t B, float* mel_out,
+                     void* ws, size_t ws_bytes, svcb_stream stream);
+/* Replaces LSTMSpeakerEncoder.compute_embedding (speaker/models/lstm.py:76-101) for a ragged batch: item b is
+ * mel rows [frame_offsets_host[b], frame_offsets_host[b+1]) of mel [*, 80] (16-byte aligned) -> out [B, 256], the mean
+ * of the 10 L2-normalised window embeddings; window_out [10 B, 256] receives those (may be NULL).  Products
+ * bf16x3 on the tensor cores with fp32 accumulation, gate math fp32.  An item's result does not depend on the batch. */
+int svcb_speaker_embed(const svcb_speaker* s, const float* mel, const int64_t* frame_offsets_host, int32_t B, float* out,
+                       float* window_out, void* ws, size_t ws_bytes, svcb_stream stream);
 
 /* Operator entry points of the encoder (unit tests):
  * out[M,N] = A[M,K] . W[N,K]^T + bias with epilogue 0: bf16 row-major out, 1: GELU(erf) then bf16

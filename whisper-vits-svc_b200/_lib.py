@@ -93,6 +93,12 @@ SIGNATURES = {
     "svcb_ivf_destroy": (None, [c_void_p]),
     "svcb_ivf_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
     "svcb_ivf_retrieve": (c_int, [c_void_p] * 5 + [c_int32, c_int32, c_float, c_void_p, c_size_t, c_void_p]),
+    "svcb_speaker_create": (c_int, [c_void_p, c_size_t, POINTER(TensorEntry), c_int32, POINTER(c_void_p)]),
+    "svcb_speaker_destroy": (None, [c_void_p]),
+    "svcb_speaker_frames": (c_int32, [c_int64]),
+    "svcb_speaker_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int64]),
+    "svcb_speaker_mel": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "svcb_speaker_embed": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "svcb_op_gemm_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_gemm_bf16": (c_int, [c_void_p] * 5 + [c_int32] * 4 + [c_void_p, c_size_t, c_void_p]),
     "svcb_op_attention_tc_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),

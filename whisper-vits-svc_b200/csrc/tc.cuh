@@ -133,6 +133,12 @@ template <int TB> struct Wg<16, TB> {
                  "}, %8, %9, p, 1, 1, 0, %11;\n}\n" : SVCB_F8(0) : "l"(da), "l"(db), "r"(acc), "n"(TB));
   }
 };
+template <int TB> struct Wg<24, TB> {
+  static __device__ __forceinline__ void ss(float (&d)[12], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %14, 0;\nwgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 {" SVCB_R8_0
+                 ", %8, %9, %10, %11}, %12, %13, p, 1, 1, 0, %15;\n}\n" : SVCB_F8(0), SVCB_F4(8) : "l"(da), "l"(db), "r"(acc), "n"(TB));
+  }
+};
 template <int TB> struct Wg<32, TB> {
   static __device__ __forceinline__ void ss(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\nwgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {" SVCB_R8_0 ", " SVCB_R8_8

@@ -229,3 +229,21 @@ def hubert_checkpoint(seed: int = 1234, n_layer: int = 12):
     sd["proj.bias"] = r.n(256, std=0.05)
     sd["label_embedding.weight"] = r.n(100, 256, std=1.0)
     return {k: v.float().contiguous() for k, v in sd.items()}
+
+
+def speaker_checkpoint(seed: int = 1234):
+    """Synthetic LSTMSpeakerEncoder(80, 256, 768, 3) checkpoint {"model": state_dict} under the reference's keys
+    (speaker/models/lstm.py:8-20,35-47).  Weights are xavier-normal like `_init_layers`, but the biases are random too
+    (the reference zeroes them) so the bias paths are exercised."""
+    r = _Gen(seed)
+    H, P = 768, 256
+    sd: Dict[str, torch.Tensor] = {}
+    for l in range(3):
+        n_in = 80 if l == 0 else P
+        b = f"layers.{l}."
+        sd[b + "lstm.weight_ih_l0"] = r.n(4 * H, n_in, std=math.sqrt(2.0 / (4 * H + n_in)))
+        sd[b + "lstm.weight_hh_l0"] = r.n(4 * H, H, std=math.sqrt(2.0 / (5 * H)))
+        sd[b + "lstm.bias_ih_l0"] = r.n(4 * H, std=0.1)
+        sd[b + "lstm.bias_hh_l0"] = r.n(4 * H, std=0.1)
+        sd[b + "linear.weight"] = r.n(P, H, std=math.sqrt(2.0 / (P + H)))
+    return {"model": {k: v.float().contiguous() for k, v in sd.items()}}
