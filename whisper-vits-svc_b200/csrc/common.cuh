@@ -311,7 +311,7 @@ bool ups_fused_supported(int Cin, int Cout, int rate, int taps, int Kn);
 bool amp_block_fused_supported(int C, int K, const int* dil);
 
 // ----------------------------------------------------------------------------- general tensor-core conv
-constexpr int kConvTcKch = 32;   // input channels per chunk (the K of one A panel): 32 lets two CTAs share an SM
+constexpr int kConvTcKch = 32;   // input channels per chunk (the K of one A panel)
 struct ConvTcParams {
   const float* x = nullptr;
   long long sxb = 0, sxc = 0, sxt = 1;   // element strides of x[b, ci, t]

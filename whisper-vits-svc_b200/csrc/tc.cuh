@@ -282,6 +282,13 @@ __device__ __forceinline__ void acc_to_smem(const float (&d)[N / 2], float* buf,
   }
 }
 
+// warpgroup-wide register reallocation (all four warps of the warpgroup execute it): producer warpgroups give
+// registers back, MMA warpgroups take them
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // named barrier over `count` threads (a multiple of 32)
 __device__ __forceinline__ void named_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
