@@ -224,6 +224,37 @@ size_t svcb_ivf_workspace_bytes(const svcb_ivf* ix, int32_t M, int32_t k);
 int svcb_ivf_retrieve(const svcb_ivf* ix, const float* x, float* out, float* dist, int64_t* ids, int32_t M, int32_t k,
                       float ratio, void* ws, size_t ws_bytes, svcb_stream stream);
 
+/* ------------------------------------------------------------------ k-means (building IVF-Flat indexes) */
+/* Lloyd k-means as faiss 1.7.4's Clustering::train and IndexIVF::add run it for the reference's svc_train_retrieval.py
+ * (feature_retrieval/index.py:122-154), and in place of its MiniBatchKMeans compression (transform.py:29-53).
+ * Rows x [n, d] fp32 row-major (16-byte aligned), d % 64 == 0 and 64 <= d <= 2048, k >= 1 centroids.  The centroids
+ * enter the assignment as pack_ivf's "ivf.wimg" / "ivf.cnorm" (svcb_ivf_create), Np = k rounded up to 256. */
+
+/* Scratch for svcb_kmeans_assign (rows in chunks of `chunk`, 0 = 16384, rounded up to 128) and svcb_kmeans_update
+ * at (n, d, k).  About chunk x (6 d + Np / 2) bytes: 210 MB at d = 1280, k = 10,000 and the default chunk. */
+size_t svcb_kmeans_workspace_bytes(int32_t n, int32_t d, int32_t k, int32_t chunk);
+/* centroids [k, d] -> wimg [Np][3 d] bf16 tile image (Np x 3 d / 2 floats, 16-byte aligned) and cnorm [Np] (|c|^2 summed
+ * in fp64 and rounded once, +inf past k): the layout of retrieval.py:pack_ivf, built on the device between iterations. */
+int svcb_kmeans_pack(const float* centroids, float* wimg, float* cnorm, int32_t k, int32_t d, svcb_stream stream);
+/* Replaces the assignment step of Clustering::train and IndexIVF::add (quantizer->assign): assign [n] int32 the nearest
+ * centroid, chosen by bf16x3 on the tensor cores (ivf_coarse_tc) with ties to the lower centroid; dist [n] =
+ * max(|x|^2 + |c|^2 - 2 x.c, 0) as faiss reports it, in fp32 from centroids [k, d] (the fp32 rows wimg was packed from)
+ * and cnorm.  A row's result does not depend on n, the chunk or its position, and its centroid is the list
+ * svcb_ivf_retrieve probes first for that row over the same wimg / cnorm. */
+int svcb_kmeans_assign(const float* x, const float* centroids, const float* wimg, const float* cnorm, int32_t* assign,
+                       float* dist, int32_t n, int32_t d, int32_t k, int32_t chunk, void* ws, size_t ws_bytes,
+                       svcb_stream stream);
+/* Replaces compute_centroids (Clustering.cpp) and the list fill of IndexIVF::add: a stable counting sort of the rows by
+ * assign -> counts [k] (may be NULL), offsets [k + 1], order [n] (each centroid's rows ascending), then, when centroids
+ * is not NULL, centroid c = (fp32 sum of its rows in that order) x (1 / count); empty centroids are left untouched.
+ * Bitwise reproducible. */
+int svcb_kmeans_update(const float* x, const int32_t* assign, float* centroids, int32_t* counts, int32_t* offsets,
+                       int32_t* order, int32_t n, int32_t d, int32_t k, void* ws, size_t ws_bytes, svcb_stream stream);
+/* The perturbation of faiss's split_clusters for pairs [npairs][2] = (empty ci, split cj), applied in order:
+ * c_ci = c_cj, then even coordinates of c_ci x (1 + 1/1024) and of c_cj x (1 - 1/1024), odd ones the other way round.
+ * The choice of cj (a random walk over the counts) is the caller's. */
+int svcb_kmeans_split(float* centroids, const int32_t* pairs, int32_t npairs, int32_t d, svcb_stream stream);
+
 /* ------------------------------------------------------------------ speaker encoder (LSTM with projection) */
 typedef struct svcb_speaker svcb_speaker;
 /* Replaces LSTMSpeakerEncoder(80, 256, 768, 3) + load_checkpoint (speaker/models/lstm.py:35-60,124-131) and the

@@ -9,7 +9,7 @@ CREPE extractors when --ppg/--vec/--pit are missing (svc_inference.py:138-154). 
 checkpoints are available (whisper_pretrain/large-v2.pt, hubert_pretrain/hubert-soft-0d54a1f4.pt);
 CREPE is out of scope (SURVEY.md §8f-4), so --pit must be given.  --enable-retrieval reads the
 reference's faiss IVF-Flat indexes without faiss and runs the search and blend on the device
-(whisper-vits-svc_b200/retrieval.py)."""
+(whisper-vits-svc_b200/retrieval.py); svc_train_retrieval.py builds those indexes on the device."""
 import argparse
 import logging
 import os

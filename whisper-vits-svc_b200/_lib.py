@@ -93,6 +93,11 @@ SIGNATURES = {
     "svcb_ivf_destroy": (None, [c_void_p]),
     "svcb_ivf_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
     "svcb_ivf_retrieve": (c_int, [c_void_p] * 5 + [c_int32, c_int32, c_float, c_void_p, c_size_t, c_void_p]),
+    "svcb_kmeans_workspace_bytes": (c_size_t, [c_int32] * 4),
+    "svcb_kmeans_pack": (c_int, [c_void_p] * 3 + [c_int32] * 2 + [c_void_p]),
+    "svcb_kmeans_assign": (c_int, [c_void_p] * 6 + [c_int32] * 4 + [c_void_p, c_size_t, c_void_p]),
+    "svcb_kmeans_update": (c_int, [c_void_p] * 6 + [c_int32] * 3 + [c_void_p, c_size_t, c_void_p]),
+    "svcb_kmeans_split": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_void_p]),
     "svcb_speaker_create": (c_int, [c_void_p, c_size_t, POINTER(TensorEntry), c_int32, POINTER(c_void_p)]),
     "svcb_speaker_destroy": (None, [c_void_p]),
     "svcb_speaker_frames": (c_int32, [c_int64]),

@@ -401,5 +401,7 @@ int launch_ivf_pack(const float* x, void* img, int M, int d, cudaStream_t s);
 // gemm_tc epilogue 8 over that image and the centroid image: cand [M][N/16][nprobe] int2 {score bits, column}
 int launch_ivf_coarse_tc(const void* A_img, const void* W_img, const float* cnorm, void* cand, int M, int N, int K, int nprobe,
                          cudaStream_t s);
+// cursor[b] = sum_{b' < b} count[b'] over n buckets (ivf_order_kernel, one CTA)
+int launch_bucket_offsets(const int* count, int* cursor, int n, cudaStream_t s);
 
 }  // namespace svcb

@@ -208,6 +208,13 @@ ivf_scan_blend_kernel(const float* __restrict__ x, const int* __restrict__ order
                       __fadd_rn(__fmul_rn(omr, xv[i].y), __fmul_rn(ratio, bl[i].y)));
 }
 
+int launch_bucket_offsets(const int* count, int* cursor, int n, cudaStream_t s) {
+  KernelScope ks("bucket_offsets", s, 0.0, 8.0 * n);
+  ivf_order_kernel<<<1, 1024, 0, s>>>(count, cursor, n);
+  SVCB_LAUNCH_CHECK("bucket_offsets");
+  return SVCB_OK;
+}
+
 static size_t align256r(size_t x) { return (x + 255) & ~(size_t)255; }
 
 struct IvfLayout {

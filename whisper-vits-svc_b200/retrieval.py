@@ -148,6 +148,22 @@ def read_ivf_flat(path) -> IVFFlat:
                    vectors=vectors, ids=ids)
 
 
+def pack_centroids(centroids: np.ndarray) -> Tuple[torch.Tensor, torch.Tensor]:
+    """centroids [nlist, d] -> ("ivf.wimg", "ivf.cnorm"): the coarse search's bf16 tile image of [-2 c_hi | -2 c_hi | -2 c_lo]
+    and |c|^2 summed in float64 (+inf on the rows padding nlist to whole 256-column tiles), both CPU float32 tensors."""
+    nlist, d = centroids.shape
+    npad = (nlist + 255) // 256 * 256
+    c = torch.zeros(npad, d, dtype=torch.float32)
+    c[:nlist] = torch.from_numpy(np.ascontiguousarray(centroids, dtype=np.float32))
+    m2 = -2.0 * c                                        # exact: a power-of-two scale
+    hi = m2.bfloat16()
+    lo = (m2 - hi.float()).bfloat16()
+    wimg = _bf16_as_f32(torch.cat([hi, hi, lo], dim=1).float())   # pairs with the query image [x_hi | x_lo | x_hi]
+    cnorm = torch.full((npad,), float("inf"), dtype=torch.float32)
+    cnorm[:nlist] = torch.from_numpy((centroids.astype(np.float64) ** 2).sum(1).astype(np.float32))
+    return wimg, cnorm
+
+
 def pack_ivf(ix: IVFFlat) -> Tuple[List[Tuple[str, torch.Tensor]], _lib.IvfConfig]:
     """-> ([(name, fp32-typed tensor)], svcb_ivf_config).  Names consumed by csrc/retrieval_api.cu (include/svcb.h)."""
     if ix.d % 64 or not 64 <= ix.d <= 2048:
@@ -155,15 +171,7 @@ def pack_ivf(ix: IVFFlat) -> Tuple[List[Tuple[str, torch.Tensor]], _lib.IvfConfi
     if not 1 <= ix.nprobe <= MAX_NPROBE:
         raise IndexFormatError(f"index nprobe {ix.nprobe} is not supported: need 1 <= nprobe <= {MAX_NPROBE}")
     d, nlist = ix.d, ix.nlist
-    npad = (nlist + 255) // 256 * 256
-    c = torch.zeros(npad, d, dtype=torch.float32)
-    c[:nlist] = torch.from_numpy(ix.centroids)
-    m2 = -2.0 * c                                        # exact: a power-of-two scale
-    hi = m2.bfloat16()
-    lo = (m2 - hi.float()).bfloat16()
-    wimg = _bf16_as_f32(torch.cat([hi, hi, lo], dim=1).float())   # pairs with the query image [x_hi | x_lo | x_hi]
-    cnorm = torch.full((npad,), float("inf"), dtype=torch.float32)
-    cnorm[:nlist] = torch.from_numpy((ix.centroids.astype(np.float64) ** 2).sum(1).astype(np.float32))
+    wimg, cnorm = pack_centroids(ix.centroids)
     items = [
         ("ivf.wimg", wimg),
         ("ivf.cnorm", cnorm),
