@@ -169,6 +169,12 @@ size_t svcb_whisper_workspace_bytes(const svcb_whisper* w, int32_t B, int32_t n_
  * fp32 residual stream (the reference itself runs fp16 on GPU, whisper/inference.py:22-23). */
 int svcb_whisper_encode(const svcb_whisper* w, const float* mel, float* out, int32_t B, int32_t n_frames,
                         void* ws, size_t ws_bytes, svcb_stream stream);
+/* svcb_whisper_encode for a ragged batch: item b is the first n_frames_host[b] (1..n_frames) columns of its mel, and
+ * its columns past them must be zero (svcb_whisper_log_mel_ragged writes them so).  Item b's first
+ * (n_frames_host[b]-1)/2+1 output rows are bitwise those of a lone svcb_whisper_encode of its own frames; its later
+ * rows are zero.  ws_bytes >= svcb_whisper_workspace_bytes(w, B, n_frames) + 8 * B (the lengths are staged there). */
+int svcb_whisper_encode_ragged(const svcb_whisper* w, const float* mel, const int32_t* n_frames_host, float* out, int32_t B,
+                               int32_t n_frames, void* ws, size_t ws_bytes, svcb_stream stream);
 
 /* ------------------------------------------------------------------ content encoder (HuBERT-Soft, SURVEY 8f-2) */
 typedef struct svcb_hubert svcb_hubert;
@@ -188,6 +194,12 @@ size_t svcb_hubert_workspace_bytes(const svcb_hubert* h, int32_t B, int32_t n_sa
  * bit 1 = the grouped positional convolution likewise. */
 int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_t B, int32_t n_samples, void* ws,
                       size_t ws_bytes, float* const* taps, int32_t flags, svcb_stream stream);
+/* svcb_hubert_units (tensor-core stem, no taps) for a ragged batch: item b is the first n_samples_host[b] samples of its
+ * row of wav (1..n_samples, at least one frame each).  Item b's first svcb_hubert_frames(n_samples_host[b]) output rows
+ * are bitwise those of a lone svcb_hubert_units of its own samples; its later rows are zero.
+ * ws_bytes >= svcb_hubert_workspace_bytes(h, B, n_samples) + 8 * B (the lengths are staged there). */
+int svcb_hubert_units_ragged(const svcb_hubert* h, const float* wav, const int32_t* n_samples_host, float* out, int32_t B,
+                             int32_t n_samples, void* ws, size_t ws_bytes, svcb_stream stream);
 
 /* Replaces whisper.audio.log_mel_spectrogram (whisper/audio.py:68-100) plus the extractor's mel noise
  * (whisper/inference.py:46,58) for B equal-length chunks of 16 kHz audio already on the device:
@@ -197,6 +209,11 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
 int svcb_whisper_log_mel(const float* audio, const float* mel_filters, const float* noise, float noise_gain,
                          float* mel, void* scratch, int32_t B, int32_t n_samples, int32_t n_mels,
                          svcb_stream stream);
+/* svcb_whisper_log_mel without noise for a ragged batch: item b is the first n_samples_host[b] (201..n_samples) samples
+ * of its row of audio, reflect-padded at its own end and floored at the max over its own n_samples_host[b]/160 frames,
+ * which are bitwise those of a lone svcb_whisper_log_mel; its later frames are zero.  scratch: >= 8*B bytes. */
+int svcb_whisper_log_mel_ragged(const float* audio, const int32_t* n_samples_host, const float* mel_filters, float* mel,
+                                void* scratch, int32_t B, int32_t n_samples, int32_t n_mels, svcb_stream stream);
 
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).

@@ -7,11 +7,9 @@ Files run on the H100 in ragged batches of up to --batch utterances; -t sets the
 normalise the wavs, at most two batches ahead of the device.  A file that fails is reported and skipped; if a
 batch fails on the device, its files are retried one by one so only the failing file is lost."""
 import argparse
-import collections
 import os
 import sys
 from argparse import RawTextHelpFormatter
-from concurrent.futures import ThreadPoolExecutor
 
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
@@ -40,54 +38,13 @@ def embed_path(wav_file, dataset_path, output_path):
 def extract_speaker_embeddings(wav_files, dataset_path, output_path, model, concurrency, batch=32):
     """Embed every file in device batches; returns the number of files that failed (each is reported and skipped).
     The loader threads run at most two batches ahead of the device, so host memory stays bounded."""
-    def load(f):
-        try:
-            return f, model.load_wav(f), None
-        except Exception as e:
-            return f, None, e
+    from whisper_vits_svc_b200 import dataset
 
-    def save(items):
-        embeds = model.embed([w for _, w in items]).cpu().numpy().astype(np.float32)
-        for (f, _), e in zip(items, embeds):
-            np.save(embed_path(f, dataset_path, output_path), e, allow_pickle=False)
+    def save(f, e):
+        np.save(embed_path(f, dataset_path, output_path), e, allow_pickle=False)
 
-    failed = 0
-    pending = collections.deque()
-    files = iter(wav_files)
-    with ThreadPoolExecutor(max(1, concurrency)) as pool:
-        def refill():
-            while len(pending) < 2 * batch:
-                f = next(files, None)
-                if f is None:
-                    return
-                pending.append(pool.submit(load, f))
-
-        done = 0
-        refill()
-        while pending:
-            chunk = [pending.popleft().result() for _ in range(min(batch, len(pending)))]
-            refill()
-            done += len(chunk)
-            good = []
-            for f, wav, err in chunk:
-                if err is None:
-                    good.append((f, wav))
-                else:
-                    failed += 1
-                    print(f"[!] skipped {f}: {err}", file=sys.stderr)
-            if not good:
-                continue
-            try:
-                save(good)
-            except Exception:
-                for item in good:   # find the file the batch failed on; the others are still written
-                    try:
-                        save([item])
-                    except Exception as e:
-                        failed += 1
-                        print(f"[!] skipped {item[0]}: {e}", file=sys.stderr)
-            print(f"{done}/{len(wav_files)}")
-    return failed
+    return dataset.run_batched(wav_files, model.load_wav, lambda wavs: model.embed(wavs).cpu().numpy().astype(np.float32),
+                               save, concurrency, batch)["failed"]
 
 
 if __name__ == "__main__":

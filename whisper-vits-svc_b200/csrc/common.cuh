@@ -305,8 +305,9 @@ struct UpsFusedParams {
   long long Ltot = 0;
 };
 int launch_ups_fused(const UpsFusedParams& p, cudaStream_t s);
+// lens (device, may be null): per-item sample counts of a ragged batch, each in [201, N]
 int launch_log_mel(const float* audio, const float* filt, const float* noise, float gain, float* out,
-                   unsigned* scratch, int B, int N, int n_mels, cudaStream_t s);
+                   unsigned* scratch, int B, int N, int n_mels, cudaStream_t s, const int* lens = nullptr);
 bool ups_fused_supported(int Cin, int Cout, int rate, int taps, int Kn);
 bool amp_block_fused_supported(int C, int K, const int* dil);
 
@@ -382,15 +383,23 @@ int launch_source2wav(const float* src, int16_t* out, size_t n, cudaStream_t s);
 // bf16 wgmma GEMM over tile images with fused epilogues (each one is described in whisper_gemm.cu)
 enum GemmEpi : int { EPI_BF16_ROWMAJOR = 0, EPI_GELU_BF16_IMAGE = 1, EPI_RESID_F32 = 2, EPI_GELU_ADD_F32 = 3, EPI_QKV_HEADS = 4,
                      EPI_GELU_CONV2_IMG = 5, EPI_GELU_VALID_S2_IMG = 6, EPI_GELU_ADD_F32_LD = 7, EPI_IVF_TOPK = 8 };
+// lens (device, may be null): per-item frame counts of a ragged batch, read by epilogue 5 only
 int launch_gemm_tc(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
-                   int M, int N, int K, GemmEpi epi, cudaStream_t s, int res_mod = 0, int aux = 0);
+                   int M, int N, int K, GemmEpi epi, cudaStream_t s, int res_mod = 0, int aux = 0, const int* lens = nullptr);
 int launch_im2col_s1_image(const float* mel, void* img, int B, int n_mels, int n, cudaStream_t s);
 int launch_im2col_s2_image(const float* h1, void* img, int B, int D, int n, int n2, cudaStream_t s, int taps = 3, int pad = 1);
-int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s);
+int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s,
+                             const int* lens = nullptr);
+// ragged batches: host ints -> device dst[0, n), stream-ordered, without a host-to-device copy
+int launch_stage_ints(const int* host, int n, int* dst, cudaStream_t s);
+// ragged batches: zero the rows t >= lens[b] (device array, every lens[b] >= min_len) of each item of fp32 [B * T, width]
+int launch_zero_tail_rows(float* out, const int* lens, int B, int T, int width, int min_len, cudaStream_t s);
 int launch_rowmajor_to_image(const void* src, void* dst, int R, int K, int rows, cudaStream_t s);
 int launch_image_to_rowmajor(const void* src, void* dst, int R, int K, cudaStream_t s);
 int launch_qkv_rowmajor_to_heads(const void* src, void* dst, int B, int T, int D, cudaStream_t s);
-int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T, int D, int heads, int vswap, cudaStream_t s);
+// lens (device, may be null): per-item position counts of a ragged batch, each in [1, T]
+int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T, int D, int heads, int vswap, cudaStream_t s,
+                                const int* lens = nullptr);
 // row LayerNorm of fp32 [M, D]: bf16 tile image (A operand of the next GEMM; y32 also gets the fp32 rows) or fp32 rows
 int launch_ln_rows(const float* x, const float* gamma, const float* beta, void* y, int M, int D, bool out_bf16,
                    cudaStream_t s, float* y32 = nullptr);

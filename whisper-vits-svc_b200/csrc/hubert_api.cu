@@ -16,6 +16,11 @@
 // Positional conv (Conv1d(768, 768, 128, groups 16): 9.4 GFLOP per 1000 frames): per group an im2col tile image
 // (K = 128 taps x 48 channels) times a [256 (48 used), K] weight image, epilogue 7 = GELU + residual into the group's 48
 // columns of the 768-wide rows; flags bit 1 selects the fp32 CUDA-core form (32 `conv1d` launches, 16 ms per 16 x 20 s).
+// Ragged batches (svcb_hubert_units_ragged): item b is its first n_b samples, T_b = svcb_hubert_frames(n_b).  Samples past
+// n_b read as conv0's zero padding, the GroupNorm statistics cover the item's own conv0 frames, the positional conv
+// reads rows past T_b as zeros and attention masks keys past T_b; the stride-2 stem convs are valid convolutions,
+// whose first T_b frames never read later ones.  Everything else is row-local, so an item's rows are the bits a lone
+// run computes, and the rows past T_b stay finite (attention reads them as V rows times P = 0).
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -73,23 +78,24 @@ groupnorm_gelu_rows_kernel(float* __restrict__ x, const float* __restrict__ gamm
 // load issue: 10 LDG per FMA chain, 1.8 ms per 16 x 20 s).
 __global__ void __launch_bounds__(256)
 hubert_conv0_stats_kernel(const float* __restrict__ wav, const float* __restrict__ w0, float2* __restrict__ stats, int N,
-                          int T0, float eps) {
+                          int T0, float eps, const int* __restrict__ lens) {
   __shared__ double red[16][8];
   __shared__ float ws[10][8];
   const int oc = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid < 80) ws[tid >> 3][tid & 7] = __ldg(w0 + (tid >> 3) * HB_C + oc * 8 + (tid & 7));   // packed [1][10][512]
   __syncthreads();
   const float* xb = wav + (size_t)b * N;
+  const int Nb = lens ? __ldg(lens + b) : N, T0b = lens ? (Nb + 80 - 10) / 5 + 1 : T0;   // the item's own samples and frames
   double s[8], q[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) { s[e] = 0.0; q[e] = 0.0; }
-  for (int t = tid; t < T0; t += 256) {
+  for (int t = tid; t < T0b; t += 256) {
     const int i0 = 5 * t - 40;
     float x[10];
 #pragma unroll
     for (int j = 0; j < 10; ++j) {
       const int i = i0 + j;
-      x[j] = (i >= 0 && i < N) ? __ldg(xb + i) : 0.f;
+      x[j] = (i >= 0 && i < Nb) ? __ldg(xb + i) : 0.f;
     }
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
@@ -109,7 +115,8 @@ hubert_conv0_stats_kernel(const float* __restrict__ wav, const float* __restrict
   if (tid < 8) {
     double S = 0.0, Q = 0.0;
     for (int i = 0; i < 8; ++i) { S += red[tid][i]; Q += red[8 + tid][i]; }
-    const double mean = S / T0, var = Q / T0 - mean * mean;
+    const int nf = lens ? (__ldg(lens + b) + 80 - 10) / 5 + 1 : T0;
+    const double mean = S / nf, var = Q / nf - mean * mean;
     stats[(size_t)b * HB_C + oc * 8 + tid] = make_float2((float)mean, (float)(1.0 / sqrt((var > 0.0 ? var : 0.0) + (double)eps)));
   }
 }
@@ -119,7 +126,7 @@ hubert_conv0_stats_kernel(const float* __restrict__ wav, const float* __restrict
 __global__ void __launch_bounds__(128)
 hubert_conv0_pack_kernel(const float* __restrict__ wav, const float* __restrict__ w0, const float2* __restrict__ stats,
                          const float* __restrict__ gamma, const float* __restrict__ beta, __nv_bfloat16* __restrict__ img,
-                         int N, int T0, int T1) {
+                         int N, int T0, int T1, const int* __restrict__ lens) {
   __shared__ float ws[10][8];
   __shared__ float2 aff[8];   // y -> y * aff.x + aff.y  (normalisation and affine folded)
   const int oc = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
@@ -134,11 +141,12 @@ hubert_conv0_pack_kernel(const float* __restrict__ wav, const float* __restrict_
   const int t = blockIdx.x * 128 + tid;
   if (t >= T0) return;
   const float* xb = wav + (size_t)b * N;
+  const int Nb = lens ? __ldg(lens + b) : N;
   float x[10];
 #pragma unroll
   for (int j = 0; j < 10; ++j) {
     const int i = 5 * t - 40 + j;
-    x[j] = (i >= 0 && i < N) ? __ldg(xb + i) : 0.f;
+    x[j] = (i >= 0 && i < Nb) ? __ldg(xb + i) : 0.f;
   }
   __align__(16) __nv_bfloat16 hv[8];
 #pragma unroll
@@ -261,15 +269,38 @@ size_t svcb_hubert_workspace_bytes(const svcb_hubert* h, int32_t B, int32_t n_sa
   return hubert_layout(B, n_samples).total;
 }
 
-int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_t B, int32_t n_samples, void* ws,
-                      size_t ws_bytes, float* const* taps, int32_t flags, svcb_stream stream) {
+}  // extern "C"
+
+// lens_host: null, or per-item sample counts of a ragged batch (flags 0 only), staged in 8 B bytes past L.total
+static int hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_t B, int32_t n_samples, void* ws,
+                        size_t ws_bytes, float* const* taps, int32_t flags, const int32_t* lens_host, cudaStream_t s) {
   if (!h || !wav || !out || B <= 0 || n_samples <= 0) { set_error("svcb_hubert_units: bad argument"); return SVCB_E_BAD_SHAPE; }
   const HLayout L = hubert_layout(B, n_samples);
   const int T = L.T[6], M = L.M;
   if (T < 1) { set_error("svcb_hubert_units: audio shorter than one frame"); return SVCB_E_BAD_SHAPE; }
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < L.total) { set_error("hubert workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<int> lens;   // [samples of item 0 .. B-1][frames of item 0 .. B-1]
+  if (lens_host) {
+    lens.resize(2 * (size_t)B);
+    for (int b = 0; b < B; ++b) {
+      const int n = lens_host[b], f = n > 0 ? hubert_layout(1, n).T[6] : 0;
+      if (n < 1 || n > n_samples || f < 1) {
+        set_error("svcb_hubert_units_ragged: item " + std::to_string(b) + " has " + std::to_string(n) + " samples; need 1.." +
+                  std::to_string(n_samples) + " and at least one frame");
+        return SVCB_E_BAD_SHAPE;
+      }
+      lens[b] = n; lens[B + b] = f;
+    }
+  }
+  const size_t need = L.total + (lens_host ? 8 * (size_t)B : 0);
+  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < need) { set_error("hubert workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
   char* base = static_cast<char*>(ws);
+  const int* d_samples = nullptr;
+  const int* d_frames = nullptr;
+  if (lens_host) {
+    int* d = reinterpret_cast<int*>(base + L.total);
+    SVCB_TRY(launch_stage_ints(lens.data(), (int)lens.size(), d, s));
+    d_samples = d; d_frames = d + B;
+  }
   float* bufa = reinterpret_cast<float*>(base + L.bufa);
   float* bufb = reinterpret_cast<float*>(base + L.bufb);
   float* rows = reinterpret_cast<float*>(base + L.rows);
@@ -300,13 +331,13 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
       float2* stats = reinterpret_cast<float2*>(base + L.stats);
       {
         KernelScope ks("hubert_conv0_stats", s, 20.0 * B * HB_C * (double)L.T[0], 4.0 * B * (double)n_samples);
-        hubert_conv0_stats_kernel<<<dim3(HB_C / 8, B), 256, 0, s>>>(wav, h->conv0_w, stats, n_samples, L.T[0], 1e-5f);
+        hubert_conv0_stats_kernel<<<dim3(HB_C / 8, B), 256, 0, s>>>(wav, h->conv0_w, stats, n_samples, L.T[0], 1e-5f, d_samples);
         SVCB_LAUNCH_CHECK("hubert_conv0_stats");
       }
       {
         KernelScope ks("hubert_conv0_pack", s, 20.0 * B * HB_C * (double)L.T[0], 4.0 * B * (double)n_samples + 2.0 * B * 3 * HB_C * (double)L.T[1]);
         hubert_conv0_pack_kernel<<<dim3((L.T[0] + 127) / 128, HB_C / 8, B), 128, 0, s>>>(
-            wav, h->conv0_w, stats, h->gn_g, h->gn_b, static_cast<__nv_bfloat16*>(img[0]), n_samples, L.T[0], L.T[1]);
+            wav, h->conv0_w, stats, h->gn_g, h->gn_b, static_cast<__nv_bfloat16*>(img[0]), n_samples, L.T[0], L.T[1], d_samples);
         SVCB_LAUNCH_CHECK("hubert_conv0_pack");
       }
     }
@@ -340,7 +371,7 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
   // y = x + GELU(pos_conv(x)[..., :-1]): 16 groups of 48 channels, 128 taps, two 24-channel halves per group
   for (int g = 0; g < HB_PG && !(flags & 2); ++g) {   // tensor cores: per group an im2col image (K = 128 x 48) x [256 (48 used), K]
     const int cg = HB_D / HB_PG, c0 = g * cg;
-    SVCB_TRY(launch_im2col_rows_image(x, base + L.posimg, B, T, HB_D, c0, cg, HB_PK, HB_PK / 2, s));
+    SVCB_TRY(launch_im2col_rows_image(x, base + L.posimg, B, T, HB_D, c0, cg, HB_PK, HB_PK / 2, s, d_frames));
     SVCB_TRY(launch_gemm_tc(base + L.posimg, h->pos_wimg[g], h->pos_bimg[g], y + c0, x + c0, M, 256, HB_PK * cg, EPI_GELU_ADD_F32_LD, s, cg, HB_D));
   }
   for (int g = 0; g < HB_PG && (flags & 2); ++g)       // flags bit 1: fp32 on the CUDA cores
@@ -361,7 +392,7 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
   for (int i = 0; i < h->n_layer; ++i) {   // post-LN layers: x = LN1(x + SA(x)); x = LN2(x + W2 gelu(W1 x))
     const HLayer& l = h->layers[i];
     SVCB_TRY(launch_gemm_tc(a, l.wqkv, l.bqkv, qkv, nullptr, M, 3 * HB_D, HB_D, EPI_QKV_HEADS, s, T));
-    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, T, HB_D, HB_H, 0, s));
+    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, T, HB_D, HB_H, 0, s, d_frames));
     SVCB_TRY(launch_gemm_tc(att, l.wo, l.bo, y, x, M, HB_D, HB_D, EPI_RESID_F32, s));
     SVCB_TRY(launch_ln_rows(y, l.ln1g, l.ln1b, a, M, HB_D, true, s, x));
     SVCB_TRY(launch_gemm_tc(a, l.w1, l.b1, mid, nullptr, M, HB_FF, HB_D, EPI_GELU_BF16_IMAGE, s));
@@ -370,7 +401,22 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
     if (i == 0) SVCB_TRY(tap(3, x, (size_t)M * HB_D));
   }
   SVCB_TRY(tap(4, x, (size_t)M * HB_D));
-  return launch_gemm_tc(a, h->proj_w, h->proj_b, out, nullptr, M, HB_OUT, HB_D, EPI_RESID_F32, s);
+  SVCB_TRY(launch_gemm_tc(a, h->proj_w, h->proj_b, out, nullptr, M, HB_OUT, HB_D, EPI_RESID_F32, s));
+  if (!lens_host) return SVCB_OK;
+  return launch_zero_tail_rows(out, d_frames, B, T, HB_OUT, *std::min_element(lens.begin() + B, lens.end()), s);
+}
+
+extern "C" {
+
+int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_t B, int32_t n_samples, void* ws,
+                      size_t ws_bytes, float* const* taps, int32_t flags, svcb_stream stream) {
+  return hubert_units(h, wav, out, B, n_samples, ws, ws_bytes, taps, flags, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int svcb_hubert_units_ragged(const svcb_hubert* h, const float* wav, const int32_t* n_samples_host, float* out, int32_t B,
+                             int32_t n_samples, void* ws, size_t ws_bytes, svcb_stream stream) {
+  if (!n_samples_host) { set_error("svcb_hubert_units_ragged: null lengths"); return SVCB_E_BAD_SHAPE; }
+  return hubert_units(h, wav, out, B, n_samples, ws, ws_bytes, nullptr, 0, n_samples_host, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

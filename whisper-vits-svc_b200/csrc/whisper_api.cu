@@ -3,6 +3,11 @@
 //   conv1+GELU (GEMM over an im2col image of the log-mel; its epilogue scatters into conv2's im2col image) ->
 //   conv2(stride 2)+GELU+pos-emb (GEMM) -> n_layer x { LN -> QKV GEMM (head-major panels) -> wgmma attention
 //   (whisper_attn_tc.cu) -> out-proj GEMM (+residual) -> LN -> MLP GEMM+GELU -> MLP GEMM (+residual) } -> ln_post
+// Ragged batches (the *_ragged entry points): item b has its own length, its log-mel frames past F_b are zeros (conv1's
+// padding), conv1 scatters its frames past F_b into conv2's image as zeros (conv2's padding: for odd F_b the last
+// position reads h1[F_b]), and attention masks keys past T_b = (F_b - 1) / 2 + 1.  The other stages are row-local, so
+// an item's rows are the bits a lone run of it computes.
+#include <algorithm>
 #include <memory>
 #include <string>
 #include <vector>
@@ -92,15 +97,37 @@ size_t svcb_whisper_workspace_bytes(const svcb_whisper* w, int32_t B, int32_t n_
   return whisper_layout(w->cfg, B, n_frames).total;
 }
 
-int svcb_whisper_encode(const svcb_whisper* w, const float* mel, float* out, int32_t B, int32_t n_frames,
-                        void* ws, size_t ws_bytes, svcb_stream stream) {
+}  // extern "C"
+
+// frames_host: null, or per-item mel frame counts of a ragged batch, staged in 8 B bytes past L.total
+static int whisper_encode(const svcb_whisper* w, const float* mel, float* out, int32_t B, int32_t n_frames, void* ws,
+                          size_t ws_bytes, const int32_t* frames_host, cudaStream_t s) {
   if (!w || !mel || !out || B <= 0 || n_frames <= 0) { set_error("svcb_whisper_encode: bad argument"); return SVCB_E_BAD_SHAPE; }
   const svcb_whisper_config& c = w->cfg;
   const WLayout L = whisper_layout(c, B, n_frames);
   if (L.n2 > c.n_ctx) { set_error("incorrect audio shape: more than n_audio_ctx positions"); return SVCB_E_BAD_SHAPE; }
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < L.total) { set_error("whisper workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<int> lens;   // [frames of item 0 .. B-1][positions of item 0 .. B-1]
+  if (frames_host) {
+    lens.resize(2 * (size_t)B);
+    for (int b = 0; b < B; ++b) {
+      if (frames_host[b] < 1 || frames_host[b] > n_frames) {
+        set_error("svcb_whisper_encode_ragged: item " + std::to_string(b) + " has " + std::to_string(frames_host[b]) +
+                  " frames; need 1.." + std::to_string(n_frames));
+        return SVCB_E_BAD_SHAPE;
+      }
+      lens[b] = frames_host[b]; lens[B + b] = (frames_host[b] - 1) / 2 + 1;
+    }
+  }
+  const size_t need = L.total + (frames_host ? 8 * (size_t)B : 0);
+  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < need) { set_error("whisper workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
   char* base = static_cast<char*>(ws);
+  const int* d_frames = nullptr;
+  const int* d_pos = nullptr;
+  if (frames_host) {
+    int* d = reinterpret_cast<int*>(base + L.total);
+    SVCB_TRY(launch_stage_ints(lens.data(), (int)lens.size(), d, s));
+    d_frames = d; d_pos = d + B;
+  }
   void* a1 = base + L.h1;
   float* x = reinterpret_cast<float*>(base + L.x);
   void* a = base + L.a; void* qkv = base + L.qkv; void* att = base + L.att; void* mid = base + L.mid;
@@ -111,7 +138,7 @@ int svcb_whisper_encode(const svcb_whisper* w, const float* mel, float* out, int
   // CUDA-core conv1 + the separate im2col pass were 2.0 of the encoder's 33.6 ms.)
   SVCB_CUDA_CHECK(cudaMemsetAsync(mid, 0, (size_t)(M + 127) / 128 * 128 * 3 * D * 2, s));
   SVCB_TRY(launch_im2col_s1_image(mel, a1, B, c.n_mels, n, s));
-  SVCB_TRY(launch_gemm_tc(a1, w->conv1_wimg, w->conv1_b, mid, nullptr, B * n, D, (3 * c.n_mels + 63) / 64 * 64, EPI_GELU_CONV2_IMG, s, n));
+  SVCB_TRY(launch_gemm_tc(a1, w->conv1_wimg, w->conv1_b, mid, nullptr, B * n, D, (3 * c.n_mels + 63) / 64 * 64, EPI_GELU_CONV2_IMG, s, n, 0, d_frames));
   // conv2 (k=3, stride 2) + GELU + positional embedding, time-major (:150-157): im2col image x the [D, 3D] weight image
   SVCB_TRY(launch_gemm_tc(mid, w->conv2_wimg, w->conv2_b, x, w->pos, M, D, 3 * D, EPI_GELU_ADD_F32, s, n2));
   // pad positions of the head-major QKV buffer are read (times P = 0) but never written: keep them finite
@@ -120,15 +147,29 @@ int svcb_whisper_encode(const svcb_whisper* w, const float* mel, float* out, int
     const WBlock& b = w->blocks[i];
     SVCB_TRY(launch_ln_rows(x, b.ln1g, b.ln1b, a, M, D, true, s));
     SVCB_TRY(launch_gemm_tc(a, b.wqkv, b.bqkv, qkv, nullptr, M, 3 * D, D, EPI_QKV_HEADS, s, n2));
-    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, n2, D, c.n_head, 0, s));
+    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, n2, D, c.n_head, 0, s, d_pos));
     SVCB_TRY(launch_gemm_tc(att, b.wo, b.bo, x, x, M, D, D, EPI_RESID_F32, s));
     SVCB_TRY(launch_ln_rows(x, b.ln2g, b.ln2b, a, M, D, true, s));
     SVCB_TRY(launch_gemm_tc(a, b.w1, b.b1, mid, nullptr, M, 4 * D, D, EPI_GELU_BF16_IMAGE, s));
     SVCB_TRY(launch_gemm_tc(mid, b.w2, b.b2, x, x, M, D, 4 * D, EPI_RESID_F32, s));
   }
-  return launch_ln_rows(x, w->lnp_g, w->lnp_b, out, M, D, false, s);
+  SVCB_TRY(launch_ln_rows(x, w->lnp_g, w->lnp_b, out, M, D, false, s));
+  if (!frames_host) return SVCB_OK;
+  return launch_zero_tail_rows(out, d_pos, B, n2, D, *std::min_element(lens.begin() + B, lens.end()), s);
 }
 
+extern "C" {
+
+int svcb_whisper_encode(const svcb_whisper* w, const float* mel, float* out, int32_t B, int32_t n_frames,
+                        void* ws, size_t ws_bytes, svcb_stream stream) {
+  return whisper_encode(w, mel, out, B, n_frames, ws, ws_bytes, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int svcb_whisper_encode_ragged(const svcb_whisper* w, const float* mel, const int32_t* n_frames_host, float* out, int32_t B,
+                               int32_t n_frames, void* ws, size_t ws_bytes, svcb_stream stream) {
+  if (!n_frames_host) { set_error("svcb_whisper_encode_ragged: null lengths"); return SVCB_E_BAD_SHAPE; }
+  return whisper_encode(w, mel, out, B, n_frames, ws, ws_bytes, n_frames_host, static_cast<cudaStream_t>(stream));
+}
 
 int svcb_whisper_log_mel(const float* audio, const float* mel_filters, const float* noise, float noise_gain,
                          float* mel, void* scratch, int32_t B, int32_t n_samples, int32_t n_mels,
@@ -137,6 +178,24 @@ int svcb_whisper_log_mel(const float* audio, const float* mel_filters, const flo
   if (B < 0 || n_samples < 0 || n_mels <= 0) { set_error("log_mel: bad shape"); return SVCB_E_BAD_SHAPE; }
   return launch_log_mel(audio, mel_filters, noise, noise_gain, mel, static_cast<unsigned*>(scratch), B, n_samples,
                         n_mels, static_cast<cudaStream_t>(stream));
+}
+
+int svcb_whisper_log_mel_ragged(const float* audio, const int32_t* n_samples_host, const float* mel_filters, float* mel,
+                                void* scratch, int32_t B, int32_t n_samples, int32_t n_mels, svcb_stream stream) {
+  if (!audio || !n_samples_host || !mel_filters || !mel || !scratch) { set_error("log_mel_ragged: null pointer"); return SVCB_E_BAD_SHAPE; }
+  if (B < 0 || n_samples < 0 || n_mels <= 0) { set_error("log_mel_ragged: bad shape"); return SVCB_E_BAD_SHAPE; }
+  for (int b = 0; b < B; ++b)
+    if (n_samples_host[b] <= 200 || n_samples_host[b] > n_samples) {
+      set_error("svcb_whisper_log_mel_ragged: item " + std::to_string(b) + " has " + std::to_string(n_samples_host[b]) +
+                " samples; need 201.." + std::to_string(n_samples) + " (the reflect padding needs more than 200)");
+      return SVCB_E_BAD_SHAPE;
+    }
+  if (B == 0) return SVCB_OK;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  unsigned* mx = static_cast<unsigned*>(scratch);
+  int* d_lens = reinterpret_cast<int*>(mx + B);
+  SVCB_TRY(launch_stage_ints(n_samples_host, B, d_lens, s));
+  return launch_log_mel(audio, mel_filters, nullptr, 0.f, mel, mx, B, n_samples, n_mels, s, d_lens);
 }
 
 size_t svcb_op_gemm_bf16_scratch_bytes(int32_t M, int32_t N, int32_t K) {

@@ -15,6 +15,10 @@
 // One CTA = (item, head, 128 queries): two warpgroups of 64 query rows (online softmax over the 64-key tiles,
 // four threads per row) and a producer warp (one 8 KB bulk copy per K / V tile into a 4-slot ring).
 // The output is written as the tile image the out-projection consumes.
+// Ragged batches (lens != null): item b attends over its first T_b = lens[b] keys only; its key loop stops at
+// ceil(T_b / 64) tiles, as a lone run of T_b positions does, so each of its query rows gets the same bits.  Query
+// tiles wholly past T_b write zeros: the next layers still read those rows (a masked key's P = 0 times its V row),
+// so they must stay finite.
 #include <cstdint>
 
 #include "common.cuh"
@@ -43,7 +47,7 @@ __device__ __forceinline__ uint32_t wa_pack(float a, float b) {
 
 __global__ void __launch_bounds__(wa::THREADS, wa::CTAS_PER_SM)
 whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out_img, int T, int Dm,
-                       int vswap) {
+                       int vswap, const int* __restrict__ lens) {
   using namespace wa;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t q_full, r_full[NS], r_empty[NS];
@@ -51,7 +55,8 @@ whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __r
   const int warp_u = tc::warp_uniform_idx();
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int heads = Dm / 64, Tp = qkv_heads_tp(T);
-  const int nk = (T + TK - 1) / TK;
+  const int Tb = lens ? __ldg(lens + b) : T;
+  const int nk = qt * TQ < Tb ? (Tb + TK - 1) / TK : 0;   // 0: a query tile past the item's end, written as zeros
   const int m_item = b * T;                       // first flat row of the item
   if (tid == 0) {
     tc::mbar_init(&q_full, 1);
@@ -107,7 +112,7 @@ whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __r
       tc::wg_hold(sc);
       if (t == 0) tc::mbar_arrive(&r_empty[slot]);
     }
-    const int nvalid = T - kt * TK;              // >= 64 except in the item's last tile
+    const int nvalid = Tb - kt * TK;             // >= 64 except in the item's last tile
     if (nvalid < TK) {
 #pragma unroll
       for (int i = 0; i < 8; ++i)
@@ -149,7 +154,7 @@ whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __r
   }
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  const float i0 = 1.f / l0, i1 = 1.f / l1;
+  const float i0 = nk ? 1.f / l0 : 0.f, i1 = nk ? 1.f / l1 : 0.f;
   // O / sum(p) -> bf16, written as the A tile image of the out-projection ([M/128][D/64][8][128][8])
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
@@ -168,14 +173,14 @@ whisper_attn_tc_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __r
 // qkv: head-major layout of common.cuh (B x 3 x heads blocks of Tp x 64, pad rows finite);
 // out_img: tile image of [B*T, D]
 int launch_whisper_attention_tc(const void* qkv_img, void* out_img, int B, int T, int D, int heads, int vswap,
-                                cudaStream_t s) {
+                                cudaStream_t s, const int* lens) {
   if (D != heads * 64 || D % 64) { set_error("whisper_attention_tc: head dim must be 64"); return SVCB_E_UNSUPPORTED; }
   if (B <= 0 || T <= 0) return SVCB_OK;
   static DevSmemCache attr_cache;
   SVCB_CUDA_CHECK(ensure_dyn_smem(whisper_attn_tc_kernel, wa::SMEM, attr_cache));
   KernelScope ks("whisper_attn_tc", s, 4.0 * B * (double)T * T * D, 2.0 * 4 * B * (double)T * D);
   whisper_attn_tc_kernel<<<dim3((T + wa::TQ - 1) / wa::TQ, heads, B), wa::THREADS, wa::SMEM, s>>>(
-      static_cast<const __nv_bfloat16*>(qkv_img), static_cast<__nv_bfloat16*>(out_img), T, D, vswap);
+      static_cast<const __nv_bfloat16*>(qkv_img), static_cast<__nv_bfloat16*>(out_img), T, D, vswap, lens);
   SVCB_LAUNCH_CHECK("whisper_attn_tc");
   return SVCB_OK;
 }

@@ -30,7 +30,8 @@ namespace svcb {
 //    N = 3 D, rows are items of res_mod positions each; pad rows are zeroed by the caller once)
 // 5: the stem's conv1 (rows = items x res_mod frames): GELU(acc + bias) scattered straight into conv2's im2col tile
 //    image A2[b * n2 + t2][j * N + co] = h1[b][co][2 t2 + j - 1] (frame t feeds (t/2, j=1) when even, ((t+1)/2, j=0)
-//    and ((t-1)/2, j=2) when odd) — no h1 tensor, no im2col pass; the caller zeroes the image once (t = -1 taps, pad rows)
+//    and ((t-1)/2, j=2) when odd) — no h1 tensor, no im2col pass; the caller zeroes the image once (t = -1 taps, pad rows).
+//    lens (ragged batches, may be null): frames t >= lens[b] are scattered as zeros, conv2's zero padding of item b
 // 6: a stride-2 VALID convolution of the HuBERT stem feeding the next one (rows = items x res_mod frames, aux = taps of
 //    the NEXT conv, 2 or 3): GELU(acc + bias) scattered into the next conv's im2col tile image
 //    A[b * Tn + t2][j * N + co] = h[b][co][2 t2 + j], Tn = (res_mod - aux) / 2 + 1 (every entry of the image is written)
@@ -52,7 +53,8 @@ __host__ __device__ inline size_t img_off(int m, int k, int KT) {
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GM_THREADS, 1)
 gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __restrict__ Wimg,
-               const float* __restrict__ bias, void* out, const float* res, int M, int N, int K, int res_mod, int aux) {
+               const float* __restrict__ bias, void* out, const float* res, int M, int N, int K, int res_mod, int aux,
+               const int* __restrict__ lens) {
   constexpr uint32_t A_BYTES = GM_BM * GM_BK * 2, B_BYTES = BN * GM_BK * 2, ST_BYTES = A_BYTES + B_BYTES;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t bar_full[GM_STAGES], bar_empty[GM_STAGES];
@@ -202,7 +204,9 @@ gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __re
               __nv_bfloat16* ob = static_cast<__nv_bfloat16*>(out);
               const int nfr = res_mod, n2 = (nfr - 1) / 2 + 1, KT2 = 3 * N / GM_BK;
               const int bi = m / nfr, t = m - bi * nfr;
-              const uint4 q0 = *reinterpret_cast<const uint4*>(h), q1 = *reinterpret_cast<const uint4*>(h + 8);
+              const bool past = lens && t >= __ldg(lens + bi);
+              const uint4 q0 = past ? make_uint4(0u, 0u, 0u, 0u) : *reinterpret_cast<const uint4*>(h);
+              const uint4 q1 = past ? make_uint4(0u, 0u, 0u, 0u) : *reinterpret_cast<const uint4*>(h + 8);
               if (t & 1) {
                 const int ta = (t + 1) >> 1, tb = (t - 1) >> 1;
                 if (ta < n2) {
@@ -242,7 +246,8 @@ gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __re
 
 template <int BN, int EPI>
 static int launch_gemm_t(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, void* out,
-                         const float* res, int M, int N, int K, int res_mod, cudaStream_t s, int aux = 0) {
+                         const float* res, int M, int N, int K, int res_mod, cudaStream_t s, int aux = 0,
+                         const int* lens = nullptr) {
   constexpr size_t smem = (size_t)GM_STAGES * (GM_BM * GM_BK * 2 + BN * GM_BK * 2) + 2 * 64 * GM_EPI_LD * 4;
   static DevSmemCache attr_cache;
   SVCB_CUDA_CHECK(ensure_dyn_smem(gemm_tc_kernel<BN, EPI>, smem, attr_cache));
@@ -252,14 +257,14 @@ static int launch_gemm_t(const __nv_bfloat16* A, const __nv_bfloat16* W, const f
   const int grid = std::min(ntiles, n_sm);
   KernelScope ks("whisper_gemm_tc", s, 2.0 * M * (double)N * K,
                  2.0 * ((double)M * K + (double)N * K) + (EPI == EPI_RESID_F32 ? 8.0 : EPI == EPI_GELU_ADD_F32 ? 4.0 : 2.0) * M * (double)N);
-  gemm_tc_kernel<BN, EPI><<<grid, GM_THREADS, smem, s>>>(A, W, bias, out, res, M, N, K, res_mod, aux);
+  gemm_tc_kernel<BN, EPI><<<grid, GM_THREADS, smem, s>>>(A, W, bias, out, res, M, N, K, res_mod, aux, lens);
   SVCB_LAUNCH_CHECK("gemm_tc");
   return SVCB_OK;
 }
 
 // A_img: tile image [ceil(M/128)][K/64][8][128][8]; W_img: tile image [N/256][K/64][8][256][8]
 int launch_gemm_tc(const void* A_img, const void* W_img, const float* bias, void* out, const float* res,
-                   int M, int N, int K, GemmEpi epi, cudaStream_t s, int res_mod, int aux) {
+                   int M, int N, int K, GemmEpi epi, cudaStream_t s, int res_mod, int aux, const int* lens) {
   if (M <= 0) return SVCB_OK;
   if (K % 64 || N % 256) { set_error("gemm_tc: need K % 64 == 0 and N % 256 == 0"); return SVCB_E_BAD_SHAPE; }
   const __nv_bfloat16* A = static_cast<const __nv_bfloat16*>(A_img);
@@ -270,7 +275,7 @@ int launch_gemm_tc(const void* A_img, const void* W_img, const float* bias, void
     case EPI_RESID_F32: return launch_gemm_t<256, EPI_RESID_F32>(A, W, bias, out, res, M, N, K, 0, s);
     case EPI_GELU_CONV2_IMG:
       if (res_mod <= 0 || M % res_mod || N % GM_BK) { set_error("gemm_tc: epilogue 5 needs rows = items x res_mod frames"); return SVCB_E_BAD_SHAPE; }
-      return launch_gemm_t<256, EPI_GELU_CONV2_IMG>(A, W, bias, out, res, M, N, K, res_mod, s);
+      return launch_gemm_t<256, EPI_GELU_CONV2_IMG>(A, W, bias, out, res, M, N, K, res_mod, s, 0, lens);
     case EPI_GELU_ADD_F32_LD:
       if (!res || res_mod <= 0 || res_mod > N || aux < res_mod) { set_error("gemm_tc: epilogue 7 needs res, valid columns (res_mod) and a leading dimension (aux)"); return SVCB_E_BAD_SHAPE; }
       return launch_gemm_t<256, EPI_GELU_ADD_F32_LD>(A, W, bias, out, res, M, N, K, res_mod, s, aux);
@@ -306,7 +311,7 @@ int launch_ivf_coarse_tc(const void* A_img, const void* W_img, const float* cnor
   KernelScope ks("ivf_coarse_tc", s, 2.0 * M * (double)N * (K / 3),
                  2.0 * ((double)M * K + (double)N * K) + 4.0 * N + 8.0 * M * (double)(N / 16) * nprobe);
   gemm_tc_kernel<256, EPI_IVF_TOPK><<<std::min(ntiles, n_sm), GM_THREADS, smem, s>>>(
-      static_cast<const __nv_bfloat16*>(A_img), static_cast<const __nv_bfloat16*>(W_img), cnorm, cand, nullptr, M, N, K, 0, nprobe);
+      static_cast<const __nv_bfloat16*>(A_img), static_cast<const __nv_bfloat16*>(W_img), cnorm, cand, nullptr, M, N, K, 0, nprobe, nullptr);
   SVCB_LAUNCH_CHECK("ivf_coarse_tc");
   return SVCB_OK;
 }
@@ -429,9 +434,10 @@ int launch_im2col_s1_image(const float* mel, void* img, int B, int n_mels, int n
 // HuBERT's positional convolution (Conv1d(768, 768, 128, padding 64, groups 16), hubert_model.py:115-121), one group:
 // A[m = b*T + t][k = j*cg + ci] = x[b*T + t + j - pad][c0 + ci] from the fp32 time-major rows x [B*T, ld] (zero outside
 // the item), cg = 48 channels per group = 6 octets per tap, K = taps * cg.  One CTA = one (row tile, k tile).
+// lens (ragged batches, may be null): rows t >= lens[b] of item b read as zeros, the convolution's zero padding.
 __global__ void __launch_bounds__(256)
 im2col_rows_image_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ img, int T, int M, int ld, int c0, int cg,
-                         int pad, int KT) {
+                         int pad, int KT, const int* __restrict__ lens) {
   const int mt = blockIdx.x, kt = blockIdx.y, opt = cg / 8;   // octets per tap
   __nv_bfloat16* dst = img + ((size_t)mt * KT + kt) * (GM_BM * GM_BK);
   for (int idx = threadIdx.x; idx < 8 * 128; idx += 256) {
@@ -443,7 +449,7 @@ im2col_rows_image_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict_
     for (int e = 0; e < 8; ++e) h[e] = __float2bfloat16_rn(0.f);
     if (m < M) {
       const int b = m / T, t = m - b * T + j - pad;
-      if (t >= 0 && t < T) {
+      if (t >= 0 && t < (lens ? __ldg(lens + b) : T)) {
         const float4* s4 = reinterpret_cast<const float4*>(x + ((size_t)b * T + t) * ld + c0 + ci);
         const float4 u0 = __ldg(s4), u1 = __ldg(s4 + 1);
         h[0] = __float2bfloat16_rn(u0.x); h[1] = __float2bfloat16_rn(u0.y); h[2] = __float2bfloat16_rn(u0.z); h[3] = __float2bfloat16_rn(u0.w);
@@ -454,13 +460,52 @@ im2col_rows_image_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict_
   }
 }
 
-int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s) {
+int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s,
+                             const int* lens) {
   if (cg % 8 || (taps * cg) % 64 || (c0 % 4) || (ld % 4)) { set_error("im2col_rows_image: channel group must be octets, K a multiple of 64"); return SVCB_E_BAD_SHAPE; }
   const int M = B * T, KT = taps * cg / 64;
   dim3 grid((M + 127) / 128, KT);
   KernelScope ks("im2col_rows_image", s, 0.0, (double)M * taps * cg * 2 + 4.0 * M * cg);
-  im2col_rows_image_kernel<<<grid, 256, 0, s>>>(x, static_cast<__nv_bfloat16*>(img), T, M, ld, c0, cg, pad, KT);
+  im2col_rows_image_kernel<<<grid, 256, 0, s>>>(x, static_cast<__nv_bfloat16*>(img), T, M, ld, c0, cg, pad, KT, lens);
   SVCB_LAUNCH_CHECK("im2col_rows_image");
+  return SVCB_OK;
+}
+
+// Ragged batches: per-item lengths reach the device as kernel parameters, 256 per launch, so that no host-to-device
+// copy (which would wait for the stream when the source is pageable) is needed.
+struct StageInts {
+  int v[256];
+};
+__global__ void stage_ints_kernel(StageInts src, int* __restrict__ dst, int n) {
+  if ((int)threadIdx.x < n) dst[threadIdx.x] = src.v[threadIdx.x];
+}
+
+int launch_stage_ints(const int* host, int n, int* dst, cudaStream_t s) {
+  for (int i = 0; i < n; i += 256) {
+    StageInts c;
+    const int m = std::min(256, n - i);
+    for (int j = 0; j < m; ++j) c.v[j] = host[i + j];
+    stage_ints_kernel<<<1, 256, 0, s>>>(c, dst + i, m);
+    SVCB_LAUNCH_CHECK("stage_ints");
+  }
+  return SVCB_OK;
+}
+
+// Ragged batches: rows t >= lens[b] of item b of the fp32 output [B * T, width] are set to zero.
+__global__ void __launch_bounds__(256)
+zero_tail_rows_kernel(float* __restrict__ out, const int* __restrict__ lens, int T, int width) {
+  const int b = blockIdx.y, t = __ldg(lens + b) + blockIdx.x;
+  if (t >= T) return;
+  float4* r = reinterpret_cast<float4*>(out + ((size_t)b * T + t) * width);
+  for (int i = threadIdx.x; i < width / 4; i += 256) r[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+int launch_zero_tail_rows(float* out, const int* lens, int B, int T, int width, int min_len, cudaStream_t s) {
+  if (width % 4) { set_error("zero_tail_rows: width must be a multiple of 4"); return SVCB_E_BAD_SHAPE; }
+  if (B <= 0 || T <= min_len) return SVCB_OK;
+  KernelScope ks("zero_tail_rows", s, 0.0, 4.0 * B * (double)(T - min_len) * width);
+  zero_tail_rows_kernel<<<dim3(T - min_len, B), 256, 0, s>>>(out, lens, T, width);
+  SVCB_LAUNCH_CHECK("zero_tail_rows");
   return SVCB_OK;
 }
 

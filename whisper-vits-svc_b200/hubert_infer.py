@@ -142,6 +142,25 @@ class HubertSoftB200:
                 taps[n] = b
         return out
 
+    @torch.no_grad()
+    def units_ragged(self, wav: torch.Tensor, n_samples: List[int]) -> torch.Tensor:
+        """`units` for a ragged batch: item b is wav[b, :n_samples[b]] (at least one frame each) -> [B, frames(N), 256];
+        item b's first frames(n_samples[b]) rows equal a lone `units` of it bit for bit, its later rows are zero."""
+        wav = wav.to(self.device, torch.float32).contiguous()
+        B, N = wav.shape
+        assert len(n_samples) == B
+        lib = _lib.load()
+        need = int(lib.svcb_hubert_workspace_bytes(self._handle, B, N)) + 8 * B
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        out = torch.empty(B, self.frames(N), 256, device=self.device, dtype=torch.float32)
+        lens = (ctypes.c_int32 * B)(*n_samples)
+        with torch.cuda.device(self.device):
+            st = lib.svcb_hubert_units_ragged(self._handle, wav.data_ptr(), lens, out.data_ptr(), B, N, self._ws.data_ptr(),
+                                              self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        _lib.check(st, "svcb_hubert_units_ragged")
+        return out
+
 
 def hubert_soft(path: str, device="cuda") -> HubertSoftB200:
     """hubert/hubert_model.py:212-222."""
@@ -181,3 +200,15 @@ def pred_vec(model: HubertSoftB200, wavPath: str, vecPath: str, device=None):
         if e - s != CHUNK and model.frames(e - s) >= 1:
             vec_a.extend(model.units(torch.from_numpy(audio[s:e])[None]).reshape(-1, 256).cpu().numpy())
     np.save(vecPath, np.asarray(vec_a, dtype=np.float32), allow_pickle=False)
+
+
+@torch.no_grad()
+def units_batch(model: HubertSoftB200, audios: List[np.ndarray]) -> List[np.ndarray]:
+    """prepare/preprocess_hubert.py:pred_vec for several files in one ragged device batch: `units` of each WHOLE file
+    (no 20 s chunking) -> float32 [frames(len), 256] per item, each equal to a lone run of it."""
+    lens = [int(a.shape[0]) for a in audios]
+    wav = np.zeros((len(audios), max(lens)), np.float32)
+    for b, a in enumerate(audios):
+        wav[b, :lens[b]] = a
+    out = model.units_ragged(torch.from_numpy(wav), lens).cpu()
+    return [out[b, :model.frames(n)].numpy() for b, n in enumerate(lens)]

@@ -30,6 +30,7 @@ SAMPLE_RATE = 16000
 N_FFT = 400
 N_MELS = 80
 HOP_LENGTH = 160
+N_SAMPLES = 30 * SAMPLE_RATE  # whisper/audio.py:19
 
 
 # ------------------------------------------------------------------------------ packing
@@ -181,6 +182,49 @@ class WhisperEncoderB200:
         _lib.check(st, "svcb_whisper_log_mel")
         return mel
 
+    @torch.no_grad()
+    def log_mel_ragged(self, audio: torch.Tensor, n_samples: List[int]) -> torch.Tensor:
+        """`log_mel` without noise for a ragged batch: item b is audio[b, :n_samples[b]] (more than 200 samples).
+        -> mel [B, n_mels, N // 160]; item b's first n_samples[b] // 160 frames equal a lone `log_mel` of it bit for
+        bit, its later frames are zero (the padding the encoder's first convolution expects)."""
+        audio = audio.to(self.device, torch.float32).contiguous()
+        B, N = audio.shape
+        assert len(n_samples) == B
+        nm = self.cfg["n_mels"]
+        mel = torch.empty(B, nm, N // HOP_LENGTH, device=self.device, dtype=torch.float32)
+        if self._lm_scratch is None or self._lm_scratch.numel() < 2 * B:
+            self._lm_scratch = torch.empty(max(2 * B, 64), dtype=torch.int32, device=self.device)
+        lens = (ctypes.c_int32 * B)(*n_samples)
+        with torch.cuda.device(self.device):
+            st = _lib.load().svcb_whisper_log_mel_ragged(
+                audio.data_ptr(), lens, self._filters.data_ptr(), mel.data_ptr(), self._lm_scratch.data_ptr(), B, N, nm,
+                ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        _lib.check(st, "svcb_whisper_log_mel_ragged")
+        return mel
+
+    @torch.no_grad()
+    def encode_ragged(self, mel: torch.Tensor, n_frames: List[int]) -> torch.Tensor:
+        """The encoder for a ragged batch: item b is mel[b, :, :n_frames[b]], whose later columns must be zero (as
+        `log_mel_ragged` leaves them).  -> [B, (n-1)//2+1, n_state]; item b's first (n_frames[b]-1)//2+1 rows equal a
+        lone run of it bit for bit, its later rows are zero."""
+        mel = mel.to(self.device, torch.float32).contiguous()
+        B, nm, n = mel.shape
+        assert nm == self.cfg["n_mels"] and len(n_frames) == B
+        n2 = (n - 1) // 2 + 1
+        assert n2 <= self.cfg["n_ctx"], "incorrect audio shape"
+        lib = _lib.load()
+        need = int(lib.svcb_whisper_workspace_bytes(self._handle, B, n)) + 8 * B
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        ws = self._ws
+        out = torch.empty(B, n2, self.cfg["n_state"], device=self.device, dtype=torch.float32)
+        lens = (ctypes.c_int32 * B)(*n_frames)
+        with torch.cuda.device(self.device):
+            st = lib.svcb_whisper_encode_ragged(self._handle, mel.data_ptr(), lens, out.data_ptr(), B, n, ws.data_ptr(),
+                                                ws.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        _lib.check(st, "svcb_whisper_encode_ragged")
+        return out
+
 
 class WhisperB200:
     """What `load_model` returns: exposes `.encoder` and `.dims` like the reference's Whisper module."""
@@ -285,3 +329,36 @@ def pred_ppg(whisper: WhisperB200, wavPath: str, ppgPath: str, device, mel_noise
     for i, (_, _, n_rows) in enumerate(plan):
         rows.extend(outs[i][:n_rows])
     np.save(ppgPath, np.asarray(rows), allow_pickle=False)
+
+
+# ------------------------------------------------------------------------------ dataset PPGs (prepare/preprocess_ppg.py)
+def pad_or_trim(audio: np.ndarray, length_max: int = N_SAMPLES, length_min: int = N_SAMPLES // 2) -> np.ndarray:
+    """whisper/audio.py:29-50 on a 1-D array: trimmed to at most 30 s, zero-padded to at least 15 s.  Clips of 15 s or
+    less all become 15 s; clips between 15 and 30 s keep their length."""
+    if audio.shape[-1] > length_max:
+        audio = audio[..., :length_max]
+    if audio.shape[-1] < length_min:
+        audio = np.pad(audio, [(0, 0)] * (audio.ndim - 1) + [(0, length_min - audio.shape[-1])])
+    return audio
+
+
+def ppg_rows(audln: int) -> int:
+    """Rows prepare/preprocess_ppg.py:29-39 keeps of a file of audln samples: ppg[:audln // 320] of the encoder's
+    (F - 1) // 2 + 1 positions for the F = len(pad_or_trim(audio)) // 160 mel frames."""
+    n = min(max(audln, N_SAMPLES // 2), N_SAMPLES)
+    return min(audln // 320, (n // HOP_LENGTH - 1) // 2 + 1)
+
+
+@torch.no_grad()
+def ppg_batch(whisper: WhisperB200, audios: List[np.ndarray]) -> List[np.ndarray]:
+    """prepare/preprocess_ppg.py:pred_ppg for several files in one ragged device batch: each 16 kHz array is
+    pad_or_trim-ed, turned into its log-mel with no noise and encoded; item b -> float32 [ppg_rows(len), n_state].
+    Each item's rows are those of a lone run of it."""
+    enc = whisper.encoder
+    padded = [pad_or_trim(np.asarray(a, dtype=np.float32)) for a in audios]
+    lens = [p.shape[0] for p in padded]
+    wav = np.zeros((len(padded), max(lens)), np.float32)
+    for b, p in enumerate(padded):
+        wav[b, :lens[b]] = p
+    ppg = enc.encode_ragged(enc.log_mel_ragged(torch.from_numpy(wav), lens), [n // HOP_LENGTH for n in lens]).cpu()
+    return [ppg[b, :ppg_rows(a.shape[0])].numpy() for b, a in enumerate(audios)]
