@@ -14,7 +14,7 @@
  *   - a model handle is immutable after creation: concurrent calls on different streams
  *     are fine when their workspaces differ;
  *   - sm_90a only, no fallback: svcb_model_create, svcb_whisper_create, svcb_hubert_create,
- *     svcb_ivf_create and svcb_speaker_create fail with SVCB_E_UNSUPPORTED elsewhere.
+ *     svcb_ivf_create, svcb_speaker_create and svcb_vad_create fail with SVCB_E_UNSUPPORTED elsewhere.
  */
 #ifndef SVCB_H_
 #define SVCB_H_
@@ -301,6 +301,25 @@ int svcb_speaker_mel(const svcb_speaker* s, const float* wav, const int64_t* sam
  * bf16x3 on the tensor cores with fp32 accumulation, gate math fp32.  An item's result does not depend on the batch. */
 int svcb_speaker_embed(const svcb_speaker* s, const float* mel, const int64_t* frame_offsets_host, int32_t B, float* out,
                        float* window_out, void* ws, size_t ws_bytes, svcb_stream stream);
+
+/* ------------------------------------------------------------------ voice-activity detector (Silero VAD, 16 kHz) */
+typedef struct svcb_vad svcb_vad;
+/* Replaces the 16 kHz branch of vad/assets/silero_vad.jit.  Blob names/layouts: whisper-vits-svc_b200/vad_infer.py:pack_vad.
+ * Fails with SVCB_E_UNSUPPORTED unless the device is sm_90. */
+int svcb_vad_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table_host, int32_t n_entries,
+                    svcb_vad** out);
+void svcb_vad_destroy(svcb_vad* v);
+/* 512-sample windows of n_samples of 16 kHz audio: ceil(n_samples / 512), 0 for an empty item */
+int64_t svcb_vad_windows(int64_t n_samples);
+/* scratch for svcb_vad_probs on B items of total_windows windows in all: 1 KB per window (layer 0's gate inputs) */
+size_t svcb_vad_workspace_bytes(const svcb_vad* v, int32_t B, int64_t total_windows);
+/* Replaces get_speech_timestamps' probability loop (vad/utils.py:262-268) for a ragged batch: item b is
+ * wav[sample_offsets_host[b] .. sample_offsets_host[b+1]) (offsets non-decreasing, checked before any launch) ->
+ * probs_out [sum_b W_b] fp32, item b's W_b = svcb_vad_windows(n_b) probabilities following item b-1's; the last window
+ * of an item is zero-padded to 512 samples and the LSTM state starts at zero for each item.  feat_out [sum_b W_b, 64]
+ * receives the encoder output of each window (may be NULL).  All fp32.  An item's result does not depend on the batch. */
+int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_offsets_host, int32_t B, float* probs_out,
+                   float* feat_out, void* ws, size_t ws_bytes, svcb_stream stream);
 
 /* Operator entry points of the encoder (unit tests):
  * out[M,N] = A[M,K] . W[N,K]^T + bias with epilogue 0: bf16 row-major out, 1: GELU(erf) then bf16

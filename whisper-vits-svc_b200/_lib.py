@@ -107,6 +107,11 @@ SIGNATURES = {
     "svcb_speaker_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int64]),
     "svcb_speaker_mel": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_size_t, c_void_p]),
     "svcb_speaker_embed": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "svcb_vad_create": (c_int, [c_void_p, c_size_t, POINTER(TensorEntry), c_int32, POINTER(c_void_p)]),
+    "svcb_vad_destroy": (None, [c_void_p]),
+    "svcb_vad_windows": (c_int64, [c_int64]),
+    "svcb_vad_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int64]),
+    "svcb_vad_probs": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "svcb_op_gemm_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_gemm_bf16": (c_int, [c_void_p] * 5 + [c_int32] * 4 + [c_void_p, c_size_t, c_void_p]),
     "svcb_op_attention_tc_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
