@@ -172,7 +172,7 @@ int svcb_whisper_encode(const svcb_whisper* w, const float* mel, float* out, int
 /* svcb_whisper_encode for a ragged batch: item b is the first n_frames_host[b] (1..n_frames) columns of its mel, and
  * its columns past them must be zero (svcb_whisper_log_mel_ragged writes them so).  Item b's first
  * (n_frames_host[b]-1)/2+1 output rows are bitwise those of a lone svcb_whisper_encode of its own frames; its later
- * rows are zero.  ws_bytes >= svcb_whisper_workspace_bytes(w, B, n_frames) + 8 * B (the lengths are staged there). */
+ * rows are zero.  ws_bytes >= svcb_whisper_workspace_bytes(w, B, n_frames), which includes a region for the lengths. */
 int svcb_whisper_encode_ragged(const svcb_whisper* w, const float* mel, const int32_t* n_frames_host, float* out, int32_t B,
                                int32_t n_frames, void* ws, size_t ws_bytes, svcb_stream stream);
 
@@ -197,7 +197,7 @@ int svcb_hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_
 /* svcb_hubert_units (tensor-core stem, no taps) for a ragged batch: item b is the first n_samples_host[b] samples of its
  * row of wav (1..n_samples, at least one frame each).  Item b's first svcb_hubert_frames(n_samples_host[b]) output rows
  * are bitwise those of a lone svcb_hubert_units of its own samples; its later rows are zero.
- * ws_bytes >= svcb_hubert_workspace_bytes(h, B, n_samples) + 8 * B (the lengths are staged there). */
+ * ws_bytes >= svcb_hubert_workspace_bytes(h, B, n_samples), which includes a region for the lengths. */
 int svcb_hubert_units_ragged(const svcb_hubert* h, const float* wav, const int32_t* n_samples_host, float* out, int32_t B,
                              int32_t n_samples, void* ws, size_t ws_bytes, svcb_stream stream);
 

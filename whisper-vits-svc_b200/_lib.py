@@ -8,6 +8,8 @@ import ctypes
 import os
 from ctypes import POINTER, c_char, c_char_p, c_float, c_int, c_int16, c_int32, c_int64, c_size_t, c_uint64, c_void_p
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsvc_b200.so")
 
@@ -174,3 +176,62 @@ def check(status: int, what: str):
 
 def last_launch_count() -> int:
     return int(load().svcb_last_launch_count())
+
+
+def cuda_device(device) -> torch.device:
+    """torch.device(device), or SvcbError when it is not a CUDA device."""
+    dev = torch.device(device)
+    if dev.type != "cuda":
+        raise SvcbError(f"libsvc_b200 computes only on a CUDA (sm_90a) device, not {dev}; there is no CPU fallback")
+    return dev
+
+
+def stream() -> c_void_p:
+    """The current device's current torch stream, as an svcb_stream."""
+    return c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def call(name: str, *args, device=None) -> None:
+    """svcb_<name>(*args, stream) on `device` (default: the current device) and its current stream."""
+    with torch.cuda.device(device):
+        st = getattr(load(), "svcb_" + name)(*args, stream())
+    check(st, "svcb_" + name)
+
+
+class Handle:
+    """A device model behind the C ABI: the packed blob (on a CUDA device) and the handle svcb_<kind>_create made from
+    it, with one grow-only workspace.  The blob lives as long as the handle; dropping the Handle destroys both.  A
+    Handle passes to any svcb_* function as the opaque handle pointer (ctypes reads `_as_parameter_`)."""
+
+    def __init__(self, kind: str, table, blob: torch.Tensor, *create_args):
+        self.kind, self._as_parameter_, self._ws = kind, None, None
+        self.device = cuda_device(blob.device)
+        entries = (TensorEntry * len(table))()
+        for e, (name, off, numel) in zip(entries, table):
+            e.name, e.offset_bytes, e.numel = name.encode(), off, numel
+        args = [ctypes.byref(a) if isinstance(a, ctypes.Structure) else a for a in create_args]
+        h = c_void_p()
+        with torch.cuda.device(self.device):
+            st = getattr(load(), f"svcb_{kind}_create")(blob.data_ptr(), blob.numel() * blob.element_size(), entries,
+                                                        len(table), *args, ctypes.byref(h))
+        check(st, f"svcb_{kind}_create")
+        self.blob, self.table, self._as_parameter_ = blob, table, h
+
+    def __del__(self):
+        if self._as_parameter_ is not None:
+            try:
+                getattr(load(), f"svcb_{self.kind}_destroy")(self)
+            except Exception:
+                pass
+
+    def workspace(self, nbytes: int) -> torch.Tensor:
+        """A uint8 device buffer of at least nbytes.  It only grows; the old buffer is freed before the larger one is
+        allocated, so the two are never held at once."""
+        if self._ws is None or self._ws.numel() < nbytes:
+            self._ws = None
+            self._ws = torch.empty(int(nbytes), dtype=torch.uint8, device=self.device)
+        return self._ws
+
+    def call(self, name: str, *args) -> None:
+        """svcb_<name>(handle, *args, stream) on the handle's device."""
+        call(name, self, *args, device=self.device)

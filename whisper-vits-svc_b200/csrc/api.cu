@@ -149,18 +149,19 @@ struct Ctx {
   bool dry = false;
   cudaStream_t stream = nullptr;
   const svcb_taps* taps = nullptr;
-  bool overflow = false;
 
   template <class T>
   T* alloc(size_t n) {
-    off = (off + 255) & ~(size_t)255;
+    off = align256(off);
     const size_t o = off;
     off += n * sizeof(T);
     if (off > peak) peak = off;
     if (dry) return reinterpret_cast<T*>((uintptr_t)4096 + o);
-    if (off > cap) { overflow = true; return nullptr; }
+    if (off > cap) return nullptr;
     return reinterpret_cast<T*>(base + o);
   }
+  // after the allocations a step makes and before its launches; a dry run sizes the workspace and checks nothing
+  int check() const { return dry ? SVCB_OK : check_workspace(base, cap, peak, "model"); }
 };
 
 #define RUN(expr)                    \
@@ -172,15 +173,6 @@ static int tap(Ctx& ctx, int id, const float* src, size_t numel) {
   if (ctx.dry || !ctx.taps || !ctx.taps->ptr[id]) return SVCB_OK;
   SVCB_CUDA_CHECK(cudaMemcpyAsync(ctx.taps->ptr[id], src, numel * sizeof(float),
                                   cudaMemcpyDeviceToDevice, ctx.stream));
-  return SVCB_OK;
-}
-
-static int check_ws(Ctx& ctx) {
-  if (ctx.overflow) {
-    set_error("workspace too small: need " + std::to_string(ctx.peak) + " bytes, have " +
-              std::to_string(ctx.cap));
-    return SVCB_E_WORKSPACE;
-  }
   return SVCB_OK;
 }
 
@@ -305,7 +297,7 @@ static int run_prior(const svcb_model* m, Ctx& ctx, const float* ppg, const floa
   float* stats = ctx.alloc<float>((size_t)B * 2 * C * T);
   const size_t attn_ws_bytes = m->attn_tc ? rel_attention_ws_bytes(B, c.enc_heads, T) : 0;
   uint8_t* attn_ws = m->attn_tc ? ctx.alloc<uint8_t>(attn_ws_bytes) : nullptr;
-  SVCB_TRY(check_ws(ctx));
+  SVCB_TRY(ctx.check());
   {  // pre / hub on time-major inputs (vits/models.py:40-46)
     ConvParams p = std_conv(m->pre, ppg, x, B, T, T, 2);
     p.sxb = (long long)T * c.ppg_dim; p.sxc = 1; p.sxt = c.ppg_dim;
@@ -359,7 +351,7 @@ static int run_flow(const svcb_model* m, Ctx& ctx, const float* z_p, const long 
   float* rs = ctx.alloc<float>((size_t)B * 2 * H * T);
   float* out = ctx.alloc<float>((size_t)B * H * T);
   float* mm = ctx.alloc<float>((size_t)B * half * T);
-  SVCB_TRY(check_ws(ctx));
+  SVCB_TRY(ctx.check());
   const float* cur = z_p;
   for (int f = c.n_flows - 1; f >= 0; --f) {
     const FlowLayer& F = m->flow[f];
@@ -521,7 +513,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
   float* SRCP = nsplit ? ctx.alloc<float>((size_t)B * Lpad) : nullptr;
   void* IMG_HI = img_bytes ? ctx.alloc<uint8_t>(img_bytes) : nullptr;
   void* IMG_LO = (img_bytes && nsplit == 3) ? ctx.alloc<uint8_t>(img_bytes) : nullptr;
-  SVCB_TRY(check_ws(ctx));
+  SVCB_TRY(ctx.check());
 
   if (nsplit && !ctx.dry) {
     dim3 grid((unsigned)((Lpad + 255) / 256), B);
@@ -547,7 +539,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
     const int chn = ch / 2, Ln = L * us.rate, sf = us.sf;
     float* X = ctx.alloc<float>((size_t)B * chn * Ln);
     float* ACC = ctx.alloc<float>((size_t)B * chn * Ln);
-    SVCB_TRY(check_ws(ctx));
+    SVCB_TRY(ctx.check());
     // ups[i](x) (ConvTranspose1d, generator.py:183) + noise_convs[i](source) (generator.py:185-186)
     if (us.form == UPS_COMB) {
       // wide stages: every phase AND the stage's noise conv in one tensor-core conv whose epilogue stores the
@@ -615,7 +607,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
       // convolutions' zero padding and are never written by the link kernels
       const size_t ib = s2d_image_bytes(B, Ln, rb[0].s2d_r);
       uint8_t* base = ctx.alloc<uint8_t>(4 * ib);
-      SVCB_TRY(check_ws(ctx));
+      SVCB_TRY(ctx.check());
       for (int q = 0; q < 4; ++q) a.s2d[q] = base + (size_t)q * ib;
       if (!ctx.dry) {
         KernelScope ks("s2d_image_clear", s, 0.0, 4.0 * ib);
@@ -662,6 +654,13 @@ int check_blob_device(const void* dev_blob) {
     return SVCB_E_UNSUPPORTED;
   }
   return SVCB_OK;
+}
+
+int check_workspace(const void* ws, size_t ws_bytes, size_t need, const char* who) {
+  if (ws && !((uintptr_t)ws & 255) && ws_bytes >= need) return SVCB_OK;
+  set_error(std::string(who) + " workspace too small or misaligned: need " + std::to_string(need) +
+            " bytes at a 256-byte boundary, have " + std::to_string(ws_bytes));
+  return SVCB_E_WORKSPACE;
 }
 
 int BlobTensors::read(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table, int32_t n) {
@@ -966,7 +965,7 @@ int svcb_source(const svcb_model* m, const float* f0, const float* rand_ini, con
   Ctx ctx;
   SVCB_TRY(make_ctx(ctx, ws, ws_bytes, nullptr, stream));
   double* scan = ctx.alloc<double>(source_scan_ws_bytes(B, T, m->cfg.n_harmonics) / sizeof(double));
-  SVCB_TRY(check_ws(ctx));
+  SVCB_TRY(ctx.check());
   return launch_source(f0, rand_ini, noise, m->merge_w, m->merge_b, source, scan, B, T, m->hop,
                        m->cfg.n_harmonics, (float)m->cfg.sampling_rate, ctx.stream);
 }
@@ -1017,7 +1016,7 @@ int svcb_infer(const svcb_model* m, const float* ppg, const float* vec, const fl
   const long long* len = reinterpret_cast<const long long*>(lengths);
   float* zp = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
   float* z = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
-  SVCB_TRY(check_ws(ctx));
+  SVCB_TRY(ctx.check());
   const size_t mark = ctx.off;
   SVCB_TRY(run_prior(m, ctx, ppg, vec, pit, len, eps, zp, B, T));
   ctx.off = mark;
@@ -1057,11 +1056,8 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
                         int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t nsplit, void* scratch,
                         size_t scratch_bytes, svcb_stream stream) {
   g_launches = 0;
-  const size_t img = (p8_image_bytes(B, C, L) + 255) & ~(size_t)255;
-  if (!scratch || ((uintptr_t)scratch & 255) || scratch_bytes < 2 * img) {
-    set_error("svcb_op_amp_conv_tc: scratch too small or misaligned");
-    return SVCB_E_WORKSPACE;
-  }
+  const size_t img = align256(p8_image_bytes(B, C, L));
+  SVCB_TRY(check_workspace(scratch, scratch_bytes, 2 * img, "svcb_op_amp_conv_tc"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   void* hi = scratch;
   void* lo = nsplit == 3 ? static_cast<char*>(scratch) + img : nullptr;
@@ -1076,7 +1072,7 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L) {
   const int r = C > 0 ? 160 / C : 0;
   if (B <= 0 || L <= 0 || !s2d_link_factor(C) || L % r) return 0;
-  return 4 * ((s2d_image_bytes(B, L, r) + 255) & ~(size_t)255) + 512;
+  return 4 * align256(s2d_image_bytes(B, L, r)) + 512;
 }
 
 int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
@@ -1086,11 +1082,8 @@ int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_ac
   g_launches = 0;
   const int r = s2d_link_factor(C);
   if (!r || B <= 0 || L <= 0 || L % r || L % 8) { set_error("svcb_op_amp_s2d_link: need C in {40, 20, 10}, L % (160/C) == 0 and L % 8 == 0"); return SVCB_E_BAD_SHAPE; }
-  const size_t img = (s2d_image_bytes(B, L, r) + 255) & ~(size_t)255;
-  if (!scratch || ((uintptr_t)scratch & 255) || scratch_bytes < 4 * img) {
-    set_error("svcb_op_amp_s2d_link: scratch too small or misaligned");
-    return SVCB_E_WORKSPACE;
-  }
+  const size_t img = align256(s2d_image_bytes(B, L, r));
+  SVCB_TRY(check_workspace(scratch, scratch_bytes, 4 * img, "svcb_op_amp_s2d_link"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* b0 = static_cast<char*>(scratch);
   SVCB_CUDA_CHECK(cudaMemsetAsync(b0, 0, 4 * img, s));

@@ -2,9 +2,11 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <algorithm>
 #include <atomic>
 #include <map>
 #include <string>
+#include <vector>
 
 #include "svcb.h"
 
@@ -16,6 +18,20 @@ void count_launch();
 // Handle creation (svcb_model_create, svcb_whisper_create, svcb_hubert_create).
 // SVCB_E_BAD_ALIGN unless the blob is 256-byte aligned, SVCB_E_UNSUPPORTED unless the current device is sm_90.
 int check_blob_device(const void* dev_blob);
+
+// Workspaces: every region starts on a 256-byte boundary.
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+// A workspace laid out region by region: take(bytes) returns the next region's offset; off is then the bytes so far.
+struct WsPlan {
+  size_t off = 0;
+  size_t take(size_t bytes) {
+    const size_t o = off;
+    off = align256(off + bytes);
+    return o;
+  }
+};
+// SVCB_E_WORKSPACE, with an error naming `who`, unless ws is non-null, 256-byte aligned and holds need bytes.
+int check_workspace(const void* ws, size_t ws_bytes, size_t need, const char* who);
 // The named tensors of a packed weight blob.
 struct BlobTensors {
   std::map<std::string, std::pair<const float*, uint64_t>> map;
@@ -394,6 +410,45 @@ int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, in
 int launch_stage_ints(const int* host, int n, int* dst, cudaStream_t s);
 // ragged batches: zero the rows t >= lens[b] (device array, every lens[b] >= min_len) of each item of fp32 [B * T, width]
 int launch_zero_tail_rows(float* out, const int* lens, int B, int T, int width, int min_len, cudaStream_t s);
+// The per-item lengths of a ragged batch (svcb_whisper_encode_ragged, svcb_hubert_units_ragged) and the output rows each
+// item gets.  validate() checks them on the host before any launch; stage() puts both in the workspace region of
+// ragged_lens_bytes(B) the layout owns.  Without lengths (a dense batch) nothing is staged and lens / out_lens stay null.
+inline size_t ragged_lens_bytes(int B) { return 8 * (size_t)B; }
+struct RaggedLens {
+  std::vector<int> host;   // [lengths of items 0 .. B-1][output lengths of items 0 .. B-1]
+  int B = 0, min_out = 0;
+  const int *lens = nullptr, *out_lens = nullptr;   // on the device, after stage()
+  // each len[b] must be in [1, max_len] and give out_len(len[b]) >= 1
+  template <class OutLen>
+  int validate(const int32_t* len, int batch, int max_len, OutLen out_len, const char* who, const char* unit) {
+    if (!len) return SVCB_OK;
+    B = batch;
+    host.resize(2 * (size_t)B);
+    for (int b = 0; b < B; ++b) {
+      const int n = len[b], r = n >= 1 && n <= max_len ? out_len(n) : 0;
+      if (r < 1) {
+        set_error(std::string(who) + ": item " + std::to_string(b) + " has " + std::to_string(n) + " " + unit + "; need 1.." +
+                  std::to_string(max_len) + " and at least one output row");
+        return SVCB_E_BAD_SHAPE;
+      }
+      host[b] = n;
+      host[B + b] = r;
+    }
+    min_out = *std::min_element(host.begin() + B, host.end());
+    return SVCB_OK;
+  }
+  int stage(void* region, cudaStream_t s) {
+    if (host.empty()) return SVCB_OK;
+    int* d = static_cast<int*>(region);
+    lens = d;
+    out_lens = d + B;
+    return launch_stage_ints(host.data(), (int)host.size(), d, s);
+  }
+  // zero the rows past each item's own of the fp32 output [B * T, width]
+  int zero_tail(float* out, int T, int width, cudaStream_t s) const {
+    return out_lens ? launch_zero_tail_rows(out, out_lens, B, T, width, min_out, s) : SVCB_OK;
+  }
+};
 int launch_rowmajor_to_image(const void* src, void* dst, int R, int K, int rows, cudaStream_t s);
 int launch_image_to_rowmajor(const void* src, void* dst, int R, int K, cudaStream_t s);
 int launch_qkv_rowmajor_to_heads(const void* src, void* dst, int B, int T, int D, cudaStream_t s);

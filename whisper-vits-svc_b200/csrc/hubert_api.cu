@@ -169,12 +169,10 @@ hubert_conv0_pack_kernel(const float* __restrict__ wav, const float* __restrict_
   else { put(t >> 1, 0); put((t >> 1) - 1, 2); }
 }
 
-static size_t align256h(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct HLayout {
   int T[7];            // frames after conv0 .. conv6
   int M;
-  size_t bufa, bufb, imgb, stats, posimg, rows, a512, x, y, a, qkv, att, mid, total;   // bufb doubles as the first im2col image
+  size_t bufa, bufb, imgb, stats, posimg, rows, a512, x, y, a, qkv, att, mid, lens, total;   // bufb doubles as the first im2col image
 };
 static HLayout hubert_layout(int B, int n_samples) {
   HLayout L;
@@ -183,24 +181,25 @@ static HLayout hubert_layout(int B, int n_samples) {
   const int T = L.T[6];
   L.M = B * T;
   const size_t Mp = ((size_t)L.M + 127) / 128 * 128;
-  size_t off = 0;
-  L.bufa = off; off = align256h(off + (size_t)B * HB_C * L.T[0] * 4);
+  WsPlan P;
+  L.bufa = P.take((size_t)B * HB_C * L.T[0] * 4);
   {  // fp32 stem: ping-pong activations [B, 512, T1]; tensor-core stem: im2col images [ceil(B T_i / 128) * 128][taps * 512] bf16
     const size_t m1 = ((size_t)B * (L.T[1] > 0 ? L.T[1] : 1) + 127) / 128 * 128, m2 = ((size_t)B * (L.T[2] > 0 ? L.T[2] : 1) + 127) / 128 * 128;
-    L.bufb = off; off = align256h(off + std::max((size_t)B * HB_C * (L.T[1] > 0 ? L.T[1] : 1) * 4, m1 * 3 * HB_C * 2));
-    L.imgb = off; off = align256h(off + m2 * 3 * HB_C * 2);
+    L.bufb = P.take(std::max((size_t)B * HB_C * (L.T[1] > 0 ? L.T[1] : 1) * 4, m1 * 3 * HB_C * 2));
+    L.imgb = P.take(m2 * 3 * HB_C * 2);
   }
-  L.stats = off; off = align256h(off + (size_t)B * HB_C * sizeof(float2));
-  L.posimg = off; off = align256h(off + Mp * (size_t)HB_PK * (HB_D / HB_PG) * 2);   // one group's im2col image, K = 128 * 48
-  L.rows = off; off = align256h(off + (size_t)(L.M > 0 ? L.M : 1) * HB_C * 4);
-  L.a512 = off; off = align256h(off + Mp * HB_C * 2);
-  L.x = off; off = align256h(off + (size_t)(L.M > 0 ? L.M : 1) * HB_D * 4);
-  L.y = off; off = align256h(off + (size_t)(L.M > 0 ? L.M : 1) * HB_D * 4);
-  L.a = off; off = align256h(off + Mp * HB_D * 2);
-  L.qkv = off; off = align256h(off + (size_t)B * qkv_heads_tp(T > 0 ? T : 1) * 3 * HB_D * 2);
-  L.att = off; off = align256h(off + Mp * HB_D * 2);
-  L.mid = off; off = align256h(off + Mp * HB_FF * 2);
-  L.total = off + 4096;
+  L.stats = P.take((size_t)B * HB_C * sizeof(float2));
+  L.posimg = P.take(Mp * (size_t)HB_PK * (HB_D / HB_PG) * 2);   // one group's im2col image, K = 128 * 48
+  L.rows = P.take((size_t)(L.M > 0 ? L.M : 1) * HB_C * 4);
+  L.a512 = P.take(Mp * HB_C * 2);
+  L.x = P.take((size_t)(L.M > 0 ? L.M : 1) * HB_D * 4);
+  L.y = P.take((size_t)(L.M > 0 ? L.M : 1) * HB_D * 4);
+  L.a = P.take(Mp * HB_D * 2);
+  L.qkv = P.take((size_t)B * qkv_heads_tp(T > 0 ? T : 1) * 3 * HB_D * 2);
+  L.att = P.take(Mp * HB_D * 2);
+  L.mid = P.take(Mp * HB_FF * 2);
+  L.lens = P.take(ragged_lens_bytes(B));
+  L.total = P.off + 4096;
   return L;
 }
 
@@ -271,36 +270,19 @@ size_t svcb_hubert_workspace_bytes(const svcb_hubert* h, int32_t B, int32_t n_sa
 
 }  // extern "C"
 
-// lens_host: null, or per-item sample counts of a ragged batch (flags 0 only), staged in 8 B bytes past L.total
+// lens_host: null, or per-item sample counts of a ragged batch (flags 0 only)
 static int hubert_units(const svcb_hubert* h, const float* wav, float* out, int32_t B, int32_t n_samples, void* ws,
                         size_t ws_bytes, float* const* taps, int32_t flags, const int32_t* lens_host, cudaStream_t s) {
   if (!h || !wav || !out || B <= 0 || n_samples <= 0) { set_error("svcb_hubert_units: bad argument"); return SVCB_E_BAD_SHAPE; }
   const HLayout L = hubert_layout(B, n_samples);
   const int T = L.T[6], M = L.M;
   if (T < 1) { set_error("svcb_hubert_units: audio shorter than one frame"); return SVCB_E_BAD_SHAPE; }
-  std::vector<int> lens;   // [samples of item 0 .. B-1][frames of item 0 .. B-1]
-  if (lens_host) {
-    lens.resize(2 * (size_t)B);
-    for (int b = 0; b < B; ++b) {
-      const int n = lens_host[b], f = n > 0 ? hubert_layout(1, n).T[6] : 0;
-      if (n < 1 || n > n_samples || f < 1) {
-        set_error("svcb_hubert_units_ragged: item " + std::to_string(b) + " has " + std::to_string(n) + " samples; need 1.." +
-                  std::to_string(n_samples) + " and at least one frame");
-        return SVCB_E_BAD_SHAPE;
-      }
-      lens[b] = n; lens[B + b] = f;
-    }
-  }
-  const size_t need = L.total + (lens_host ? 8 * (size_t)B : 0);
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < need) { set_error("hubert workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
+  RaggedLens ragged;   // samples, frames
+  SVCB_TRY(ragged.validate(lens_host, B, n_samples, [](int n) { return hubert_layout(1, n).T[6]; }, "svcb_hubert_units_ragged",
+                         "samples"));
+  SVCB_TRY(check_workspace(ws, ws_bytes, L.total, "hubert"));
   char* base = static_cast<char*>(ws);
-  const int* d_samples = nullptr;
-  const int* d_frames = nullptr;
-  if (lens_host) {
-    int* d = reinterpret_cast<int*>(base + L.total);
-    SVCB_TRY(launch_stage_ints(lens.data(), (int)lens.size(), d, s));
-    d_samples = d; d_frames = d + B;
-  }
+  SVCB_TRY(ragged.stage(base + L.lens, s));
   float* bufa = reinterpret_cast<float*>(base + L.bufa);
   float* bufb = reinterpret_cast<float*>(base + L.bufb);
   float* rows = reinterpret_cast<float*>(base + L.rows);
@@ -331,13 +313,13 @@ static int hubert_units(const svcb_hubert* h, const float* wav, float* out, int3
       float2* stats = reinterpret_cast<float2*>(base + L.stats);
       {
         KernelScope ks("hubert_conv0_stats", s, 20.0 * B * HB_C * (double)L.T[0], 4.0 * B * (double)n_samples);
-        hubert_conv0_stats_kernel<<<dim3(HB_C / 8, B), 256, 0, s>>>(wav, h->conv0_w, stats, n_samples, L.T[0], 1e-5f, d_samples);
+        hubert_conv0_stats_kernel<<<dim3(HB_C / 8, B), 256, 0, s>>>(wav, h->conv0_w, stats, n_samples, L.T[0], 1e-5f, ragged.lens);
         SVCB_LAUNCH_CHECK("hubert_conv0_stats");
       }
       {
         KernelScope ks("hubert_conv0_pack", s, 20.0 * B * HB_C * (double)L.T[0], 4.0 * B * (double)n_samples + 2.0 * B * 3 * HB_C * (double)L.T[1]);
         hubert_conv0_pack_kernel<<<dim3((L.T[0] + 127) / 128, HB_C / 8, B), 128, 0, s>>>(
-            wav, h->conv0_w, stats, h->gn_g, h->gn_b, static_cast<__nv_bfloat16*>(img[0]), n_samples, L.T[0], L.T[1], d_samples);
+            wav, h->conv0_w, stats, h->gn_g, h->gn_b, static_cast<__nv_bfloat16*>(img[0]), n_samples, L.T[0], L.T[1], ragged.lens);
         SVCB_LAUNCH_CHECK("hubert_conv0_pack");
       }
     }
@@ -371,7 +353,7 @@ static int hubert_units(const svcb_hubert* h, const float* wav, float* out, int3
   // y = x + GELU(pos_conv(x)[..., :-1]): 16 groups of 48 channels, 128 taps, two 24-channel halves per group
   for (int g = 0; g < HB_PG && !(flags & 2); ++g) {   // tensor cores: per group an im2col image (K = 128 x 48) x [256 (48 used), K]
     const int cg = HB_D / HB_PG, c0 = g * cg;
-    SVCB_TRY(launch_im2col_rows_image(x, base + L.posimg, B, T, HB_D, c0, cg, HB_PK, HB_PK / 2, s, d_frames));
+    SVCB_TRY(launch_im2col_rows_image(x, base + L.posimg, B, T, HB_D, c0, cg, HB_PK, HB_PK / 2, s, ragged.out_lens));
     SVCB_TRY(launch_gemm_tc(base + L.posimg, h->pos_wimg[g], h->pos_bimg[g], y + c0, x + c0, M, 256, HB_PK * cg, EPI_GELU_ADD_F32_LD, s, cg, HB_D));
   }
   for (int g = 0; g < HB_PG && (flags & 2); ++g)       // flags bit 1: fp32 on the CUDA cores
@@ -392,7 +374,7 @@ static int hubert_units(const svcb_hubert* h, const float* wav, float* out, int3
   for (int i = 0; i < h->n_layer; ++i) {   // post-LN layers: x = LN1(x + SA(x)); x = LN2(x + W2 gelu(W1 x))
     const HLayer& l = h->layers[i];
     SVCB_TRY(launch_gemm_tc(a, l.wqkv, l.bqkv, qkv, nullptr, M, 3 * HB_D, HB_D, EPI_QKV_HEADS, s, T));
-    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, T, HB_D, HB_H, 0, s, d_frames));
+    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, T, HB_D, HB_H, 0, s, ragged.out_lens));
     SVCB_TRY(launch_gemm_tc(att, l.wo, l.bo, y, x, M, HB_D, HB_D, EPI_RESID_F32, s));
     SVCB_TRY(launch_ln_rows(y, l.ln1g, l.ln1b, a, M, HB_D, true, s, x));
     SVCB_TRY(launch_gemm_tc(a, l.w1, l.b1, mid, nullptr, M, HB_FF, HB_D, EPI_GELU_BF16_IMAGE, s));
@@ -402,8 +384,7 @@ static int hubert_units(const svcb_hubert* h, const float* wav, float* out, int3
   }
   SVCB_TRY(tap(4, x, (size_t)M * HB_D));
   SVCB_TRY(launch_gemm_tc(a, h->proj_w, h->proj_b, out, nullptr, M, HB_OUT, HB_D, EPI_RESID_F32, s));
-  if (!lens_host) return SVCB_OK;
-  return launch_zero_tail_rows(out, d_frames, B, T, HB_OUT, *std::min_element(lens.begin() + B, lens.end()), s);
+  return ragged.zero_tail(out, T, HB_OUT, s);
 }
 
 extern "C" {

@@ -202,7 +202,6 @@ km_split_kernel(float* __restrict__ centroids, const int* __restrict__ pairs, in
   }
 }
 
-static size_t km_align(size_t x) { return (x + 255) & ~(size_t)255; }
 static int km_np(int k) { return (k + 255) / 256 * 256; }
 static int km_chunk(int chunk) { return chunk <= 0 ? KM_DEFAULT_CHUNK : (chunk + 127) / 128 * 128; }
 
@@ -218,9 +217,10 @@ struct KmAssignLayout {
 };
 static KmAssignLayout km_assign_layout(int d, int k, int chunk) {
   KmAssignLayout L;
-  L.img = 0;
-  L.cand = km_align((size_t)chunk * 3 * d * 2);
-  L.total = km_align(L.cand + (size_t)chunk * (km_np(k) / 16) * sizeof(int2));
+  WsPlan P;
+  L.img = P.take((size_t)chunk * 3 * d * 2);
+  L.cand = P.take((size_t)chunk * (km_np(k) / 16) * sizeof(int2));
+  L.total = P.off;
   return L;
 }
 
@@ -232,9 +232,10 @@ static KmUpdateLayout km_update_layout(int n, int k) {
   KmUpdateLayout L;
   L.TR = km_tile_rows(n, k);
   L.ntiles = std::max(1, (n + L.TR - 1) / L.TR);
-  L.tcount = 0;
-  L.ext = km_align((size_t)L.ntiles * k * 4);
-  L.total = km_align(L.ext + (size_t)(k + 1) * 4);
+  WsPlan P;
+  L.tcount = P.take((size_t)L.ntiles * k * 4);
+  L.ext = P.take((size_t)(k + 1) * 4);
+  L.total = P.off;
   return L;
 }
 
@@ -291,7 +292,7 @@ int svcb_kmeans_assign(const float* x, const float* centroids, const float* wimg
   if (n == 0) return SVCB_OK;
   const int ch = std::min(km_chunk(chunk), (n + 127) / 128 * 128);
   const KmAssignLayout L = km_assign_layout(d, k, ch);
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < L.total) { set_error("kmeans assign workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
+  SVCB_TRY(check_workspace(ws, ws_bytes, L.total, "kmeans assign"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* base = static_cast<char*>(ws);
   const int Np = km_np(k);
@@ -316,7 +317,7 @@ int svcb_kmeans_update(const float* x, const int32_t* assign, float* centroids, 
     return SVCB_E_BAD_SHAPE;
   }
   const KmUpdateLayout L = km_update_layout(n, k);
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < L.total) { set_error("kmeans update workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
+  SVCB_TRY(check_workspace(ws, ws_bytes, L.total, "kmeans update"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* base = static_cast<char*>(ws);
   int* tcount = reinterpret_cast<int*>(base + L.tcount);

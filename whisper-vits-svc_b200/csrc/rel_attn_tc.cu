@@ -343,10 +343,7 @@ int launch_rel_attention_tc(const float* qkv, const float* ek, const float* ev, 
     return SVCB_E_UNSUPPORTED;
   }
   if (B <= 0 || T <= 0) return SVCB_OK;
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < rel_attention_ws_bytes(B, heads, T)) {
-    set_error("rel_attention_tc: scratch too small or misaligned");
-    return SVCB_E_WORKSPACE;
-  }
+  SVCB_TRY(check_workspace(ws, ws_bytes, rel_attention_ws_bytes(B, heads, T), "rel_attention_tc"));
   const int nq = (T + ra::TQ - 1) / ra::TQ, nk = (T + ra::TK - 1) / ra::TK;
   uint8_t* qimg = static_cast<uint8_t*>(ws);
   uint8_t* kimg = qimg + (size_t)B * heads * nq * ra::Q_TILE;

@@ -215,22 +215,20 @@ int launch_bucket_offsets(const int* count, int* cursor, int n, cudaStream_t s) 
   return SVCB_OK;
 }
 
-static size_t align256r(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct IvfLayout {
   size_t img, cand, probe, count, cursor, order, total;
 };
 static IvfLayout ivf_layout(int d, int Np, int nlist, int np, int M) {
   IvfLayout L;
   const size_t Mp = ((size_t)M + 127) / 128 * 128;
-  size_t off = 0;
-  L.img = off; off = align256r(off + Mp * 3 * d * 2);
-  L.cand = off; off = align256r(off + (size_t)M * (Np / 16) * np * sizeof(int2));
-  L.probe = off; off = align256r(off + (size_t)M * np * 4);
-  L.count = off; off = align256r(off + (size_t)(nlist + 1) * 4);
-  L.cursor = off; off = align256r(off + (size_t)(nlist + 1) * 4);
-  L.order = off; off = align256r(off + (size_t)M * 4);
-  L.total = off;
+  WsPlan P;
+  L.img = P.take(Mp * 3 * d * 2);
+  L.cand = P.take((size_t)M * (Np / 16) * np * sizeof(int2));
+  L.probe = P.take((size_t)M * np * 4);
+  L.count = P.take((size_t)(nlist + 1) * 4);
+  L.cursor = P.take((size_t)(nlist + 1) * 4);
+  L.order = P.take((size_t)M * 4);
+  L.total = P.off;
   return L;
 }
 
@@ -292,7 +290,7 @@ int svcb_ivf_retrieve(const svcb_ivf* ix, const float* x, float* out, float* dis
   const svcb_ivf_config& c = ix->cfg;
   const int np = c.nprobe;
   const IvfLayout L = ivf_layout(c.d, ix->Np, c.nlist, np, M);
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < L.total) { set_error("ivf workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
+  SVCB_TRY(check_workspace(ws, ws_bytes, L.total, "ivf"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* base = static_cast<char*>(ws);
   int* probe = reinterpret_cast<int*>(base + L.probe);

@@ -337,21 +337,19 @@ spk_finish_kernel(const float* __restrict__ proj, float* __restrict__ out, float
   out[(size_t)b * SPK_P + j] = acc / (float)SPK_NWIN;
 }
 
-static size_t align256s(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct SpkLayout {
   size_t img, G, himg, proj, last, total;
 };
 // R = Lw * Mp rows; the layer-0 rows (R x 128 fp32) live in the projection buffer
 static SpkLayout spk_layout(size_t R, int Mp) {
   SpkLayout L;
-  size_t off = 0;
-  L.img = off; off = align256s(off + R * 3 * SPK_P * 2);
-  L.G = off; off = align256s(off + R * SPK_G4 * 4);
-  L.himg = off; off = align256s(off + R * SPK_HK * 2);
-  L.proj = off; off = align256s(off + R * SPK_P * 4);
-  L.last = off; off = align256s(off + (size_t)Mp * SPK_HK * 2);
-  L.total = off;
+  WsPlan P;
+  L.img = P.take(R * 3 * SPK_P * 2);
+  L.G = P.take(R * SPK_G4 * 4);
+  L.himg = P.take(R * SPK_HK * 2);
+  L.proj = P.take(R * SPK_P * 4);
+  L.last = P.take((size_t)Mp * SPK_HK * 2);
+  L.total = P.off;
   return L;
 }
 static int spk_mp(int nb) { return (nb * SPK_NWIN + 127) / 128 * 128; }
@@ -467,7 +465,7 @@ int svcb_speaker_embed(const svcb_speaker* sp, const float* mel, const int64_t* 
     const int Mp = spk_mp(it.n), rows = SPK_NWIN * it.n;
     const size_t R = (size_t)Lw * Mp;
     const SpkLayout L = spk_layout(R, Mp);
-    if (!ws || ((uintptr_t)ws & 255) || ws_bytes < L.total) { set_error("speaker workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
+    SVCB_TRY(check_workspace(ws, ws_bytes, L.total, "speaker"));
     void* img = base + L.img;
     float* G = reinterpret_cast<float*>(base + L.G);
     __nv_bfloat16* himg = reinterpret_cast<__nv_bfloat16*>(base + L.himg);

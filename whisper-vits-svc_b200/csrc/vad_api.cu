@@ -339,8 +339,6 @@ vad_rec_kernel(const float* __restrict__ wrec, const float* __restrict__ b1, con
   }
 }
 
-static size_t align256v(size_t x) { return (x + 255) & ~(size_t)255; }
-
 static DevSmemCache g_front_smem, g_rec_smem_v;
 
 }  // namespace svcb
@@ -410,7 +408,7 @@ int64_t svcb_vad_windows(int64_t n_samples) { return n_samples <= 0 ? 0 : (n_sam
 
 size_t svcb_vad_workspace_bytes(const svcb_vad* v, int32_t B, int64_t total_windows) {
   if (!v || B <= 0 || total_windows <= 0) return 0;
-  return align256v((size_t)total_windows * VAD_G * sizeof(float));
+  return align256((size_t)total_windows * VAD_G * sizeof(float));
 }
 
 int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_offsets_host, int32_t B, float* probs_out,
@@ -427,10 +425,7 @@ int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_of
   }
   if (total == 0) return SVCB_OK;
   if (!wav || !probs_out) { set_error("svcb_vad_probs: bad argument"); return SVCB_E_BAD_SHAPE; }
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < svcb_vad_workspace_bytes(v, B, total)) {
-    set_error("vad workspace too small or misaligned");
-    return SVCB_E_WORKSPACE;
-  }
+  SVCB_TRY(check_workspace(ws, ws_bytes, svcb_vad_workspace_bytes(v, B, total), "vad"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   float* G = static_cast<float*>(ws);
   SVCB_CUDA_CHECK(ensure_dyn_smem(vad_front_kernel, VAD_FRONT_SMEM, g_front_smem));

@@ -7,7 +7,6 @@
 // padding), conv1 scatters its frames past F_b into conv2's image as zeros (conv2's padding: for odd F_b the last
 // position reads h1[F_b]), and attention masks keys past T_b = (F_b - 1) / 2 + 1.  The other stages are row-local, so
 // an item's rows are the bits a lone run of it computes.
-#include <algorithm>
 #include <memory>
 #include <string>
 #include <vector>
@@ -29,10 +28,8 @@ struct svcb_whisper {
 
 using namespace svcb;
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct WLayout {
-  size_t h1, x, a, qkv, att, mid, total;
+  size_t h1, x, a, qkv, att, mid, lens, total;
   int n2, M;
 };
 static WLayout whisper_layout(const svcb_whisper_config& c, int B, int n) {
@@ -40,17 +37,18 @@ static WLayout whisper_layout(const svcb_whisper_config& c, int B, int n) {
   L.n2 = (n - 1) / 2 + 1;
   L.M = B * L.n2;
   const size_t D = c.n_state;
-  size_t off = 0;
-  // im2col tile image of the log-mel for conv1: [ceil(B n / 128)][K1p / 64][8][128][8] bf16, K1p = 3 n_mels padded to 64
-  L.h1 = off; off = align256(off + ((size_t)B * n + 127) / 128 * 128 * ((3 * (size_t)c.n_mels + 63) / 64 * 64) * 2);
-  L.x = off; off = align256(off + (size_t)L.M * D * 4);
   const size_t Mp = (size_t)(L.M + 127) / 128 * 128;  // tile images are padded to whole 128-row tiles
-  L.a = off; off = align256(off + Mp * D * 2);
+  WsPlan P;
+  // im2col tile image of the log-mel for conv1: [ceil(B n / 128)][K1p / 64][8][128][8] bf16, K1p = 3 n_mels padded to 64
+  L.h1 = P.take(((size_t)B * n + 127) / 128 * 128 * ((3 * (size_t)c.n_mels + 63) / 64 * 64) * 2);
+  L.x = P.take((size_t)L.M * D * 4);
+  L.a = P.take(Mp * D * 2);
   // QKV in the attention kernel's head-major layout (common.cuh qkv_heads_off): items padded to 128 positions
-  L.qkv = off; off = align256(off + (size_t)B * qkv_heads_tp(L.n2) * 3 * D * 2);
-  L.att = off; off = align256(off + Mp * D * 2);
-  L.mid = off; off = align256(off + Mp * 4 * D * 2);
-  L.total = off + 4096;
+  L.qkv = P.take((size_t)B * qkv_heads_tp(L.n2) * 3 * D * 2);
+  L.att = P.take(Mp * D * 2);
+  L.mid = P.take(Mp * 4 * D * 2);
+  L.lens = P.take(ragged_lens_bytes(B));
+  L.total = P.off + 4096;
   return L;
 }
 
@@ -99,35 +97,18 @@ size_t svcb_whisper_workspace_bytes(const svcb_whisper* w, int32_t B, int32_t n_
 
 }  // extern "C"
 
-// frames_host: null, or per-item mel frame counts of a ragged batch, staged in 8 B bytes past L.total
+// frames_host: null, or per-item mel frame counts of a ragged batch
 static int whisper_encode(const svcb_whisper* w, const float* mel, float* out, int32_t B, int32_t n_frames, void* ws,
                           size_t ws_bytes, const int32_t* frames_host, cudaStream_t s) {
   if (!w || !mel || !out || B <= 0 || n_frames <= 0) { set_error("svcb_whisper_encode: bad argument"); return SVCB_E_BAD_SHAPE; }
   const svcb_whisper_config& c = w->cfg;
   const WLayout L = whisper_layout(c, B, n_frames);
   if (L.n2 > c.n_ctx) { set_error("incorrect audio shape: more than n_audio_ctx positions"); return SVCB_E_BAD_SHAPE; }
-  std::vector<int> lens;   // [frames of item 0 .. B-1][positions of item 0 .. B-1]
-  if (frames_host) {
-    lens.resize(2 * (size_t)B);
-    for (int b = 0; b < B; ++b) {
-      if (frames_host[b] < 1 || frames_host[b] > n_frames) {
-        set_error("svcb_whisper_encode_ragged: item " + std::to_string(b) + " has " + std::to_string(frames_host[b]) +
-                  " frames; need 1.." + std::to_string(n_frames));
-        return SVCB_E_BAD_SHAPE;
-      }
-      lens[b] = frames_host[b]; lens[B + b] = (frames_host[b] - 1) / 2 + 1;
-    }
-  }
-  const size_t need = L.total + (frames_host ? 8 * (size_t)B : 0);
-  if (!ws || ((uintptr_t)ws & 255) || ws_bytes < need) { set_error("whisper workspace too small or misaligned"); return SVCB_E_WORKSPACE; }
+  RaggedLens ragged;   // frames, positions
+  SVCB_TRY(ragged.validate(frames_host, B, n_frames, [](int f) { return (f - 1) / 2 + 1; }, "svcb_whisper_encode_ragged", "frames"));
+  SVCB_TRY(check_workspace(ws, ws_bytes, L.total, "whisper"));
   char* base = static_cast<char*>(ws);
-  const int* d_frames = nullptr;
-  const int* d_pos = nullptr;
-  if (frames_host) {
-    int* d = reinterpret_cast<int*>(base + L.total);
-    SVCB_TRY(launch_stage_ints(lens.data(), (int)lens.size(), d, s));
-    d_frames = d; d_pos = d + B;
-  }
+  SVCB_TRY(ragged.stage(base + L.lens, s));
   void* a1 = base + L.h1;
   float* x = reinterpret_cast<float*>(base + L.x);
   void* a = base + L.a; void* qkv = base + L.qkv; void* att = base + L.att; void* mid = base + L.mid;
@@ -138,7 +119,7 @@ static int whisper_encode(const svcb_whisper* w, const float* mel, float* out, i
   // CUDA-core conv1 + the separate im2col pass were 2.0 of the encoder's 33.6 ms.)
   SVCB_CUDA_CHECK(cudaMemsetAsync(mid, 0, (size_t)(M + 127) / 128 * 128 * 3 * D * 2, s));
   SVCB_TRY(launch_im2col_s1_image(mel, a1, B, c.n_mels, n, s));
-  SVCB_TRY(launch_gemm_tc(a1, w->conv1_wimg, w->conv1_b, mid, nullptr, B * n, D, (3 * c.n_mels + 63) / 64 * 64, EPI_GELU_CONV2_IMG, s, n, 0, d_frames));
+  SVCB_TRY(launch_gemm_tc(a1, w->conv1_wimg, w->conv1_b, mid, nullptr, B * n, D, (3 * c.n_mels + 63) / 64 * 64, EPI_GELU_CONV2_IMG, s, n, 0, ragged.lens));
   // conv2 (k=3, stride 2) + GELU + positional embedding, time-major (:150-157): im2col image x the [D, 3D] weight image
   SVCB_TRY(launch_gemm_tc(mid, w->conv2_wimg, w->conv2_b, x, w->pos, M, D, 3 * D, EPI_GELU_ADD_F32, s, n2));
   // pad positions of the head-major QKV buffer are read (times P = 0) but never written: keep them finite
@@ -147,15 +128,14 @@ static int whisper_encode(const svcb_whisper* w, const float* mel, float* out, i
     const WBlock& b = w->blocks[i];
     SVCB_TRY(launch_ln_rows(x, b.ln1g, b.ln1b, a, M, D, true, s));
     SVCB_TRY(launch_gemm_tc(a, b.wqkv, b.bqkv, qkv, nullptr, M, 3 * D, D, EPI_QKV_HEADS, s, n2));
-    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, n2, D, c.n_head, 0, s, d_pos));
+    SVCB_TRY(launch_whisper_attention_tc(qkv, att, B, n2, D, c.n_head, 0, s, ragged.out_lens));
     SVCB_TRY(launch_gemm_tc(att, b.wo, b.bo, x, x, M, D, D, EPI_RESID_F32, s));
     SVCB_TRY(launch_ln_rows(x, b.ln2g, b.ln2b, a, M, D, true, s));
     SVCB_TRY(launch_gemm_tc(a, b.w1, b.b1, mid, nullptr, M, 4 * D, D, EPI_GELU_BF16_IMAGE, s));
     SVCB_TRY(launch_gemm_tc(mid, b.w2, b.b2, x, x, M, D, 4 * D, EPI_RESID_F32, s));
   }
   SVCB_TRY(launch_ln_rows(x, w->lnp_g, w->lnp_b, out, M, D, false, s));
-  if (!frames_host) return SVCB_OK;
-  return launch_zero_tail_rows(out, d_pos, B, n2, D, *std::min_element(lens.begin() + B, lens.end()), s);
+  return ragged.zero_tail(out, n2, D, s);
 }
 
 extern "C" {
@@ -209,7 +189,7 @@ int svcb_op_gemm_bf16(const void* A_bf16, const void* W_bf16, const float* bias,
   if (!scratch || scratch_bytes < svcb_op_gemm_bf16_scratch_bytes(M, N, K)) { set_error("gemm scratch too small"); return SVCB_E_WORKSPACE; }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* a_img = static_cast<char*>(scratch);
-  char* w_img = a_img + (((size_t)(M + 127) / 128 * 128 * K * 2 + 255) & ~(size_t)255);
+  char* w_img = a_img + align256((size_t)(M + 127) / 128 * 128 * K * 2);
   SVCB_TRY(launch_rowmajor_to_image(A_bf16, a_img, M, K, 128, s));
   SVCB_TRY(launch_rowmajor_to_image(W_bf16, w_img, N, K, 256, s));
   return launch_gemm_tc(a_img, w_img, bias, out, res, M, N, K, static_cast<GemmEpi>(epilogue), s);
@@ -224,10 +204,7 @@ size_t svcb_op_attention_tc_bf16_scratch_bytes(int32_t B, int32_t T, int32_t D) 
 int svcb_op_attention_tc_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, int32_t T, int32_t D, int32_t heads,
                               int32_t v_layout, void* scratch, size_t scratch_bytes, svcb_stream stream) {
   // row-major q|k|v in, converted to the GEMM tile image the encoder produces; result converted back
-  if (!scratch || ((uintptr_t)scratch & 255) || scratch_bytes < svcb_op_attention_tc_bf16_scratch_bytes(B, T, D)) {
-    set_error("attention_tc scratch too small or misaligned");
-    return SVCB_E_WORKSPACE;
-  }
+  SVCB_TRY(check_workspace(scratch, scratch_bytes, svcb_op_attention_tc_bf16_scratch_bytes(B, T, D), "attention_tc"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t M = (size_t)B * T;
   char* qimg = static_cast<char*>(scratch);

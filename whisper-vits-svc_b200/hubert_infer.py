@@ -84,28 +84,13 @@ class HubertSoftB200:
     """`HubertSoft` of the reference for inference: `units(wav)` with wav [B, 1, N] or [B, N] -> [B, T, 256] fp32."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], device):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.SvcbError("HuBERT-Soft runs only on a CUDA (sm_90a) device; no CPU fallback")
+        self.device = _lib.cuda_device(device)
         items, self.n_layer = pack_hubert(state_dict)
         blob_cpu, table = pack.build_blob(items)
-        blob = blob_cpu.to(self.device)
-        lib = _lib.load()
-        entries = (_lib.TensorEntry * len(table))()
-        for e, (name, off, numel) in zip(entries, table):
-            e.name = name.encode(); e.offset_bytes = off; e.numel = numel
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            st = lib.svcb_hubert_create(blob.data_ptr(), blob.numel() * 4, entries, len(table), self.n_layer, ctypes.byref(h))
-        _lib.check(st, "svcb_hubert_create")
-        self._blob, self._handle, self._ws = blob, h, None
+        self._handle = _lib.Handle("hubert", table, blob_cpu.to(self.device), self.n_layer)
 
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) is not None:
-                _lib.load().svcb_hubert_destroy(self._handle)
-        except Exception:
-            pass
+    def _workspace(self, B: int, N: int) -> torch.Tensor:
+        return self._handle.workspace(_lib.load().svcb_hubert_workspace_bytes(self._handle, B, N))
 
     def eval(self):
         return self
@@ -121,22 +106,17 @@ class HubertSoftB200:
             wav = wav[:, 0]
         wav = wav.to(self.device, torch.float32).contiguous()
         B, N = wav.shape
-        lib = _lib.load()
         T = self.frames(N)
         if T < 1:
             raise _lib.SvcbError("audio shorter than one HuBERT frame")
-        need = int(lib.svcb_hubert_workspace_bytes(self._handle, B, N))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        ws = self._workspace(B, N)
         out = torch.empty(B, T, 256, device=self.device, dtype=torch.float32)
         tap_arr = None
         if taps is not None:
             bufs = [torch.empty(B, T, w, device=self.device, dtype=torch.float32) for w in TAP_WIDTH]
             tap_arr = (ctypes.c_void_p * len(bufs))(*[b.data_ptr() for b in bufs])
-        with torch.cuda.device(self.device):
-            st = lib.svcb_hubert_units(self._handle, wav.data_ptr(), out.data_ptr(), B, N, self._ws.data_ptr(), self._ws.numel(),
-                                       tap_arr, 3 if fp32_stem else 0, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check(st, "svcb_hubert_units")
+        self._handle.call("hubert_units", wav.data_ptr(), out.data_ptr(), B, N, ws.data_ptr(), ws.numel(), tap_arr,
+                          3 if fp32_stem else 0)
         if taps is not None:
             for n, b in zip(TAP_NAMES, bufs):
                 taps[n] = b
@@ -149,16 +129,10 @@ class HubertSoftB200:
         wav = wav.to(self.device, torch.float32).contiguous()
         B, N = wav.shape
         assert len(n_samples) == B
-        lib = _lib.load()
-        need = int(lib.svcb_hubert_workspace_bytes(self._handle, B, N)) + 8 * B
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        ws = self._workspace(B, N)
         out = torch.empty(B, self.frames(N), 256, device=self.device, dtype=torch.float32)
         lens = (ctypes.c_int32 * B)(*n_samples)
-        with torch.cuda.device(self.device):
-            st = lib.svcb_hubert_units_ragged(self._handle, wav.data_ptr(), lens, out.data_ptr(), B, N, self._ws.data_ptr(),
-                                              self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check(st, "svcb_hubert_units_ragged")
+        self._handle.call("hubert_units_ragged", wav.data_ptr(), lens, out.data_ptr(), B, N, ws.data_ptr(), ws.numel())
         return out
 
 

@@ -39,10 +39,7 @@ class SynthesizerInfer(torch.nn.Module):
         self._keys = list(proto.keys())
         for k, v in proto.items():
             self.register_buffer(self._mangle(k), v, persistent=True)
-        self._handle = None
-        self._blob = None
-        self._ws = None
-        self._packed_device = None
+        self._handle: Optional[_lib.Handle] = None
 
     # ---- state-dict surface (reference key names) -----------------------------------------
     @staticmethod
@@ -62,7 +59,7 @@ class SynthesizerInfer(torch.nn.Module):
                 if tuple(sd[k].shape) != tuple(cur.shape):
                     raise ValueError(f"shape mismatch for {k}: {tuple(sd[k].shape)} vs {tuple(cur.shape)}")
                 cur.copy_(sd[k].to(cur.device, torch.float32))
-        self._release()
+        self._handle = None
         return self
 
     def remove_weight_norm(self):
@@ -75,30 +72,14 @@ class SynthesizerInfer(torch.nn.Module):
         return self.inference(ppg, vec, pit, spk, ppg_l, source, **kw)
 
     # ---- device plumbing -------------------------------------------------------------------
-    def _release(self):
-        if self._handle is not None:
-            _lib.load().svcb_model_destroy(self._handle)
-        self._handle = None
-        self._blob = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
-
     def _device(self) -> torch.device:
         return getattr(self, self._mangle(self._keys[0])).device
 
     def _ensure(self):
-        dev = self._device()
-        if dev.type != "cuda":
-            raise _lib.SvcbError("SynthesizerInfer computes only on a CUDA device (sm_90a); "
-                                 "call .to('cuda') first. There is no CPU fallback.")
-        if self._handle is not None and self._packed_device == dev:
+        dev = _lib.cuda_device(self._device())
+        if self._handle is not None and self._handle.device == dev:
             return
-        self._release()
-        lib = _lib.load()
+        self._handle = None
         sd_cpu = {k: v.detach().cpu() for k, v in self.state_dict().items()}
         items = pack.pack_svc_state_dict(sd_cpu, self._cfg)
         blob_cpu, table = pack.build_blob(items)
@@ -107,40 +88,18 @@ class SynthesizerInfer(torch.nn.Module):
     def install_blob(self, blob_dev: torch.Tensor, table):
         """Create the device handle from an already packed blob (used by the multi-GPU path after
         the NCCL broadcast of rank 0's blob)."""
-        lib = _lib.load()
-        self._release()
-        entries = (_lib.TensorEntry * len(table))()
-        for e, (name, off, numel) in zip(entries, table):
-            e.name = name.encode()
-            e.offset_bytes = off
-            e.numel = numel
-        cfg = _lib.Config.from_dict(self._cfg)
-        handle = ctypes.c_void_p()
-        with torch.cuda.device(blob_dev.device):
-            st = lib.svcb_model_create(blob_dev.data_ptr(), blob_dev.numel() * 4, entries, len(table),
-                                       ctypes.byref(cfg), ctypes.byref(handle))
-        _lib.check(st, "svcb_model_create")
-        self._blob = blob_dev
-        self._table = table
-        self._handle = handle
-        self._packed_device = blob_dev.device
+        self._handle = None
+        self._handle = _lib.Handle("model", table, blob_dev, _lib.Config.from_dict(self._cfg))
 
     def packed_blob(self):
         self._ensure()
-        return self._blob, self._table
+        return self._handle.blob, self._handle.table
 
     def _workspace(self, B: int, T: int) -> torch.Tensor:
-        need = int(_lib.load().svcb_workspace_bytes(self._handle, B, T))
-        if self._ws is None or self._ws.numel() < need or self._ws.device != self._packed_device:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self._packed_device)
-        return self._ws
-
-    @staticmethod
-    def _stream():
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        return self._handle.workspace(_lib.load().svcb_workspace_bytes(self._handle, B, T))
 
     def _f32(self, t: torch.Tensor) -> torch.Tensor:
-        return t.to(self._packed_device, torch.float32).contiguous()
+        return t.to(self._handle.device, torch.float32).contiguous()
 
     def _taps(self, taps: Optional[Dict[str, torch.Tensor]]):
         if not taps:
@@ -160,7 +119,7 @@ class SynthesizerInfer(torch.nn.Module):
         B, T = f0.shape
         L = T * self.hop
         nh = self._cfg["n_harmonics"]
-        dev = self._packed_device
+        dev = self._handle.device
         if rand_ini is None:
             rand_ini = torch.rand(B, nh, device=dev)
         if noise is None:
@@ -171,10 +130,8 @@ class SynthesizerInfer(torch.nn.Module):
         # the source scan needs O(B*T) bytes, not the pipeline's peak: the host loop calls this on the
         # whole utterance before chunking (svc_inference.py:89-91)
         ws = torch.empty(int(_lib.load().svcb_source_workspace_bytes(self._handle, B, T)), dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = _lib.load().svcb_source(self._handle, f0.data_ptr(), rand_ini.data_ptr(), noise.data_ptr(),
-                                         out.data_ptr(), B, T, ws.data_ptr(), ws.numel(), self._stream())
-        _lib.check(st, "svcb_source")
+        self._handle.call("source", f0.data_ptr(), rand_ini.data_ptr(), noise.data_ptr(), out.data_ptr(), B, T,
+                          ws.data_ptr(), ws.numel())
         return out
 
     @torch.no_grad()
@@ -183,9 +140,7 @@ class SynthesizerInfer(torch.nn.Module):
         self._ensure()
         src = self._f32(source).reshape(-1)
         out = torch.empty(src.numel(), dtype=torch.int16, device=src.device)
-        with torch.cuda.device(src.device):
-            st = _lib.load().svcb_source2wav(src.data_ptr(), out.data_ptr(), src.numel(), self._stream())
-        _lib.check(st, "svcb_source2wav")
+        _lib.call("source2wav", src.data_ptr(), out.data_ptr(), src.numel(), device=src.device)
         return out.cpu().numpy()
 
     @torch.no_grad()
@@ -194,7 +149,7 @@ class SynthesizerInfer(torch.nn.Module):
         ppg [B,T,ppg_dim], vec [B,T,vec_dim], pit [B,T], spk [B,spk_dim], ppg_l [B] int64,
         source [B,1,T*hop] -> wave [B,1,T*hop]."""
         self._ensure()
-        dev = self._packed_device
+        dev = self._handle.device
         ppg, vec, pit, spk, source = map(self._f32, (ppg, vec, pit, spk, source))
         B, T, _ = ppg.shape
         C = self._cfg["inter_channels"]
@@ -206,60 +161,46 @@ class SynthesizerInfer(torch.nn.Module):
         assert source.shape == (B, 1, T * self.hop) and eps.shape == (B, C, T)
         wave = torch.empty(B, 1, T * self.hop, device=dev, dtype=torch.float32)
         ws = self._workspace(B, T)
-        with torch.cuda.device(dev):
-            st = _lib.load().svcb_infer(self._handle, ppg.data_ptr(), vec.data_ptr(), pit.data_ptr(),
-                                        spk.data_ptr(), lengths.data_ptr(), source.data_ptr(), eps.data_ptr(),
-                                        wave.data_ptr(), B, T, ws.data_ptr(), ws.numel(), self._taps(taps),
-                                        self._stream())
-        _lib.check(st, "svcb_infer")
+        self._handle.call("infer", ppg.data_ptr(), vec.data_ptr(), pit.data_ptr(), spk.data_ptr(), lengths.data_ptr(),
+                          source.data_ptr(), eps.data_ptr(), wave.data_ptr(), B, T, ws.data_ptr(), ws.numel(),
+                          self._taps(taps))
         return wave
 
     # ---- stage entry points (parity tests, profiling) ---------------------------------------
     @torch.no_grad()
     def prior(self, ppg, vec, pit, ppg_l, eps, taps=None):
         self._ensure()
-        dev = self._packed_device
+        dev = self._handle.device
         ppg, vec, pit, eps = map(self._f32, (ppg, vec, pit, eps))
         B, T, _ = ppg.shape
         lengths = ppg_l.to(dev, torch.int64).contiguous()
         z_p = torch.empty(B, self._cfg["inter_channels"], T, device=dev)
         ws = self._workspace(B, T)
-        with torch.cuda.device(dev):
-            st = _lib.load().svcb_prior(self._handle, ppg.data_ptr(), vec.data_ptr(), pit.data_ptr(),
-                                        lengths.data_ptr(), eps.data_ptr(), z_p.data_ptr(), B, T,
-                                        ws.data_ptr(), ws.numel(), self._taps(taps), self._stream())
-        _lib.check(st, "svcb_prior")
+        self._handle.call("prior", ppg.data_ptr(), vec.data_ptr(), pit.data_ptr(), lengths.data_ptr(), eps.data_ptr(),
+                          z_p.data_ptr(), B, T, ws.data_ptr(), ws.numel(), self._taps(taps))
         return z_p
 
     @torch.no_grad()
     def flow_reverse(self, z_p, ppg_l, spk, taps=None):
         self._ensure()
-        dev = self._packed_device
         z_p, spk = self._f32(z_p), self._f32(spk)
         B, C, T = z_p.shape
-        lengths = ppg_l.to(dev, torch.int64).contiguous()
+        lengths = ppg_l.to(self._handle.device, torch.int64).contiguous()
         z = torch.empty_like(z_p)
         ws = self._workspace(B, T)
-        with torch.cuda.device(dev):
-            st = _lib.load().svcb_flow(self._handle, z_p.data_ptr(), lengths.data_ptr(), spk.data_ptr(),
-                                       z.data_ptr(), B, T, ws.data_ptr(), ws.numel(), self._taps(taps),
-                                       self._stream())
-        _lib.check(st, "svcb_flow")
+        self._handle.call("flow", z_p.data_ptr(), lengths.data_ptr(), spk.data_ptr(), z.data_ptr(), B, T, ws.data_ptr(),
+                          ws.numel(), self._taps(taps))
         return z
 
     @torch.no_grad()
     def generator(self, spk, z, source, taps=None):
         """Generator.inference(spk, x, har_source) (vits_decoder/generator.py:175-200)."""
         self._ensure()
-        dev = self._packed_device
         spk, z, source = map(self._f32, (spk, z, source))
         B, U, T = z.shape
         assert U == self._cfg["gen_input"] and source.shape == (B, 1, T * self.hop)
-        wave = torch.empty(B, 1, T * self.hop, device=dev)
+        wave = torch.empty(B, 1, T * self.hop, device=self._handle.device)
         ws = self._workspace(B, T)
-        with torch.cuda.device(dev):
-            st = _lib.load().svcb_generator(self._handle, spk.data_ptr(), z.data_ptr(), source.data_ptr(),
-                                            wave.data_ptr(), B, T, ws.data_ptr(), ws.numel(),
-                                            self._taps(taps), self._stream())
-        _lib.check(st, "svcb_generator")
+        self._handle.call("generator", spk.data_ptr(), z.data_ptr(), source.data_ptr(), wave.data_ptr(), B, T,
+                          ws.data_ptr(), ws.numel(), self._taps(taps))
         return wave

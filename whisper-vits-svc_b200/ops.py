@@ -2,15 +2,9 @@
 The same kernels the stage pipelines launch; no fallback."""
 from __future__ import annotations
 
-import ctypes
-
 import torch
 
 from . import _lib, pack
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _c(t):
@@ -27,9 +21,8 @@ def conv1d(x, weight, bias=None, stride=1, padding=0, dilation=1, act=0):
     b = _c(bias) if bias is not None else None
     Tout = (Tin + 2 * padding - dilation * (K - 1) - 1) // stride + 1
     y = torch.empty(B, Cout, Tout, device=x.device)
-    st = _lib.load().svcb_op_conv1d(x.data_ptr(), wp.data_ptr(), b.data_ptr() if b is not None else None,
-                                    y.data_ptr(), B, Cin, Cout, Tin, K, stride, dilation, padding, act, _s())
-    _lib.check(st, "svcb_op_conv1d")
+    _lib.call("op_conv1d", x.data_ptr(), wp.data_ptr(), b.data_ptr() if b is not None else None,
+              y.data_ptr(), B, Cin, Cout, Tin, K, stride, dilation, padding, act, device=x.device)
     return y
 
 
@@ -40,9 +33,8 @@ def snake_alias(x, alpha, beta, fu, fd):
     ib = _c((1.0 / (torch.exp(beta.float().cpu()) + 1e-9)).to(x.device))
     fu, fd = _c(fu.reshape(-1).to(x.device)), _c(fd.reshape(-1).to(x.device))
     y = torch.empty_like(x)
-    st = _lib.load().svcb_op_snake_alias(x.data_ptr(), y.data_ptr(), ea.data_ptr(), ib.data_ptr(),
-                                         fu.data_ptr(), fd.data_ptr(), B, C, L, _s())
-    _lib.check(st, "svcb_op_snake_alias")
+    _lib.call("op_snake_alias", x.data_ptr(), y.data_ptr(), ea.data_ptr(), ib.data_ptr(),
+              fu.data_ptr(), fd.data_ptr(), B, C, L, device=x.device)
     return y
 
 
@@ -53,10 +45,8 @@ def layernorm_c(x, r, gamma, beta, eps=1e-5):
     stride = C if gamma.dim() == 2 else 0
     r_ = _c(r) if r is not None else None
     y = torch.empty_like(x)
-    st = _lib.load().svcb_op_layernorm_c(x.data_ptr(), r_.data_ptr() if r_ is not None else None,
-                                         gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), B, C, T, stride,
-                                         eps, _s())
-    _lib.check(st, "svcb_op_layernorm_c")
+    _lib.call("op_layernorm_c", x.data_ptr(), r_.data_ptr() if r_ is not None else None,
+              gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), B, C, T, stride, eps, device=x.device)
     return y
 
 
@@ -68,15 +58,13 @@ def rel_attention(qkv, emb_k, emb_v, lengths, heads=2, window=4, tc=False):
     lengths = lengths.to(qkv.device, torch.int64).contiguous()
     out = torch.empty(B, H, T, device=qkv.device)
     if tc:
-        lib = _lib.load()
-        scratch = torch.empty(int(lib.svcb_op_rel_attention_tc_scratch_bytes(B, heads, T)), dtype=torch.uint8, device=qkv.device)
-        st = lib.svcb_op_rel_attention_tc(qkv.data_ptr(), ek.data_ptr(), ev.data_ptr(), lengths.data_ptr(), out.data_ptr(),
-                                          B, H, heads, window, T, scratch.data_ptr(), scratch.numel(), _s())
-        _lib.check(st, "svcb_op_rel_attention_tc")
+        scratch = torch.empty(int(_lib.load().svcb_op_rel_attention_tc_scratch_bytes(B, heads, T)), dtype=torch.uint8,
+                              device=qkv.device)
+        _lib.call("op_rel_attention_tc", qkv.data_ptr(), ek.data_ptr(), ev.data_ptr(), lengths.data_ptr(), out.data_ptr(),
+                  B, H, heads, window, T, scratch.data_ptr(), scratch.numel(), device=qkv.device)
         return out
-    st = _lib.load().svcb_op_rel_attention(qkv.data_ptr(), ek.data_ptr(), ev.data_ptr(), lengths.data_ptr(),
-                                           out.data_ptr(), B, H, heads, window, T, _s())
-    _lib.check(st, "svcb_op_rel_attention")
+    _lib.call("op_rel_attention", qkv.data_ptr(), ek.data_ptr(), ev.data_ptr(), lengths.data_ptr(),
+              out.data_ptr(), B, H, heads, window, T, device=qkv.device)
     return out
 
 
@@ -92,13 +80,11 @@ def amp_conv_tc(x, alpha, beta, fu, fd, weight, bias, dilation=1, res=None, nspl
     b = _c(bias)
     r = _c(res) if res is not None else None
     y = torch.empty_like(x)
-    lib = _lib.load()
-    scratch = torch.empty(int(lib.svcb_op_amp_conv_tc_scratch_bytes(B, C, L)), dtype=torch.uint8, device=x.device)
-    st = lib.svcb_op_amp_conv_tc(x.data_ptr(), y.data_ptr(), r.data_ptr() if r is not None else None,
-                                 ea.data_ptr(), ib.data_ptr(), fu.data_ptr(), fd.data_ptr(),
-                                 wtc.data_ptr(), b.data_ptr(), B, C, L, K, dilation, nsplit,
-                                 scratch.data_ptr(), scratch.numel(), _s())
-    _lib.check(st, "svcb_op_amp_conv_tc")
+    scratch = torch.empty(int(_lib.load().svcb_op_amp_conv_tc_scratch_bytes(B, C, L)), dtype=torch.uint8, device=x.device)
+    _lib.call("op_amp_conv_tc", x.data_ptr(), y.data_ptr(), r.data_ptr() if r is not None else None,
+              ea.data_ptr(), ib.data_ptr(), fu.data_ptr(), fd.data_ptr(),
+              wtc.data_ptr(), b.data_ptr(), B, C, L, K, dilation, nsplit,
+              scratch.data_ptr(), scratch.numel(), device=x.device)
     return y
 
 
@@ -122,14 +108,12 @@ def amp_s2d_link(x, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=Non
     rs = _c(res) if res is not None else None
     y = torch.empty_like(x)
     y_act = torch.empty_like(x) if alpha_out is not None else None
-    lib = _lib.load()
-    scratch = torch.empty(int(lib.svcb_op_amp_s2d_link_scratch_bytes(B, C, L)), dtype=torch.uint8, device=x.device)
-    st = lib.svcb_op_amp_s2d_link(x.data_ptr(), y.data_ptr(), rs.data_ptr() if rs is not None else None,
-                                  y_act.data_ptr() if y_act is not None else None, ea_i.data_ptr(), ib_i.data_ptr(),
-                                  ea_o.data_ptr() if ea_o is not None else None, ib_o.data_ptr() if ib_o is not None else None,
-                                  fu.data_ptr(), fd.data_ptr(), w.data_ptr(), b.data_ptr(), B, C, L, K, dilation,
-                                  scratch.data_ptr(), scratch.numel(), _s())
-    _lib.check(st, "svcb_op_amp_s2d_link")
+    scratch = torch.empty(int(_lib.load().svcb_op_amp_s2d_link_scratch_bytes(B, C, L)), dtype=torch.uint8, device=x.device)
+    _lib.call("op_amp_s2d_link", x.data_ptr(), y.data_ptr(), rs.data_ptr() if rs is not None else None,
+              y_act.data_ptr() if y_act is not None else None, ea_i.data_ptr(), ib_i.data_ptr(),
+              ea_o.data_ptr() if ea_o is not None else None, ib_o.data_ptr() if ib_o is not None else None,
+              fu.data_ptr(), fd.data_ptr(), w.data_ptr(), b.data_ptr(), B, C, L, K, dilation,
+              scratch.data_ptr(), scratch.numel(), device=x.device)
     return y, y_act
 
 
@@ -144,9 +128,8 @@ def conv_tc(x, weight, bias=None, dilation=1, res=None, lengths=None, nsplit=3, 
     ln = lengths.to(x.device, torch.int64).contiguous() if lengths is not None else None
     cout_real = Cout // 2 if (flags & 4) else Cout
     y = torch.zeros(B, cout_real, T, device=x.device)
-    st = _lib.load().svcb_op_conv_tc(x.data_ptr(), wtc.data_ptr(), b.data_ptr() if b is not None else None,
-                                     y.data_ptr(), r.data_ptr() if r is not None else None,
-                                     ln.data_ptr() if ln is not None else None, B, Cin, Cout, T, K, dilation,
-                                     nsplit, flags, act, _s())
-    _lib.check(st, "svcb_op_conv_tc")
+    _lib.call("op_conv_tc", x.data_ptr(), wtc.data_ptr(), b.data_ptr() if b is not None else None,
+              y.data_ptr(), r.data_ptr() if r is not None else None,
+              ln.data_ptr() if ln is not None else None, B, Cin, Cout, T, K, dilation,
+              nsplit, flags, act, device=x.device)
     return y

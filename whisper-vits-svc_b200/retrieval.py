@@ -8,7 +8,6 @@ an index vector, or probed lists holding fewer than k vectors) are defined here 
 the weight equally, otherwise the blend runs over the neighbours found, and a row with none passes through unchanged."""
 from __future__ import annotations
 
-import ctypes
 import logging
 import struct
 from dataclasses import dataclass
@@ -195,28 +194,10 @@ class DeviceIVFIndex:
             raise ValueError(f"n-retrieval-vectors must be <= {MAX_K}")
         # index.py:44's `0 > ratio > 1` never holds, so the reference accepts any ratio; so does this class
         self.ratio, self.k, self.d, self.nlist = float(ratio), int(n_nearest_vectors), ix.d, ix.nlist
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.SvcbError("feature retrieval runs only on a CUDA (sm_90a) device; no CPU fallback")
+        self.device = _lib.cuda_device(device)
         items, cfg = pack_ivf(ix)
         blob_cpu, table = pack.build_blob(items)
-        blob = blob_cpu.to(self.device)
-        lib = _lib.load()
-        entries = (_lib.TensorEntry * len(table))()
-        for e, (name, off, numel) in zip(entries, table):
-            e.name = name.encode(); e.offset_bytes = off; e.numel = numel
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            st = lib.svcb_ivf_create(blob.data_ptr(), blob.numel() * 4, entries, len(table), ctypes.byref(cfg), ctypes.byref(h))
-        _lib.check(st, "svcb_ivf_create")
-        self._blob, self._handle, self._ws = blob, h, None
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) is not None:
-                _lib.load().svcb_ivf_destroy(self._handle)
-        except Exception:
-            pass
+        self._handle = _lib.Handle("ivf", table, blob_cpu.to(self.device), cfg)
 
     def _run(self, x: torch.Tensor, k: int, ratio: float, want_out: bool, want_search: bool):
         if x.dim() != 2 or x.shape[1] != self.d:
@@ -227,16 +208,10 @@ class DeviceIVFIndex:
         dist = torch.empty(M, k, device=self.device, dtype=torch.float32) if want_search else None
         ids = torch.empty(M, k, device=self.device, dtype=torch.int64) if want_search else None
         if M:
-            lib = _lib.load()
-            need = int(lib.svcb_ivf_workspace_bytes(self._handle, M, k))
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            ws = self._handle.workspace(_lib.load().svcb_ivf_workspace_bytes(self._handle, M, k))
             ptr = lambda t: None if t is None else t.data_ptr()   # noqa: E731
-            with torch.cuda.device(self.device):
-                st = lib.svcb_ivf_retrieve(self._handle, xd.data_ptr(), ptr(out), ptr(dist), ptr(ids), M, k, float(np.float32(ratio)),
-                                           self._ws.data_ptr(), self._ws.numel(),
-                                           ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-            _lib.check(st, "svcb_ivf_retrieve")
+            self._handle.call("ivf_retrieve", xd.data_ptr(), ptr(out), ptr(dist), ptr(ids), M, k, float(np.float32(ratio)),
+                              ws.data_ptr(), ws.numel())
         return out, dist, ids
 
     @torch.no_grad()

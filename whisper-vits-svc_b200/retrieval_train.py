@@ -17,7 +17,6 @@ Deliberate deviations from the reference:
 * the `*.npy` files are read in sorted path order rather than `rglob` order, so the index is reproducible."""
 from __future__ import annotations
 
-import ctypes
 import logging
 import struct
 import time
@@ -43,17 +42,6 @@ def default_nlist(n: int) -> int:
 
 
 # ------------------------------------------------------------------------------------------------ device steps
-def _cuda(device) -> torch.device:
-    dev = torch.device(device)
-    if dev.type != "cuda":
-        raise _lib.SvcbError("index training runs only on a CUDA (sm_90a) device; no CPU fallback")
-    return dev
-
-
-def _stream(dev):
-    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def _workspace(n: int, d: int, k: int, chunk: int, dev) -> torch.Tensor:
     need = int(_lib.load().svcb_kmeans_workspace_bytes(n, d, k, chunk))
     if need == 0:
@@ -67,9 +55,7 @@ def pack_device(centroids: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     npad = (k + 255) // 256 * 256
     wimg = torch.empty(npad * 3 * d // 2, dtype=torch.float32, device=centroids.device)
     cnorm = torch.empty(npad, dtype=torch.float32, device=centroids.device)
-    with torch.cuda.device(centroids.device):
-        st = _lib.load().svcb_kmeans_pack(centroids.data_ptr(), wimg.data_ptr(), cnorm.data_ptr(), k, d, _stream(centroids.device))
-    _lib.check(st, "svcb_kmeans_pack")
+    _lib.call("kmeans_pack", centroids.data_ptr(), wimg.data_ptr(), cnorm.data_ptr(), k, d, device=centroids.device)
     return wimg, cnorm
 
 
@@ -84,10 +70,8 @@ def assign(x: torch.Tensor, centroids: torch.Tensor, wimg: torch.Tensor, cnorm: 
     dist = torch.empty(n, dtype=torch.float32, device=dev)
     if ws is None:
         ws = _workspace(n, d, k, chunk, dev)
-    with torch.cuda.device(dev):
-        st = _lib.load().svcb_kmeans_assign(x.data_ptr(), centroids.data_ptr(), wimg.data_ptr(), cnorm.data_ptr(), a.data_ptr(),
-                                            dist.data_ptr(), n, d, k, chunk, ws.data_ptr(), ws.numel(), _stream(dev))
-    _lib.check(st, "svcb_kmeans_assign")
+    _lib.call("kmeans_assign", x.data_ptr(), centroids.data_ptr(), wimg.data_ptr(), cnorm.data_ptr(), a.data_ptr(),
+              dist.data_ptr(), n, d, k, chunk, ws.data_ptr(), ws.numel(), device=dev)
     return a, dist
 
 
@@ -102,10 +86,8 @@ def update(x: torch.Tensor, a: torch.Tensor, k: int, centroids: torch.Tensor | N
     if ws is None:
         ws = _workspace(n, d, k, 0, dev)
     cptr = None if centroids is None else centroids.data_ptr()
-    with torch.cuda.device(dev):
-        st = _lib.load().svcb_kmeans_update(x.data_ptr(), a.data_ptr(), cptr, counts.data_ptr(), offsets.data_ptr(),
-                                            order.data_ptr(), n, d, k, ws.data_ptr(), ws.numel(), _stream(dev))
-    _lib.check(st, "svcb_kmeans_update")
+    _lib.call("kmeans_update", x.data_ptr(), a.data_ptr(), cptr, counts.data_ptr(), offsets.data_ptr(),
+              order.data_ptr(), n, d, k, ws.data_ptr(), ws.numel(), device=dev)
     return counts, offsets, order
 
 
@@ -114,10 +96,7 @@ def split(centroids: torch.Tensor, pairs: List[Tuple[int, int]]) -> None:
     if not pairs:
         return
     p = torch.tensor(pairs, dtype=torch.int32).to(centroids.device)
-    with torch.cuda.device(centroids.device):
-        st = _lib.load().svcb_kmeans_split(centroids.data_ptr(), p.data_ptr(), len(pairs), centroids.shape[1],
-                                           _stream(centroids.device))
-    _lib.check(st, "svcb_kmeans_split")
+    _lib.call("kmeans_split", centroids.data_ptr(), p.data_ptr(), len(pairs), centroids.shape[1], device=centroids.device)
 
 
 def split_plan(hassign: np.ndarray, n: int, rng: np.random.Generator) -> List[Tuple[int, int]]:
@@ -152,7 +131,7 @@ def kmeans_step(x: torch.Tensor, centroids: torch.Tensor, chunk: int = 0):
 
 # ------------------------------------------------------------------------------------------------ training
 def _device_rows(x, device) -> torch.Tensor:
-    dev = _cuda(device)
+    dev = _lib.cuda_device(device)
     t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
     return t.to(dev, torch.float32).contiguous()
 

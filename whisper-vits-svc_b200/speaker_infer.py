@@ -192,36 +192,14 @@ def window_offsets(T: int) -> List[int]:
 
 
 # ------------------------------------------------------------------------------------------------ the model
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 class SpeakerEncoderB200:
     """LSTMSpeakerEncoder(80, 256, 768, 3) with its AudioProcessor, for inference."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], audio: dict, device):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.SvcbError("the speaker encoder runs only on a CUDA (sm_90a) device; no CPU fallback")
+        self.device = _lib.cuda_device(device)
         self.audio = dict(audio)
         blob_cpu, table = pack.build_blob(pack_speaker(state_dict, self.audio))
-        blob = blob_cpu.to(self.device)
-        lib = _lib.load()
-        entries = (_lib.TensorEntry * len(table))()
-        for e, (name, off, numel) in zip(entries, table):
-            e.name = name.encode(); e.offset_bytes = off; e.numel = numel
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            st = lib.svcb_speaker_create(blob.data_ptr(), blob.numel() * 4, entries, len(table), ctypes.byref(h))
-        _lib.check(st, "svcb_speaker_create")
-        self._blob, self._handle, self._ws = blob, h, None
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) is not None:
-                _lib.load().svcb_speaker_destroy(self._handle)
-        except Exception:
-            pass
+        self._handle = _lib.Handle("speaker", table, blob_cpu.to(self.device))
 
     @staticmethod
     def frames(n_samples: int) -> int:
@@ -243,9 +221,7 @@ class SpeakerEncoderB200:
         flat = torch.cat(wavs).to(self.device) if wavs else torch.zeros(0, device=self.device)
         mel = torch.empty(max(fo[-1], 1), N_MELS, device=self.device, dtype=torch.float32)
         offs = (ctypes.c_int64 * len(so))(*so)
-        with torch.cuda.device(self.device):
-            st = _lib.load().svcb_speaker_mel(self._handle, flat.data_ptr(), offs, len(wavs), mel.data_ptr(), None, 0, _stream())
-        _lib.check(st, "svcb_speaker_mel")
+        self._handle.call("speaker_mel", flat.data_ptr(), offs, len(wavs), mel.data_ptr(), None, 0)
         return mel[:fo[-1]], fo
 
     @torch.no_grad()
@@ -253,18 +229,12 @@ class SpeakerEncoderB200:
         """mel [sum T_b, 80] (time-major), frame offsets [B + 1] -> [B, 256] (and the window embeddings [B, 10, 256])."""
         mel = mel.to(self.device, torch.float32).contiguous()
         B = len(frame_offsets) - 1
-        lib = _lib.load()
-        need = int(lib.svcb_speaker_workspace_bytes(self._handle, B, int(HOP * max(1, mel.shape[0]))))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        ws = self._handle.workspace(_lib.load().svcb_speaker_workspace_bytes(self._handle, B, int(HOP * max(1, mel.shape[0]))))
         out = torch.empty(B, PROJ, device=self.device, dtype=torch.float32)
         wout = torch.empty(B, NUM_WINDOWS, PROJ, device=self.device, dtype=torch.float32) if windows else None
         offs = (ctypes.c_int64 * (B + 1))(*[int(o) for o in frame_offsets])
-        with torch.cuda.device(self.device):
-            st = lib.svcb_speaker_embed(self._handle, mel.data_ptr(), offs, B, out.data_ptr(),
-                                        wout.data_ptr() if windows else None, self._ws.data_ptr(), self._ws.numel(), _stream())
-        _lib.check(st, "svcb_speaker_embed")
+        self._handle.call("speaker_embed", mel.data_ptr(), offs, B, out.data_ptr(), wout.data_ptr() if windows else None,
+                          ws.data_ptr(), ws.numel())
         return (out, wout) if windows else out
 
     def melspectrogram(self, wav) -> torch.Tensor:

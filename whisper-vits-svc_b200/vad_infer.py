@@ -113,35 +113,16 @@ def windows(n_samples: int) -> int:
     return -(-int(n_samples) // WINDOW) if n_samples > 0 else 0
 
 
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+_stream = _lib.stream   # the stream argument of a direct svcb_vad_* call on a VadB200's `_handle`
 
 
 class VadB200:
     """The 16 kHz Silero VAD, for inference on ragged batches of recordings."""
 
     def __init__(self, tensors: Dict[str, torch.Tensor], device):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.SvcbError("the VAD runs only on a CUDA (sm_90a) device; no CPU fallback")
+        self.device = _lib.cuda_device(device)
         blob_cpu, table = pack.build_blob(pack_vad(tensors))
-        blob = blob_cpu.to(self.device)
-        lib = _lib.load()
-        entries = (_lib.TensorEntry * len(table))()
-        for e, (name, off, numel) in zip(entries, table):
-            e.name = name.encode(); e.offset_bytes = off; e.numel = numel
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            st = lib.svcb_vad_create(blob.data_ptr(), blob.numel() * 4, entries, len(table), ctypes.byref(h))
-        _lib.check(st, "svcb_vad_create")
-        self._blob, self._handle, self._ws = blob, h, None
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) is not None:
-                _lib.load().svcb_vad_destroy(self._handle)
-        except Exception:
-            pass
+        self._handle = _lib.Handle("vad", table, blob_cpu.to(self.device))
 
     @torch.no_grad()
     def speech_probs_device(self, wavs: Sequence, features: bool = False):
@@ -156,17 +137,11 @@ class VadB200:
         probs = torch.empty(max(W, 1), device=self.device, dtype=torch.float32)
         feat = torch.empty(max(W, 1), HIDDEN, device=self.device, dtype=torch.float32) if features else None
         if W > 0:
-            lib = _lib.load()
-            need = int(lib.svcb_vad_workspace_bytes(self._handle, len(wavs), W))
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = None
-                self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            ws = self._handle.workspace(_lib.load().svcb_vad_workspace_bytes(self._handle, len(wavs), W))
             flat = torch.cat(wavs).to(self.device)
             offs = (ctypes.c_int64 * len(so))(*so)
-            with torch.cuda.device(self.device):
-                st = lib.svcb_vad_probs(self._handle, flat.data_ptr(), offs, len(wavs), probs.data_ptr(),
-                                        feat.data_ptr() if features else None, self._ws.data_ptr(), self._ws.numel(), _stream())
-            _lib.check(st, "svcb_vad_probs")
+            self._handle.call("vad_probs", flat.data_ptr(), offs, len(wavs), probs.data_ptr(),
+                              feat.data_ptr() if features else None, ws.data_ptr(), ws.numel())
         out = (probs[:W], wo)
         return out + (feat[:W],) if features else out
 

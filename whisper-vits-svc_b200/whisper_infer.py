@@ -108,36 +108,16 @@ class WhisperEncoderB200:
     """`whisper.encoder(mel)` of the reference: mel [B, n_mels, n] -> [B, (n-1)//2+1, n_state] fp32."""
 
     def __init__(self, ckpt: dict, device):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.SvcbError("the Whisper encoder runs only on a CUDA (sm_90a) device; no CPU fallback")
+        self.device = _lib.cuda_device(device)
         self.dims = dict(ckpt["dims"])
         items, self.cfg = pack_whisper(ckpt)
         blob_cpu, table = pack.build_blob(items)
-        self._install(blob_cpu.to(self.device), table)
-        self._ws = None
+        self._handle = _lib.Handle("whisper", table, blob_cpu.to(self.device), _lib.WhisperConfig(**self.cfg))
         self._filters = mel_filters(self.cfg["n_mels"]).to(self.device).contiguous()
         self._lm_scratch = None
 
-    def _install(self, blob, table):
-        lib = _lib.load()
-        entries = (_lib.TensorEntry * len(table))()
-        for e, (name, off, numel) in zip(entries, table):
-            e.name = name.encode(); e.offset_bytes = off; e.numel = numel
-        cfg = _lib.WhisperConfig(**self.cfg)
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            st = lib.svcb_whisper_create(blob.data_ptr(), blob.numel() * 4, entries, len(table), ctypes.byref(cfg),
-                                         ctypes.byref(h))
-        _lib.check(st, "svcb_whisper_create")
-        self._blob, self._table, self._handle = blob, table, h
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) is not None:
-                _lib.load().svcb_whisper_destroy(self._handle)
-        except Exception:
-            pass
+    def _workspace(self, B: int, n: int) -> torch.Tensor:
+        return self._handle.workspace(_lib.load().svcb_whisper_workspace_bytes(self._handle, B, n))
 
     @torch.no_grad()
     def __call__(self, mel: torch.Tensor) -> torch.Tensor:
@@ -146,17 +126,10 @@ class WhisperEncoderB200:
         assert nm == self.cfg["n_mels"]
         n2 = (n - 1) // 2 + 1
         assert n2 <= self.cfg["n_ctx"], "incorrect audio shape"  # whisper/model.py:155
-        lib = _lib.load()
-        need = int(lib.svcb_whisper_workspace_bytes(self._handle, B, n))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        ws = self._workspace(B, n)
         out = torch.empty(B, n2, self.cfg["n_state"], device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            st = lib.svcb_whisper_encode(self._handle, mel.data_ptr(), out.data_ptr(), B, n, self._ws.data_ptr(),
-                                         self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check(st, "svcb_whisper_encode")
+        self._handle.call("whisper_encode", mel.data_ptr(), out.data_ptr(), B, n, ws.data_ptr(), ws.numel())
         return out
-
 
     @torch.no_grad()
     def log_mel(self, audio: torch.Tensor, noise: Optional[torch.Tensor] = None, noise_gain: float = 0.1) -> torch.Tensor:
@@ -174,12 +147,8 @@ class WhisperEncoderB200:
             assert tuple(noise.shape) == (B, nm, F)
         if self._lm_scratch is None or self._lm_scratch.numel() < B:
             self._lm_scratch = torch.empty(max(B, 64), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            st = _lib.load().svcb_whisper_log_mel(
-                audio.data_ptr(), self._filters.data_ptr(), noise.data_ptr() if noise is not None else None,
-                float(noise_gain), mel.data_ptr(), self._lm_scratch.data_ptr(), B, N, nm,
-                ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check(st, "svcb_whisper_log_mel")
+        _lib.call("whisper_log_mel", audio.data_ptr(), self._filters.data_ptr(), noise.data_ptr() if noise is not None else None,
+                  float(noise_gain), mel.data_ptr(), self._lm_scratch.data_ptr(), B, N, nm, device=self.device)
         return mel
 
     @torch.no_grad()
@@ -195,11 +164,8 @@ class WhisperEncoderB200:
         if self._lm_scratch is None or self._lm_scratch.numel() < 2 * B:
             self._lm_scratch = torch.empty(max(2 * B, 64), dtype=torch.int32, device=self.device)
         lens = (ctypes.c_int32 * B)(*n_samples)
-        with torch.cuda.device(self.device):
-            st = _lib.load().svcb_whisper_log_mel_ragged(
-                audio.data_ptr(), lens, self._filters.data_ptr(), mel.data_ptr(), self._lm_scratch.data_ptr(), B, N, nm,
-                ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check(st, "svcb_whisper_log_mel_ragged")
+        _lib.call("whisper_log_mel_ragged", audio.data_ptr(), lens, self._filters.data_ptr(), mel.data_ptr(),
+                  self._lm_scratch.data_ptr(), B, N, nm, device=self.device)
         return mel
 
     @torch.no_grad()
@@ -212,17 +178,10 @@ class WhisperEncoderB200:
         assert nm == self.cfg["n_mels"] and len(n_frames) == B
         n2 = (n - 1) // 2 + 1
         assert n2 <= self.cfg["n_ctx"], "incorrect audio shape"
-        lib = _lib.load()
-        need = int(lib.svcb_whisper_workspace_bytes(self._handle, B, n)) + 8 * B
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-        ws = self._ws
+        ws = self._workspace(B, n)
         out = torch.empty(B, n2, self.cfg["n_state"], device=self.device, dtype=torch.float32)
         lens = (ctypes.c_int32 * B)(*n_frames)
-        with torch.cuda.device(self.device):
-            st = lib.svcb_whisper_encode_ragged(self._handle, mel.data_ptr(), lens, out.data_ptr(), B, n, ws.data_ptr(),
-                                                ws.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-        _lib.check(st, "svcb_whisper_encode_ragged")
+        self._handle.call("whisper_encode_ragged", mel.data_ptr(), lens, out.data_ptr(), B, n, ws.data_ptr(), ws.numel())
         return out
 
 
