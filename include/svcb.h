@@ -215,6 +215,16 @@ int svcb_whisper_log_mel(const float* audio, const float* mel_filters, const flo
 int svcb_whisper_log_mel_ragged(const float* audio, const int32_t* n_samples_host, const float* mel_filters, float* mel,
                                 void* scratch, int32_t B, int32_t n_samples, int32_t n_mels, svcb_stream stream);
 
+/* ------------------------------------------------------------------ linear spectrogram (training data, 32 kHz) */
+/* Replaces vits/spectrogram.py:spectrogram_torch(y, 1024, sr, 320, 1024, center=False) as prepare/preprocess_spec.py
+ * calls it, for a ragged batch: item b is audio[sample_offsets_host[b] .. sample_offsets_host[b+1]) (fp32, already
+ * divided by max_wav_value), n_b = its length, which must exceed 352 (the reflect padding); B > 0.
+ * out: fp32, item b's [513, n_b / 320] block bin-major, following item b-1's block.  Reflect pad 352 at both ends,
+ * periodic-Hann frames of 1024 at hop 320, magnitude sqrt(re^2 + im^2 + 1e-6), all in fp32 by a direct DFT.  Each
+ * item's block is bitwise that of a lone call.  scratch is not used at present and may be NULL. */
+int svcb_linear_spec_ragged(const float* audio, const int64_t* sample_offsets_host, int32_t B, float* out, void* scratch,
+                            size_t scratch_bytes, svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */

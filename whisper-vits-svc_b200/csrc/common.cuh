@@ -206,6 +206,52 @@ __device__ __forceinline__ void snake8_packed(const float (&x)[24], const SnakeT
 }
 #endif
 
+#ifdef __CUDACC__
+// Direct fp32 DFT of real 1024-sample frames held in shared memory, for CTAs of 256 threads (spk_mel_kernel,
+// spec_kernel).  tw[n] = (cos, sin)(2 pi n / 1024); bin k's twiddle for sample n is tw[k n mod 1024].
+constexpr int kDftN = 1024, kDftThreads = 256;
+__device__ __forceinline__ void dft1024_twiddles(float2* tw, int tid) {
+  for (int n = tid; n < kDftN; n += kDftThreads) {
+    float s, c;
+    sincospif(2.f * (float)n / (float)kDftN, &s, &c);
+    tw[n] = make_float2(c, s);
+  }
+}
+// Bins tid and tid + 256 of FT frames xw[f][0..1024): one twiddle load feeds 2 x FT FMAs.  mg[h][f] = mag(re, im) of
+// bin tid + 256 h, frame f.  Bin 512 (the alternating sum) is left to the caller.
+template <int FT, class Mag>
+__device__ __forceinline__ void dft1024_bins(const float2* tw, const float (*xw)[kDftN], int tid, float (&mg)[2][FT], Mag mag) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int k = tid + kDftThreads * h;
+    float re[FT], im[FT];
+#pragma unroll
+    for (int f = 0; f < FT; ++f) { re[f] = 0.f; im[f] = 0.f; }
+#pragma unroll 2
+    for (int n = 0; n < kDftN; n += 4) {
+      const float2 t0 = tw[(k * n) & (kDftN - 1)], t1 = tw[(k * (n + 1)) & (kDftN - 1)];
+      const float2 t2 = tw[(k * (n + 2)) & (kDftN - 1)], t3 = tw[(k * (n + 3)) & (kDftN - 1)];
+#pragma unroll
+      for (int f = 0; f < FT; ++f) {
+        const float4 x = *reinterpret_cast<const float4*>(&xw[f][n]);
+        re[f] = fmaf(x.x, t0.x, re[f]); im[f] = fmaf(x.x, t0.y, im[f]);
+        re[f] = fmaf(x.y, t1.x, re[f]); im[f] = fmaf(x.y, t1.y, im[f]);
+        re[f] = fmaf(x.z, t2.x, re[f]); im[f] = fmaf(x.z, t2.y, im[f]);
+        re[f] = fmaf(x.w, t3.x, re[f]); im[f] = fmaf(x.w, t3.y, im[f]);
+      }
+    }
+#pragma unroll
+    for (int f = 0; f < FT; ++f) mg[h][f] = mag(re[f], im[f]);
+  }
+}
+// Bin 512 of one frame: the alternating sum, accumulated pair by pair.
+__device__ __forceinline__ float dft1024_nyquist(const float* x) {
+  float s = 0.f;
+  for (int n = 0; n < kDftN; n += 2) s += x[n] - x[n + 1];
+  return s;
+}
+#endif
+
 // ----------------------------------------------------------------------------- conv1d
 enum ConvFlags : int {
   CONV_IN_MASK = 1,    // x[b,:,t] treated as 0 for t >= lengths[b]

@@ -83,11 +83,7 @@ spk_mel_kernel(const float* __restrict__ wav, const float* __restrict__ fb, cons
   const int tid = threadIdx.x;
   const long long f0 = it.f_off[0] + (long long)blockIdx.x * SPK_FT, fend = it.f_off[it.n];
   const float pre = __ldg(audio);
-  for (int n = tid; n < SPK_NFFT; n += 256) {
-    float s, c;
-    sincospif(2.f * (float)n / (float)SPK_NFFT, &s, &c);
-    tw[n] = make_float2(c, s);
-  }
+  dft1024_twiddles(tw, tid);
   for (int i = tid; i < SPK_FT * SPK_NFFT; i += 256) {
     const int fr = i / SPK_NFFT, n = i - fr * SPK_NFFT;
     const long long gf = f0 + fr;
@@ -107,35 +103,10 @@ spk_mel_kernel(const float* __restrict__ wav, const float* __restrict__ fb, cons
     xw[fr][n] = v;
   }
   __syncthreads();
-  // bins tid and tid + 256 for all SPK_FT frames: one twiddle load feeds 2 x SPK_FT FMAs; twiddle index k n mod 1024
   float mg[2][SPK_FT];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int k = tid + 256 * h;
-    float re[SPK_FT], im[SPK_FT];
-#pragma unroll
-    for (int f = 0; f < SPK_FT; ++f) { re[f] = 0.f; im[f] = 0.f; }
-#pragma unroll 2
-    for (int n = 0; n < SPK_NFFT; n += 4) {
-      const float2 t0 = tw[(k * n) & (SPK_NFFT - 1)], t1 = tw[(k * (n + 1)) & (SPK_NFFT - 1)];
-      const float2 t2 = tw[(k * (n + 2)) & (SPK_NFFT - 1)], t3 = tw[(k * (n + 3)) & (SPK_NFFT - 1)];
-#pragma unroll
-      for (int f = 0; f < SPK_FT; ++f) {
-        const float4 x = *reinterpret_cast<const float4*>(&xw[f][n]);
-        re[f] = fmaf(x.x, t0.x, re[f]); im[f] = fmaf(x.x, t0.y, im[f]);
-        re[f] = fmaf(x.y, t1.x, re[f]); im[f] = fmaf(x.y, t1.y, im[f]);
-        re[f] = fmaf(x.z, t2.x, re[f]); im[f] = fmaf(x.z, t2.y, im[f]);
-        re[f] = fmaf(x.w, t3.x, re[f]); im[f] = fmaf(x.w, t3.y, im[f]);
-      }
-    }
-#pragma unroll
-    for (int f = 0; f < SPK_FT; ++f) mg[h][f] = sqrtf(re[f] * re[f] + im[f] * im[f]);
-  }
-  float nyq = 0.f;   // bin 512: the alternating sum
-  if (tid < SPK_FT) {
-    for (int n = 0; n < SPK_NFFT; n += 2) nyq += xw[tid][n] - xw[tid][n + 1];
-    nyq = fabsf(nyq);
-  }
+  dft1024_bins<SPK_FT>(tw, xw, tid, mg, [](float re, float im) { return sqrtf(re * re + im * im); });
+  float nyq = 0.f;   // bin 512
+  if (tid < SPK_FT) nyq = fabsf(dft1024_nyquist(xw[tid]));
   __syncthreads();
   float* mag = &xw[0][0];
   constexpr int MLD = SPK_BINS + 3;
