@@ -225,6 +225,24 @@ int svcb_whisper_log_mel_ragged(const float* audio, const int32_t* n_samples_hos
 int svcb_linear_spec_ragged(const float* audio, const int64_t* sample_offsets_host, int32_t B, float* out, void* scratch,
                             size_t scratch_bytes, svcb_stream stream);
 
+/* ------------------------------------------------------------------ resampling of raw recordings (training data) */
+/* Replaces librosa.load(path, sr=sample_rate)'s resampling in prepare/preprocess_a.py:11 (resample_wave), as
+ * scipy.signal.resample_poly's polyphase FIR, for a ragged batch at one ratio up/down (sr_out / sr_in, reduced):
+ * item b is x[in_offsets_host[b] .. in_offsets_host[b+1]) (fp32 mono), n_b >= 1; B >= 1; up, down >= 1.
+ * taps: the fp64 filter firwin(2 half + 1, 1 / max(up, down), ('kaiser', 5.0)) * up, half = 10 max(up, down), with
+ * down - half % down leading zeros (n_taps in all); pre_remove = (half + leading zeros) / down.  Output j of item b is
+ * sum_k taps[k] xup[(j + pre_remove) down - k], xup[i] = x[i / up] where up divides i and 0 <= i / up < n_b, else 0,
+ * accumulated in fp64 and rounded once to fp32.  y: item b's ceil(n_b up / down) samples, following item b-1's from
+ * y[0].  Each item is bitwise that of a lone call.  The host does not call this for up == down == 1. */
+int svcb_resample_ragged(const float* x, const int64_t* in_offsets_host, int32_t B, int32_t up, int32_t down,
+                         const double* taps, int64_t n_taps, int64_t pre_remove, float* y, svcb_stream stream);
+/* Replaces prepare/preprocess_a.py:12-14 per item: y[offsets_host[b] .. offsets_host[b+1]) (fp32, n_b >= 1, B >= 1)
+ * -> out at the same offsets, int16: y / m1 * 0.6 / max(0.01, max|y / m1 * 0.6|) * 32767 * 0.6 in float32 steps,
+ * truncated toward zero, with m1 = max|y| of the item.  peak[b] = m1 (fp32, B entries); 0 marks a silent item, whose
+ * output is zeros (the reference divides by zero there). */
+int svcb_pcm16_normalise_ragged(const float* y, const int64_t* offsets_host, int32_t B, int16_t* out, float* peak,
+                                svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */

@@ -1,0 +1,126 @@
+"""Resampling of raw recordings for training on the H100 path: `librosa.load(path, sr)` and the int16 normalisation of
+the reference's `prepare/preprocess_a.py:resample_wave`, behind the C ABI (`svcb_resample_ragged`,
+`svcb_pcm16_normalise_ragged`, csrc/resample_api.cu).  No CPU fallback: a CUDA (sm_90a) device is required.
+
+The resampler is scipy.signal.resample_poly's polyphase Kaiser FIR (the project's resampling rule, as in
+`whisper_infer.load_audio`), evaluated with fp64 taps and accumulation and rounded once to float32, so the output is
+`resample_poly(x.astype(float64), up, down).astype(float32)`.  librosa 0.10.1 resamples with soxr instead: the lengths
+agree, ceil(n sr_out / sr_in), and the values differ slightly.  When the rates are equal nothing is resampled."""
+from __future__ import annotations
+
+import ctypes
+import math
+from typing import List, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from . import _lib
+
+_TAPS = {}   # (up, down, device) -> (device fp64 taps, pre_remove)
+
+
+def decode_wav(path: str) -> Tuple[int, np.ndarray]:
+    """(rate, float32 mono) of a .wav as librosa decodes it: integer PCM scaled to [-1, 1) (8-bit is unsigned around
+    128), float PCM as stored, channels averaged."""
+    from scipy.io import wavfile
+    rate, x = wavfile.read(path)
+    if x.dtype == np.uint8:     # 8-bit WAV is unsigned with the zero level at 128
+        x = (x.astype(np.float32) - 128.0) / 128.0
+    elif x.dtype.kind in "iu":
+        x = x.astype(np.float32) / float(np.iinfo(x.dtype).max + 1)
+    x = x.astype(np.float32)
+    if x.ndim > 1:
+        x = x.mean(axis=1)
+    return int(rate), x
+
+
+def load(path: str) -> Tuple[np.ndarray, int]:
+    """(float32 mono samples, rate) of a .wav; ValueError for a file without samples or with non-finite ones."""
+    rate, x = decode_wav(path)
+    if x.shape[0] == 0:
+        raise ValueError("no samples")
+    if not np.isfinite(x).all():
+        raise ValueError("non-finite samples")
+    return x, rate
+
+
+def ratio(sr_in: int, sr_out: int) -> Tuple[int, int]:
+    """(up, down): sr_out / sr_in reduced by their gcd."""
+    sr_in, sr_out = int(sr_in), int(sr_out)
+    if sr_in < 1 or sr_out < 1:
+        raise ValueError(f"sampling rates must be positive, got {sr_in} -> {sr_out}")
+    g = math.gcd(sr_in, sr_out)
+    return sr_out // g, sr_in // g
+
+
+def out_len(n: int, sr_in: int, sr_out: int) -> int:
+    """Samples after resampling n: ceil(n up / down), resample_poly's and librosa's length."""
+    up, down = ratio(sr_in, sr_out)
+    return -(-int(n) * up // down)
+
+
+def design(up: int, down: int) -> Tuple[np.ndarray, int]:
+    """resample_poly's filter for up/down in fp64, pre-padded so output j sits at input phase (j + pre_remove) down:
+    (taps, pre_remove)."""
+    from scipy.signal import firwin
+    half = 10 * max(up, down)
+    h = firwin(2 * half + 1, 1.0 / max(up, down), window=("kaiser", 5.0)) * up
+    pre = down - half % down
+    return np.concatenate([np.zeros(pre), h]), (half + pre) // down
+
+
+def _device_taps(up: int, down: int, dev: torch.device):
+    key = (up, down, str(dev))
+    if key not in _TAPS:
+        taps, rm = design(up, down)
+        _TAPS[key] = (torch.from_numpy(taps).to(dev), rm)
+    return _TAPS[key]
+
+
+def _offsets(lens: Sequence[int]):
+    o = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    return (ctypes.c_int64 * len(o))(*o.tolist()), o
+
+
+def _resample_device(audios: Sequence, sr_in: int, sr_out: int, dev: torch.device):
+    """The batch resampled on the device: (flat float32 device tensor, output offsets).  Equal rates copy the input."""
+    up, down = ratio(sr_in, sr_out)
+    clips = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1) for a in audios]
+    flat = torch.from_numpy(np.concatenate(clips)).to(dev)
+    if up == down:
+        return flat, _offsets([c.shape[0] for c in clips])
+    in_c, _ = _offsets([c.shape[0] for c in clips])
+    out_c, o = _offsets([-(-c.shape[0] * up // down) for c in clips])
+    taps, rm = _device_taps(up, down, dev)
+    y = torch.empty(max(int(o[-1]), 1), dtype=torch.float32, device=dev)
+    _lib.call("resample_ragged", flat.data_ptr(), in_c, len(clips), up, down, taps.data_ptr(), taps.numel(), rm,
+              y.data_ptr(), device=dev)
+    return y, (out_c, o)
+
+
+@torch.no_grad()
+def resample_batch(audios: Sequence, sr_in: int, sr_out: int, device="cuda") -> List[np.ndarray]:
+    """Clips at sr_in (ragged, each at least one sample) -> float32 clips at sr_out, one device call."""
+    dev = _lib.cuda_device(device)
+    if not audios:
+        return []
+    y, (_, o) = _resample_device(audios, sr_in, sr_out, dev)
+    host = y.cpu().numpy()
+    return [host[o[i]:o[i + 1]] for i in range(len(audios))]
+
+
+@torch.no_grad()
+def pcm16_batch(audios: Sequence, sr_in: int, sr_out: int, device="cuda") -> Tuple[List[np.ndarray], np.ndarray]:
+    """Clips at sr_in -> (int16 clips at sr_out as resample_wave writes them, float32 peaks max|y|), one resampling
+    and one normalising call; only the int16 samples and the peaks are copied back.  A peak of 0 marks a silent clip,
+    whose samples are zeros (the reference would divide by zero)."""
+    dev = _lib.cuda_device(device)
+    if not audios:
+        return [], np.zeros(0, np.float32)
+    y, (offs, o) = _resample_device(audios, sr_in, sr_out, dev)
+    out = torch.empty(max(int(o[-1]), 1), dtype=torch.int16, device=dev)
+    peak = torch.empty(len(audios), dtype=torch.float32, device=dev)
+    _lib.call("pcm16_normalise_ragged", y.data_ptr(), offs, len(audios), out.data_ptr(), peak.data_ptr(), device=dev)
+    host = out.cpu().numpy()
+    return [host[o[i]:o[i + 1]] for i in range(len(audios))], peak.cpu().numpy()

@@ -236,16 +236,9 @@ def load_audio(path: str, sr: int = SAMPLE_RATE) -> np.ndarray:
     scipy: int PCM -> [-1,1), channel mean, polyphase resampling.  Differences from the reference
     extractor: .wav only (librosa/audioread decode more containers), and `resample_poly` instead of
     librosa's soxr/kaiser resampler, so PPGs of non-16 kHz files differ slightly from the reference's."""
-    from scipy.io import wavfile
     from scipy.signal import resample_poly
-    rate, x = wavfile.read(path)
-    if x.dtype == np.uint8:     # 8-bit WAV is unsigned with the zero level at 128
-        x = (x.astype(np.float32) - 128.0) / 128.0
-    elif x.dtype.kind in "iu":
-        x = x.astype(np.float32) / float(np.iinfo(x.dtype).max + 1)
-    x = x.astype(np.float32)
-    if x.ndim > 1:
-        x = x.mean(axis=1)
+    from .resample import decode_wav
+    rate, x = decode_wav(path)
     if rate != sr:
         g = math.gcd(int(rate), sr)
         x = resample_poly(x, sr // g, int(rate) // g).astype(np.float32)
