@@ -8,6 +8,7 @@ import ctypes
 import os
 from ctypes import POINTER, c_char, c_char_p, c_float, c_int, c_int16, c_int32, c_int64, c_size_t, c_uint64, c_void_p
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -199,6 +200,33 @@ def call(name: str, *args, device=None) -> None:
     with torch.cuda.device(device):
         st = getattr(load(), "svcb_" + name)(*args, stream())
     check(st, "svcb_" + name)
+
+
+def offsets(lengths):
+    """The prefix sums [0, l0, l0 + l1, ...] as a ctypes int64 array: a ragged batch's `*_offsets_host` argument."""
+    o = [0]
+    for n in lengths:
+        o.append(o[-1] + int(n))
+    return (c_int64 * len(o))(*o)
+
+
+def ragged(clips, device):
+    """1-D clips (numpy arrays, tensors or lists) -> (their float32 concatenation on `device`, offsets).  Clips already
+    on the device are joined by one kernel.  Host clips are copied straight into their slices of the device buffer,
+    since joining them on the host first is a few times slower."""
+    xs = [(c.float() if torch.is_tensor(c) else torch.as_tensor(np.asarray(c, np.float32))).reshape(-1) for c in clips]
+    offs = offsets(x.numel() for x in xs)
+    if xs and all(x.is_cuda for x in xs):
+        return torch.cat(xs).to(device), offs
+    flat = torch.empty(offs[-1], dtype=torch.float32, device=device)
+    for b, x in enumerate(xs):
+        flat[offs[b]:offs[b + 1]].copy_(x)
+    return flat, offs
+
+
+def split(x, offs):
+    """x cut at the offsets: one piece per item."""
+    return [x[offs[b]:offs[b + 1]] for b in range(len(offs) - 1)]
 
 
 class Handle:

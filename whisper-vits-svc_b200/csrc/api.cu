@@ -663,6 +663,25 @@ int check_workspace(const void* ws, size_t ws_bytes, size_t need, const char* wh
   return SVCB_E_WORKSPACE;
 }
 
+int check_ragged(const char* who, const int64_t* offsets_host, int32_t B, int32_t min_items, int64_t min_len,
+                 const char* unit, const char* why) {
+  if (B < min_items) {
+    set_error(std::string(who) + ": B = " + std::to_string(B) + (min_items > 0 ? "; need at least one item" : " is negative"));
+    return SVCB_E_BAD_SHAPE;
+  }
+  if (offsets_host[0] < 0) { set_error(std::string(who) + ": negative first offset"); return SVCB_E_BAD_SHAPE; }
+  for (int b = 0; b < B; ++b) {
+    const int64_t n = offsets_host[b + 1] - offsets_host[b];
+    if (n < min_len) {
+      set_error(std::string(who) + ": item " + std::to_string(b) + " has " + std::to_string(n) + " " + unit +
+                "; need at least " + std::to_string(min_len) + (n < 0 ? " (the offsets decrease)" : "") +
+                (why ? std::string("; ") + why : std::string()));
+      return SVCB_E_BAD_SHAPE;
+    }
+  }
+  return SVCB_OK;
+}
+
 int BlobTensors::read(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table, int32_t n) {
   const char* blob = static_cast<const char*>(dev_blob);
   for (int i = 0; i < n; ++i) {

@@ -115,6 +115,43 @@ int device_sm_count();   // of the current device (cached per device); 0 on erro
     if (_s != SVCB_OK) return _s; \
   } while (0)
 
+// Ragged batches of flat buffers with int64 host offsets (spec, resample, pcm16, VAD, speaker mel / embed).  A pass of
+// up to G items rides in the kernel parameters: item b reads [in[b], in[b+1]) and writes [out[b], out[b+1]); output
+// offsets count from the batch's first item.
+template <int G>
+struct ItemPass {
+  int n;
+  long long in[G + 1];
+  long long out[G + 1];
+};
+// SVCB_E_BAD_SHAPE, with an error naming `who`, unless B >= min_items, offsets[0] >= 0 and every item is at least
+// min_len `unit` long; `why`, when given, ends the message.
+int check_ragged(const char* who, const int64_t* offsets_host, int32_t B, int32_t min_items, int64_t min_len,
+                 const char* unit, const char* why);
+// Runs body(pass, g0) on each pass of up to G items (g0 = its first item), with out[i + 1] = out[i] + out_len(item i's
+// length) continued from the pass before.  Returns the first status that is not SVCB_OK.
+template <int G, class OutLen, class Body>
+int for_each_pass(const int64_t* offsets_host, int32_t B, OutLen out_len, Body body) {
+  long long o = 0;
+  for (int g0 = 0; g0 < B; g0 += G) {
+    ItemPass<G> p;
+    p.n = std::min(G, B - g0);
+    p.out[0] = o;
+    for (int i = 0; i <= p.n; ++i) p.in[i] = offsets_host[g0 + i];
+    for (int i = 0; i < p.n; ++i) p.out[i + 1] = p.out[i] + out_len(p.in[i + 1] - p.in[i]);
+    o = p.out[p.n];
+    SVCB_TRY(body(static_cast<const ItemPass<G>&>(p), g0));
+  }
+  return SVCB_OK;
+}
+#ifdef __CUDACC__
+// The item of a pass's offsets (in or out) that holds position x < off[n]: the first b' >= b with off[b' + 1] > x.
+__device__ __forceinline__ int item_of(const long long* off, long long x, int b = 0) {
+  while (off[b + 1] <= x) ++b;
+  return b;
+}
+#endif
+
 // sin() for the Snake activations of the tensor-core / fused paths: two-constant Cody-Waite reduction
 // to [-pi, pi] followed by the hardware approximation.  `__sinf` alone multiplies by 1/2pi in fp32 first,
 // so its absolute error grows like |x| * 2^-24: trained BigVGAN log-alphas reach e^alpha ~ 10-50, i.e.

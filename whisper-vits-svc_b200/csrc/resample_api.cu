@@ -7,7 +7,7 @@
 //   pcm16_peak   per-item max|y| (exact: a block max, then atomicMax on the non-negative float's bit pattern)
 //   pcm16        the reference's float32 steps y / m1 * 0.6 / m2 * 32767 * 0.6, truncated to int16
 //
-// Ragged batches: an item table per pass of up to RS_GROUP items rides in the kernel parameters, and a CTA's tile of
+// Ragged batches: each pass of up to RS_GROUP items rides in the kernel parameters (ItemPass), and a CTA's tile of
 // consecutive outputs may straddle items.  An output depends on its own item only and comes from the same
 // instructions in any batch, so a ragged batch is bitwise equal to each item run alone.
 #include <algorithm>
@@ -23,12 +23,6 @@ constexpr int RS_GROUP = 128;                                 // items per pass
 constexpr long long RS_X_CAP_MAX = 32768;                     // staged input floats per CTA, at most
 constexpr size_t RS_SMEM_MAX = 200 * 1024;                    // dynamic shared memory: taps (if they fit) + input
 constexpr int PK_THREADS = 256, PK_TILE = PK_THREADS * 16;    // normaliser: elements per CTA
-
-struct RsItems {   // one pass: inputs x[in_off[b], in_off[b+1]) -> outputs y[out_off[b], out_off[b+1])
-  int n;
-  long long in_off[RS_GROUP + 1];
-  long long out_off[RS_GROUP + 1];
-};
 
 struct RsFilter {
   const double* taps;   // pre-padded filter, n_taps long
@@ -48,25 +42,24 @@ __device__ __forceinline__ void rs_span(long long jl, long long n, const RsFilte
 
 // grid ceil(outputs / RS_TILE), RS_THREADS threads, dynamic shared memory [taps (doubles) if taps_in_smem][x_cap floats].
 __global__ void __launch_bounds__(RS_THREADS)
-resample_kernel(const float* __restrict__ x, float* __restrict__ y, RsItems it, RsFilter f) {
+resample_kernel(const float* __restrict__ x, float* __restrict__ y, ItemPass<RS_GROUP> it, RsFilter f) {
   extern __shared__ __align__(16) unsigned char rs_smem[];
   double* hs = reinterpret_cast<double*>(rs_smem);
   float* xs = reinterpret_cast<float*>(rs_smem + (f.taps_in_smem ? f.n_taps * (long long)sizeof(double) : 0));
   __shared__ long long s_lo, s_hi;
   __shared__ int s_b0;
   const int tid = threadIdx.x;
-  const long long j0 = it.out_off[0] + (long long)blockIdx.x * RS_TILE;
-  const long long jend = min(j0 + RS_TILE, it.out_off[it.n]);
+  const long long j0 = it.out[0] + (long long)blockIdx.x * RS_TILE;
+  const long long jend = min(j0 + RS_TILE, it.out[it.n]);
   if (tid == 0) {   // the tile's items and the input span its outputs read
     long long t, lo, hi;
-    int b = 0;
-    while (it.out_off[b + 1] <= j0) ++b;
+    int b = item_of(it.out, j0);
     s_b0 = b;
-    rs_span(j0 - it.out_off[b], it.in_off[b + 1] - it.in_off[b], f, t, lo, hi);
-    s_lo = it.in_off[b] + lo;
-    while (it.out_off[b + 1] < jend) ++b;
-    rs_span(jend - 1 - it.out_off[b], it.in_off[b + 1] - it.in_off[b], f, t, lo, hi);
-    s_hi = it.in_off[b] + hi + 1;
+    rs_span(j0 - it.out[b], it.in[b + 1] - it.in[b], f, t, lo, hi);
+    s_lo = it.in[b] + lo;
+    b = item_of(it.out, jend - 1, b);
+    rs_span(jend - 1 - it.out[b], it.in[b + 1] - it.in[b], f, t, lo, hi);
+    s_hi = it.in[b] + hi + 1;
   }
   __syncthreads();
   const long long x_lo = s_lo, span = s_hi - s_lo;
@@ -83,11 +76,11 @@ resample_kernel(const float* __restrict__ x, float* __restrict__ y, RsItems it, 
   for (int r = 0; r < RS_PER_THREAD; ++r) {
     const long long j = j0 + tid + (long long)r * RS_THREADS;
     if (j >= jend) break;
-    while (it.out_off[b + 1] <= j) ++b;
+    b = item_of(it.out, j, b);
     long long t, lo, hi;
-    rs_span(j - it.out_off[b], it.in_off[b + 1] - it.in_off[b], f, t, lo, hi);
+    rs_span(j - it.out[b], it.in[b + 1] - it.in[b], f, t, lo, hi);
     const int cnt = (int)max(hi - lo + 1, 0ll);
-    const float* xq = xp + (it.in_off[b] - (staged ? x_lo : 0ll) + hi);   // input hi, read backwards
+    const float* xq = xp + (it.in[b] - (staged ? x_lo : 0ll) + hi);   // input hi, read backwards
     const double* hq = hp + (t - hi * f.up);                             // its tap, read forwards by `up`
     double acc = 0.0;
     for (int m = 0; m < cnt; ++m) acc = fma(hq[(long long)m * f.up], (double)xq[-m], acc);
@@ -95,28 +88,21 @@ resample_kernel(const float* __restrict__ x, float* __restrict__ y, RsItems it, 
   }
 }
 
-struct PkItems {   // one pass: items [off[b], off[b+1]) of y and out; peak points at the pass's first item
-  int n;
-  long long off[RS_GROUP + 1];
-};
-
+// The normaliser's items are [in[b], in[b+1]) of both y and out; peak points at the pass's first item.
 // grid ceil(elements / PK_TILE): each CTA reduces max|y| of every item its tile touches, one block reduction each.
 __global__ void __launch_bounds__(PK_THREADS)
-pcm16_peak_kernel(const float* __restrict__ y, unsigned int* __restrict__ peak_bits, PkItems it) {
+pcm16_peak_kernel(const float* __restrict__ y, unsigned int* __restrict__ peak_bits, ItemPass<RS_GROUP> it) {
   __shared__ int s_b0, s_b1;
   __shared__ float red[PK_THREADS / 32];
   const int tid = threadIdx.x;
-  const long long e0 = it.off[0] + (long long)blockIdx.x * PK_TILE, e1 = min(e0 + PK_TILE, it.off[it.n]);
+  const long long e0 = it.in[0] + (long long)blockIdx.x * PK_TILE, e1 = min(e0 + PK_TILE, it.in[it.n]);
   if (tid == 0) {
-    int b = 0;
-    while (it.off[b + 1] <= e0) ++b;
-    s_b0 = b;
-    while (it.off[b + 1] < e1) ++b;
-    s_b1 = b;
+    s_b0 = item_of(it.in, e0);
+    s_b1 = item_of(it.in, e1 - 1, s_b0);
   }
   __syncthreads();
   for (int b = s_b0; b <= s_b1; ++b) {
-    const long long lo = max(e0, it.off[b]), hi = min(e1, it.off[b + 1]);
+    const long long lo = max(e0, it.in[b]), hi = min(e1, it.in[b + 1]);
     float m = 0.f;
     for (long long e = lo + tid; e < hi; e += PK_THREADS) m = fmaxf(m, fabsf(__ldg(y + e)));
 #pragma unroll
@@ -136,19 +122,15 @@ pcm16_peak_kernel(const float* __restrict__ y, unsigned int* __restrict__ peak_b
 // max|y / m1| is m1 / m1 = 1 exactly (division is monotone), so m2 = max(0.01, 1 * 0.6) = 0.6f.  Silent items
 // (m1 = 0) give zeros; the host skips them.
 __global__ void __launch_bounds__(PK_THREADS)
-pcm16_kernel(const float* __restrict__ y, const float* __restrict__ peak, int16_t* __restrict__ out, PkItems it) {
+pcm16_kernel(const float* __restrict__ y, const float* __restrict__ peak, int16_t* __restrict__ out, ItemPass<RS_GROUP> it) {
   __shared__ int s_b0;
   const int tid = threadIdx.x;
-  const long long e0 = it.off[0] + (long long)blockIdx.x * PK_TILE, e1 = min(e0 + PK_TILE, it.off[it.n]);
-  if (tid == 0) {
-    int b = 0;
-    while (it.off[b + 1] <= e0) ++b;
-    s_b0 = b;
-  }
+  const long long e0 = it.in[0] + (long long)blockIdx.x * PK_TILE, e1 = min(e0 + PK_TILE, it.in[it.n]);
+  if (tid == 0) s_b0 = item_of(it.in, e0);
   __syncthreads();
   int b = s_b0;
   for (long long e = e0 + tid; e < e1; e += PK_THREADS) {
-    while (it.off[b + 1] <= e) ++b;
+    b = item_of(it.in, e, b);
     const float m1 = peak[b];
     int16_t v16 = 0;
     if (m1 > 0.f) {
@@ -159,19 +141,6 @@ pcm16_kernel(const float* __restrict__ y, const float* __restrict__ peak, int16_
     }
     out[e] = v16;
   }
-}
-
-// Host checks shared by both entry points: B >= 1, offsets[0] >= 0 and every item of at least one sample.
-static bool check_items(const char* who, const int64_t* offsets, int32_t B) {
-  if (B < 1) { set_error(std::string(who) + ": B = " + std::to_string(B) + "; need at least one item"); return false; }
-  if (offsets[0] < 0) { set_error(std::string(who) + ": negative first offset"); return false; }
-  for (int b = 0; b < B; ++b)
-    if (offsets[b + 1] - offsets[b] < 1) {
-      set_error(std::string(who) + ": item " + std::to_string(b) + " has " + std::to_string(offsets[b + 1] - offsets[b]) +
-                " samples; need at least 1 (offsets must increase)");
-      return false;
-    }
-  return true;
 }
 
 }  // namespace svcb
@@ -190,7 +159,7 @@ int svcb_resample_ragged(const float* x, const int64_t* in_offsets_host, int32_t
               std::to_string(pre_remove));
     return SVCB_E_BAD_SHAPE;
   }
-  if (!check_items(who, in_offsets_host, B)) return SVCB_E_BAD_SHAPE;
+  SVCB_TRY(check_ragged(who, in_offsets_host, B, 1, 1, "samples", nullptr));
   RsFilter f;
   f.taps = taps; f.n_taps = n_taps; f.rm = pre_remove; f.up = up; f.down = down;
   // worst input span of a tile: T down / up for its outputs plus a filter's reach at each end (DESIGN.md §5)
@@ -200,36 +169,26 @@ int svcb_resample_ragged(const float* x, const int64_t* in_offsets_host, int32_t
   SVCB_CUDA_CHECK(cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const double taps_per_out = (double)((n_taps + up - 1) / up);
-  long long o = 0;
-  for (int g0 = 0; g0 < B; g0 += RS_GROUP) {
-    RsItems it;
-    it.n = std::min(RS_GROUP, B - g0);
-    it.out_off[0] = o;
-    for (int i = 0; i <= it.n; ++i) it.in_off[i] = in_offsets_host[g0 + i];
-    for (int i = 0; i < it.n; ++i)
-      it.out_off[i + 1] = it.out_off[i] + ((it.in_off[i + 1] - it.in_off[i]) * up + down - 1) / down;   // ceil(n up / down)
-    const long long n_out = it.out_off[it.n] - o, n_in = it.in_off[it.n] - it.in_off[0];
-    o = it.out_off[it.n];
+  const auto out_len = [=](long long n) { return (n * up + down - 1) / down; };   // ceil(n up / down)
+  return for_each_pass<RS_GROUP>(in_offsets_host, B, out_len, [&](const ItemPass<RS_GROUP>& it, int) -> int {
+    const long long n_out = it.out[it.n] - it.out[0], n_in = it.in[it.n] - it.in[0];
     KernelScope ks("resample", s, 2.0 * taps_per_out * (double)n_out,
                    4.0 * (double)(n_in + n_out) + 8.0 * (double)n_taps);
     resample_kernel<<<(unsigned)((n_out + RS_TILE - 1) / RS_TILE), RS_THREADS, smem, s>>>(x, y, it, f);
     SVCB_LAUNCH_CHECK("resample");
-  }
-  return SVCB_OK;
+    return SVCB_OK;
+  });
 }
 
 int svcb_pcm16_normalise_ragged(const float* y, const int64_t* offsets_host, int32_t B, int16_t* out, float* peak,
                                 svcb_stream stream) {
   static const char* who = "svcb_pcm16_normalise_ragged";
   if (!y || !out || !peak || !offsets_host) { set_error(std::string(who) + ": null pointer"); return SVCB_E_BAD_SHAPE; }
-  if (!check_items(who, offsets_host, B)) return SVCB_E_BAD_SHAPE;
+  SVCB_TRY(check_ragged(who, offsets_host, B, 1, 1, "samples", nullptr));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   SVCB_CUDA_CHECK(cudaMemsetAsync(peak, 0, sizeof(float) * (size_t)B, s));
-  for (int g0 = 0; g0 < B; g0 += RS_GROUP) {
-    PkItems it;
-    it.n = std::min(RS_GROUP, B - g0);
-    for (int i = 0; i <= it.n; ++i) it.off[i] = offsets_host[g0 + i];
-    const long long n = it.off[it.n] - it.off[0];
+  return for_each_pass<RS_GROUP>(offsets_host, B, [](long long n) { return n; }, [&](const ItemPass<RS_GROUP>& it, int g0) -> int {
+    const long long n = it.in[it.n] - it.in[0];
     const unsigned grid = (unsigned)((n + PK_TILE - 1) / PK_TILE);
     {
       KernelScope ks("pcm16_peak", s, 0.0, 4.0 * (double)n);
@@ -239,8 +198,8 @@ int svcb_pcm16_normalise_ragged(const float* y, const int64_t* offsets_host, int
     KernelScope ks("pcm16", s, 0.0, 6.0 * (double)n);
     pcm16_kernel<<<grid, PK_THREADS, 0, s>>>(y, peak + g0, out, it);
     SVCB_LAUNCH_CHECK("pcm16");
-  }
-  return SVCB_OK;
+    return SVCB_OK;
+  });
 }
 
 }  // extern "C"

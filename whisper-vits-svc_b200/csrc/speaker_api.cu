@@ -48,15 +48,8 @@ constexpr uint32_t REC_W_BYTES = 2u * (SPK_H / 8) * SPK_NC * 16;   // W_hh hi + 
 constexpr uint32_t REC_A_BYTES = 128u * 64 * 2;                    // one 128-row k-tile of the h image
 constexpr size_t REC_SMEM = REC_W_BYTES + REC_STAGES * REC_A_BYTES + 2 * 64 * REC_LD * 4 + SPK_MAXMP * SPK_UPC * 4;
 
-struct SpkMelItems {   // one pass: n items, samples [s_off[b], s_off[b+1]) -> mel rows [f_off[b], f_off[b+1])
-  int n;
-  long long s_off[SPK_GROUP + 1];
-  long long f_off[SPK_GROUP + 1];
-};
-struct SpkItems {      // one pass: n items, mel rows [f_off[b], f_off[b+1])
-  int n;
-  long long f_off[SPK_GROUP + 1];
-};
+// A pass of svcb_speaker_mel takes samples in and writes mel rows out; one of svcb_speaker_embed reads mel rows in.
+using SpkPass = ItemPass<SPK_GROUP>;
 
 // element offset of (m, k) in a gemm_tc tile image with KT k-tiles per 128-row tile (csrc/whisper_gemm.cu)
 __host__ __device__ inline size_t spk_img_off(size_t m, int k, int KT) {
@@ -77,11 +70,11 @@ __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence
 // audio = {preemphasis, ref_level_db, min_level_db, max_norm}
 __global__ void __launch_bounds__(256)
 spk_mel_kernel(const float* __restrict__ wav, const float* __restrict__ fb, const float* __restrict__ audio,
-               float* __restrict__ out, SpkMelItems it) {
+               float* __restrict__ out, SpkPass it) {
   __shared__ float2 tw[SPK_NFFT];
   __shared__ __align__(16) float xw[SPK_FT][SPK_NFFT];   // windowed frames, then the magnitudes [SPK_FT][SPK_BINS + 3]
   const int tid = threadIdx.x;
-  const long long f0 = it.f_off[0] + (long long)blockIdx.x * SPK_FT, fend = it.f_off[it.n];
+  const long long f0 = it.out[0] + (long long)blockIdx.x * SPK_FT, fend = it.out[it.n];
   const float pre = __ldg(audio);
   dft1024_twiddles(tw, tid);
   for (int i = tid; i < SPK_FT * SPK_NFFT; i += 256) {
@@ -89,11 +82,10 @@ spk_mel_kernel(const float* __restrict__ wav, const float* __restrict__ fb, cons
     const long long gf = f0 + fr;
     float v = 0.f;
     if (gf < fend) {
-      int b = 0;
-      while (it.f_off[b + 1] <= gf) ++b;
-      const long long N = it.s_off[b + 1] - it.s_off[b];
-      const float* x = wav + it.s_off[b];
-      long long s = (gf - it.f_off[b]) * SPK_HOP + n - SPK_NFFT / 2;   // center=True, reflect padding
+      const int b = item_of(it.out, gf);
+      const long long N = it.in[b + 1] - it.in[b];
+      const float* x = wav + it.in[b];
+      long long s = (gf - it.out[b]) * SPK_HOP + n - SPK_NFFT / 2;   // center=True, reflect padding
       if (s < 0) s = -s;
       if (s >= N) s = 2 * (N - 1) - s;
       // lfilter([1, -pre], [1]) with x[-1] = 0, applied before the padding
@@ -133,7 +125,7 @@ spk_mel_kernel(const float* __restrict__ wav, const float* __restrict__ fb, cons
 // x[m][0..128) for m = t * Mp + r: the mel frame of window r at step t (zero past the window's end, for k >= 80 and
 // for pad rows r >= 10 n)
 __global__ void __launch_bounds__(256)
-spk_gather0_kernel(const float* __restrict__ mel, float* __restrict__ x, SpkItems it, int Mp, size_t R) {
+spk_gather0_kernel(const float* __restrict__ mel, float* __restrict__ x, SpkPass it, int Mp, size_t R) {
   const size_t idx = (size_t)blockIdx.x * 256 + threadIdx.x;
   if (idx >= R * (SPK_K0 / 4)) return;
   const size_t m = idx / (SPK_K0 / 4);
@@ -142,8 +134,8 @@ spk_gather0_kernel(const float* __restrict__ mel, float* __restrict__ x, SpkItem
   float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
   if (r < SPK_NWIN * it.n && q < SPK_MELS / 4) {
     const int b = r / SPK_NWIN, w = r - b * SPK_NWIN;
-    const long long T = it.f_off[b + 1] - it.f_off[b], L = T < SPK_WIN ? T : SPK_WIN;
-    if (t < L) v = __ldg(reinterpret_cast<const float4*>(mel + (it.f_off[b] + spk_win_offset(T - L, w) + t) * SPK_MELS) + q);
+    const long long T = it.in[b + 1] - it.in[b], L = T < SPK_WIN ? T : SPK_WIN;
+    if (t < L) v = __ldg(reinterpret_cast<const float4*>(mel + (it.in[b] + spk_win_offset(T - L, w) + t) * SPK_MELS) + q);
   }
   reinterpret_cast<float4*>(x + m * SPK_K0)[q] = v;
 }
@@ -267,7 +259,7 @@ spk_lstm_rec_kernel(const __nv_bfloat16* __restrict__ whh, const float* __restri
 // The last layer's h at each window's own last step: row r of a [Mp][2304] h image (pad rows: step Lw - 1), so the last
 // projection runs over Mp rows instead of Lw x Mp.  Thread = one 16-byte octet.
 __global__ void __launch_bounds__(256)
-spk_gather_last_kernel(const __nv_bfloat16* __restrict__ himg, __nv_bfloat16* __restrict__ last, SpkItems it, int Mp, int Lw) {
+spk_gather_last_kernel(const __nv_bfloat16* __restrict__ himg, __nv_bfloat16* __restrict__ last, SpkPass it, int Mp, int Lw) {
   constexpr int KT = SPK_HK / 64, NO = SPK_HK / 8;
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= Mp * NO) return;
@@ -275,7 +267,7 @@ spk_gather_last_kernel(const __nv_bfloat16* __restrict__ himg, __nv_bfloat16* __
   long long t = Lw - 1;
   if (r < SPK_NWIN * it.n) {
     const int b = r / SPK_NWIN;
-    const long long T = it.f_off[b + 1] - it.f_off[b];
+    const long long T = it.in[b + 1] - it.in[b];
     t = (T < SPK_WIN ? T : SPK_WIN) - 1;
   }
   *reinterpret_cast<uint4*>(last + spk_img_off(r, 8 * o, KT)) =
@@ -285,7 +277,7 @@ spk_gather_last_kernel(const __nv_bfloat16* __restrict__ himg, __nv_bfloat16* __
 // one CTA per item, thread = embedding dim: F.normalize(d[:, -1]) per window (lstm.py:69-74), then the mean of the 10.
 // proj: the last layer's projection of the gathered last steps, [Mp][256]
 __global__ void __launch_bounds__(256)
-spk_finish_kernel(const float* __restrict__ proj, float* __restrict__ out, float* __restrict__ wout, SpkItems it) {
+spk_finish_kernel(const float* __restrict__ proj, float* __restrict__ out, float* __restrict__ wout, SpkPass it) {
   __shared__ float red[8];
   const int b = blockIdx.x, j = threadIdx.x, lane = j & 31, warp = j >> 5;
   float acc = 0.f;
@@ -390,49 +382,30 @@ size_t svcb_speaker_workspace_bytes(const svcb_speaker* sp, int32_t B, int64_t t
 int svcb_speaker_mel(const svcb_speaker* sp, const float* wav, const int64_t* sample_offsets_host, int32_t B, float* mel_out,
                      void* ws, size_t ws_bytes, svcb_stream stream) {
   (void)ws; (void)ws_bytes;
-  if (!sp || !wav || !mel_out || !sample_offsets_host || B < 0) { set_error("svcb_speaker_mel: bad argument"); return SVCB_E_BAD_SHAPE; }
-  for (int b = 0; b < B; ++b)
-    if (sample_offsets_host[b] < 0 || sample_offsets_host[b + 1] - sample_offsets_host[b] <= SPK_NFFT / 2) {
-      set_error("svcb_speaker_mel: item " + std::to_string(b) + " has " +
-                std::to_string(sample_offsets_host[b + 1] - sample_offsets_host[b]) +
-                " samples; the reflect-padded STFT needs more than 512");
-      return SVCB_E_BAD_SHAPE;
-    }
+  if (!sp || !wav || !mel_out || !sample_offsets_host) { set_error("svcb_speaker_mel: bad argument"); return SVCB_E_BAD_SHAPE; }
+  SVCB_TRY(check_ragged("svcb_speaker_mel", sample_offsets_host, B, 0, SPK_NFFT / 2 + 1, "samples",
+                        "the reflect-padded STFT pads 512 at each end"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  long long frame = 0;
-  for (int g0 = 0; g0 < B; g0 += SPK_GROUP) {
-    SpkMelItems it;
-    it.n = std::min(SPK_GROUP, B - g0);
-    it.f_off[0] = frame;
-    for (int i = 0; i <= it.n; ++i) it.s_off[i] = sample_offsets_host[g0 + i];
-    for (int i = 0; i < it.n; ++i) it.f_off[i + 1] = it.f_off[i] + svcb_speaker_frames(it.s_off[i + 1] - it.s_off[i]);
-    const long long F = it.f_off[it.n] - it.f_off[0];
-    frame = it.f_off[it.n];
+  return for_each_pass<SPK_GROUP>(sample_offsets_host, B, svcb_speaker_frames, [&](const SpkPass& it, int) -> int {
+    const long long F = it.out[it.n] - it.out[0];
     KernelScope ks("spk_mel", s, (double)F * (4.0 * SPK_NFFT * SPK_BINS + 2.0 * SPK_BINS * SPK_MELS),
-                   4.0 * ((double)(it.s_off[it.n] - it.s_off[0]) + (double)SPK_MELS * F));
+                   4.0 * ((double)(it.in[it.n] - it.in[0]) + (double)SPK_MELS * F));
     spk_mel_kernel<<<(unsigned)((F + SPK_FT - 1) / SPK_FT), 256, 0, s>>>(wav, sp->fb, sp->audio, mel_out, it);
     SVCB_LAUNCH_CHECK("spk_mel");
-  }
-  return SVCB_OK;
+    return SVCB_OK;
+  });
 }
 
 int svcb_speaker_embed(const svcb_speaker* sp, const float* mel, const int64_t* frame_offsets_host, int32_t B, float* out,
                        float* window_out, void* ws, size_t ws_bytes, svcb_stream stream) {
-  if (!sp || !mel || !out || !frame_offsets_host || B < 0) { set_error("svcb_speaker_embed: bad argument"); return SVCB_E_BAD_SHAPE; }
+  if (!sp || !mel || !out || !frame_offsets_host) { set_error("svcb_speaker_embed: bad argument"); return SVCB_E_BAD_SHAPE; }
   if ((uintptr_t)mel & 15) { set_error("svcb_speaker_embed: mel must be 16-byte aligned"); return SVCB_E_BAD_ALIGN; }
-  for (int b = 0; b < B; ++b)
-    if (frame_offsets_host[b] < 0 || frame_offsets_host[b + 1] <= frame_offsets_host[b]) {
-      set_error("svcb_speaker_embed: item " + std::to_string(b) + " has no mel frames");
-      return SVCB_E_BAD_SHAPE;
-    }
+  SVCB_TRY(check_ragged("svcb_speaker_embed", frame_offsets_host, B, 0, 1, "mel frames", nullptr));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* base = static_cast<char*>(ws);
-  for (int g0 = 0; g0 < B; g0 += SPK_GROUP) {
-    SpkItems it;
-    it.n = std::min(SPK_GROUP, B - g0);
+  return for_each_pass<SPK_GROUP>(frame_offsets_host, B, [](long long n) { return n; }, [&](const SpkPass& it, int g0) -> int {
     int Lw = 0;
-    for (int i = 0; i <= it.n; ++i) it.f_off[i] = frame_offsets_host[g0 + i];
-    for (int i = 0; i < it.n; ++i) Lw = std::max<int>(Lw, (int)std::min<long long>(SPK_WIN, it.f_off[i + 1] - it.f_off[i]));
+    for (int i = 0; i < it.n; ++i) Lw = std::max<int>(Lw, (int)std::min<long long>(SPK_WIN, it.in[i + 1] - it.in[i]));
     const int Mp = spk_mp(it.n), rows = SPK_NWIN * it.n;
     const size_t R = (size_t)Lw * Mp;
     const SpkLayout L = spk_layout(R, Mp);
@@ -489,8 +462,8 @@ int svcb_speaker_embed(const svcb_speaker* sp, const float* mel, const int64_t* 
                                              it);
       SVCB_LAUNCH_CHECK("spk_finish");
     }
-  }
-  return SVCB_OK;
+    return SVCB_OK;
+  });
 }
 
 }  // extern "C"

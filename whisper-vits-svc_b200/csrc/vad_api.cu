@@ -31,12 +31,6 @@ constexpr int VAD_BUF = 128;      // floats per window of an encoder buffer (the
 constexpr size_t VAD_FRONT_SMEM = sizeof(float) * (VAD_WPC * VAD_PW + VAD_WPC * VAD_FEAT * VAD_NF + 3 * VAD_WPC * VAD_BUF + VAD_WPC * 8);
 constexpr size_t VAD_REC_SMEM = sizeof(float) * (3 * VAD_H * VAD_G + 2 * VAD_H + VAD_G);
 
-struct VadItems {   // one pass: n items, samples [s_off[b], s_off[b+1]) -> windows [w_off[b], w_off[b+1])
-  int n;
-  long long s_off[VAD_GROUP + 1];
-  long long w_off[VAD_GROUP + 1];
-};
-
 struct VadWeights {
   const float* basis4;   // [2 (re, im)][64 k-quads][128 bins][4]: bins 0 .. 127
   const float* nyq;      // [2][256]: bin 128
@@ -92,16 +86,11 @@ __device__ void vad_dw(const float* x, int xws, int C, const float* __restrict__
   }
 }
 
-__device__ __forceinline__ int vad_item_of(const VadItems& it, long long gw) {
-  int b = 0;
-  while (it.w_off[b + 1] <= gw) ++b;
-  return b;
-}
-
 // ----------------------------------------------------------------------------------------------------- front end
-// grid ceil(windows of the pass / VAD_WPC), 256 threads
+// grid ceil(windows of the pass / VAD_WPC), 256 threads; it: samples in, windows out
 __global__ void __launch_bounds__(256)
-vad_front_kernel(const float* __restrict__ wav, VadWeights P, VadItems it, float* __restrict__ G, float* __restrict__ feat_out) {
+vad_front_kernel(const float* __restrict__ wav, VadWeights P, ItemPass<VAD_GROUP> it, float* __restrict__ G,
+                 float* __restrict__ feat_out) {
   extern __shared__ __align__(16) float sm[];
   float* xw = sm;                                       // [VAD_WPC][704]
   float* fe = xw + VAD_WPC * VAD_PW;                    // [VAD_WPC][258][8]: magnitude, then the normalised log
@@ -110,15 +99,15 @@ vad_front_kernel(const float* __restrict__ wav, VadWeights P, VadItems it, float
   float* bR = bB + VAD_WPC * VAD_BUF;
   float* fm = bR + VAD_WPC * VAD_BUF;                   // [VAD_WPC][8] bin means of each frame
   const int tid = threadIdx.x;
-  const long long w_first = it.w_off[0] + (long long)blockIdx.x * VAD_WPC, w_end = it.w_off[it.n];
+  const long long w_first = it.out[0] + (long long)blockIdx.x * VAD_WPC, w_end = it.out[it.n];
 
   for (int i = tid; i < VAD_WPC * VAD_PW; i += 256) {
     const int w = i / VAD_PW, p = i - w * VAD_PW;
     const long long gw = w_first + w;
     float v = 0.f;
     if (gw < w_end) {
-      const int b = vad_item_of(it, gw);
-      const long long s0 = it.s_off[b] + (gw - it.w_off[b]) * VAD_WIN, n = it.s_off[b + 1] - s0;   // n >= 1
+      const int b = item_of(it.out, gw);
+      const long long s0 = it.in[b] + (gw - it.out[b]) * VAD_WIN, n = it.in[b + 1] - s0;   // n >= 1
       int s = p - VAD_PAD;                              // reflect inside the zero-padded 512-sample window
       if (s < 0) s = -s;
       if (s >= VAD_WIN) s = 2 * (VAD_WIN - 1) - s;
@@ -268,14 +257,14 @@ vad_front_kernel(const float* __restrict__ wav, VadWeights P, VadItems it, float
 // of both layers in registers.  wrec = [W_hh0^T | W_ih1^T | W_hh1^T], each [64][256].
 __global__ void __launch_bounds__(256, 1)
 vad_rec_kernel(const float* __restrict__ wrec, const float* __restrict__ b1, const float* __restrict__ wdec,
-               const float* __restrict__ G, float* __restrict__ probs, VadItems it) {
+               const float* __restrict__ G, float* __restrict__ probs, ItemPass<VAD_GROUP> it) {
   extern __shared__ __align__(16) float sm[];
   float* W = sm;                       // [3][64][256]
   float* h0 = W + 3 * VAD_H * VAD_G;   // [64]
   float* h1 = h0 + VAD_H;              // [64]
   float* gt = h1 + VAD_H;              // [256]
   const int j = threadIdx.x, lane = j & 31;
-  const long long w0 = it.w_off[blockIdx.x], nw = it.w_off[blockIdx.x + 1] - w0;
+  const long long w0 = it.out[blockIdx.x], nw = it.out[blockIdx.x + 1] - w0;
   if (nw <= 0) return;
   for (int i = j; i < 3 * VAD_H * VAD_G / 4; i += 256)
     reinterpret_cast<float4*>(W)[i] = __ldg(reinterpret_cast<const float4*>(wrec) + i);
@@ -413,16 +402,10 @@ size_t svcb_vad_workspace_bytes(const svcb_vad* v, int32_t B, int64_t total_wind
 
 int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_offsets_host, int32_t B, float* probs_out,
                    float* feat_out, void* ws, size_t ws_bytes, svcb_stream stream) {
-  if (!v || !sample_offsets_host || B < 0) { set_error("svcb_vad_probs: bad argument"); return SVCB_E_BAD_SHAPE; }
-  if (sample_offsets_host[0] < 0) { set_error("svcb_vad_probs: negative first sample offset"); return SVCB_E_BAD_SHAPE; }
+  if (!v || !sample_offsets_host) { set_error("svcb_vad_probs: bad argument"); return SVCB_E_BAD_SHAPE; }
+  SVCB_TRY(check_ragged("svcb_vad_probs", sample_offsets_host, B, 0, 0, "samples", nullptr));
   long long total = 0;
-  for (int b = 0; b < B; ++b) {
-    if (sample_offsets_host[b + 1] < sample_offsets_host[b]) {
-      set_error("svcb_vad_probs: sample offsets of item " + std::to_string(b) + " decrease");
-      return SVCB_E_BAD_SHAPE;
-    }
-    total += svcb_vad_windows(sample_offsets_host[b + 1] - sample_offsets_host[b]);
-  }
+  for (int b = 0; b < B; ++b) total += svcb_vad_windows(sample_offsets_host[b + 1] - sample_offsets_host[b]);
   if (total == 0) return SVCB_OK;
   if (!wav || !probs_out) { set_error("svcb_vad_probs: bad argument"); return SVCB_E_BAD_SHAPE; }
   SVCB_TRY(check_workspace(ws, ws_bytes, svcb_vad_workspace_bytes(v, B, total), "vad"));
@@ -430,16 +413,9 @@ int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_of
   float* G = static_cast<float*>(ws);
   SVCB_CUDA_CHECK(ensure_dyn_smem(vad_front_kernel, VAD_FRONT_SMEM, g_front_smem));
   SVCB_CUDA_CHECK(ensure_dyn_smem(vad_rec_kernel, VAD_REC_SMEM, g_rec_smem_v));
-  long long win = 0;
-  for (int g0 = 0; g0 < B; g0 += VAD_GROUP) {
-    VadItems it;
-    it.n = std::min(VAD_GROUP, B - g0);
-    it.w_off[0] = win;
-    for (int i = 0; i <= it.n; ++i) it.s_off[i] = sample_offsets_host[g0 + i];
-    for (int i = 0; i < it.n; ++i) it.w_off[i + 1] = it.w_off[i] + svcb_vad_windows(it.s_off[i + 1] - it.s_off[i]);
-    const long long W = it.w_off[it.n] - win;
-    win = it.w_off[it.n];
-    if (W == 0) continue;
+  return for_each_pass<VAD_GROUP>(sample_offsets_host, B, svcb_vad_windows, [&](const ItemPass<VAD_GROUP>& it, int) -> int {
+    const long long W = it.out[it.n] - it.out[0];
+    if (W == 0) return SVCB_OK;
     {
       KernelScope ks("vad_front", s, (double)W * VAD_NF * (2.0 * VAD_FEAT * VAD_NFFT + 4.0 * 16 * VAD_FEAT + 2.0 * VAD_G * VAD_H),
                      (double)W * 4.0 * (VAD_WIN + VAD_G + (feat_out ? VAD_H : 0)));
@@ -451,8 +427,8 @@ int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_of
       vad_rec_kernel<<<it.n, 256, VAD_REC_SMEM, s>>>(v->wrec, v->b1, v->wdec, G, probs_out, it);
       SVCB_LAUNCH_CHECK("vad_rec");
     }
-  }
-  return SVCB_OK;
+    return SVCB_OK;
+  });
 }
 
 }  // extern "C"

@@ -8,7 +8,6 @@ The resampler is scipy.signal.resample_poly's polyphase Kaiser FIR (the project'
 agree, ceil(n sr_out / sr_in), and the values differ slightly.  When the rates are equal nothing is resampled."""
 from __future__ import annotations
 
-import ctypes
 import math
 from typing import List, Sequence, Tuple
 
@@ -78,25 +77,19 @@ def _device_taps(up: int, down: int, dev: torch.device):
     return _TAPS[key]
 
 
-def _offsets(lens: Sequence[int]):
-    o = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
-    return (ctypes.c_int64 * len(o))(*o.tolist()), o
-
-
 def _resample_device(audios: Sequence, sr_in: int, sr_out: int, dev: torch.device):
     """The batch resampled on the device: (flat float32 device tensor, output offsets).  Equal rates copy the input."""
     up, down = ratio(sr_in, sr_out)
-    clips = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1) for a in audios]
-    flat = torch.from_numpy(np.concatenate(clips)).to(dev)
+    flat, so = _lib.ragged(audios, dev)
     if up == down:
-        return flat, _offsets([c.shape[0] for c in clips])
-    in_c, _ = _offsets([c.shape[0] for c in clips])
-    out_c, o = _offsets([-(-c.shape[0] * up // down) for c in clips])
+        return flat, so
+    B = len(so) - 1
+    oo = _lib.offsets(out_len(so[b + 1] - so[b], sr_in, sr_out) for b in range(B))
     taps, rm = _device_taps(up, down, dev)
-    y = torch.empty(max(int(o[-1]), 1), dtype=torch.float32, device=dev)
-    _lib.call("resample_ragged", flat.data_ptr(), in_c, len(clips), up, down, taps.data_ptr(), taps.numel(), rm,
-              y.data_ptr(), device=dev)
-    return y, (out_c, o)
+    y = torch.empty(max(oo[-1], 1), dtype=torch.float32, device=dev)
+    _lib.call("resample_ragged", flat.data_ptr(), so, B, up, down, taps.data_ptr(), taps.numel(), rm, y.data_ptr(),
+              device=dev)
+    return y, oo
 
 
 @torch.no_grad()
@@ -105,9 +98,8 @@ def resample_batch(audios: Sequence, sr_in: int, sr_out: int, device="cuda") -> 
     dev = _lib.cuda_device(device)
     if not audios:
         return []
-    y, (_, o) = _resample_device(audios, sr_in, sr_out, dev)
-    host = y.cpu().numpy()
-    return [host[o[i]:o[i + 1]] for i in range(len(audios))]
+    y, oo = _resample_device(audios, sr_in, sr_out, dev)
+    return _lib.split(y.cpu().numpy(), oo)
 
 
 @torch.no_grad()
@@ -118,9 +110,8 @@ def pcm16_batch(audios: Sequence, sr_in: int, sr_out: int, device="cuda") -> Tup
     dev = _lib.cuda_device(device)
     if not audios:
         return [], np.zeros(0, np.float32)
-    y, (offs, o) = _resample_device(audios, sr_in, sr_out, dev)
-    out = torch.empty(max(int(o[-1]), 1), dtype=torch.int16, device=dev)
+    y, oo = _resample_device(audios, sr_in, sr_out, dev)
+    out = torch.empty(max(oo[-1], 1), dtype=torch.int16, device=dev)
     peak = torch.empty(len(audios), dtype=torch.float32, device=dev)
-    _lib.call("pcm16_normalise_ragged", y.data_ptr(), offs, len(audios), out.data_ptr(), peak.data_ptr(), device=dev)
-    host = out.cpu().numpy()
-    return [host[o[i]:o[i + 1]] for i in range(len(audios))], peak.cpu().numpy()
+    _lib.call("pcm16_normalise_ragged", y.data_ptr(), oo, len(audios), out.data_ptr(), peak.data_ptr(), device=dev)
+    return _lib.split(out.cpu().numpy(), oo), peak.cpu().numpy()

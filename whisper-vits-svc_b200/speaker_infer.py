@@ -211,17 +211,11 @@ class SpeakerEncoderB200:
     @torch.no_grad()
     def mel_batch(self, wavs: Sequence) -> Tuple[torch.Tensor, List[int]]:
         """Ragged batch of prepared waveforms -> (mel [sum T_b, 80] on the device, frame offsets [B + 1])."""
-        wavs = [torch.as_tensor(np.asarray(w, np.float32)).reshape(-1) for w in wavs]
-        so = [0]
-        for w in wavs:
-            so.append(so[-1] + int(w.numel()))
-        fo = [0]
-        for b in range(len(wavs)):
-            fo.append(fo[-1] + self.frames(so[b + 1] - so[b]))
-        flat = torch.cat(wavs).to(self.device) if wavs else torch.zeros(0, device=self.device)
+        flat, so = _lib.ragged(wavs, self.device)
+        B = len(so) - 1
+        fo = list(_lib.offsets(self.frames(so[b + 1] - so[b]) for b in range(B)))
         mel = torch.empty(max(fo[-1], 1), N_MELS, device=self.device, dtype=torch.float32)
-        offs = (ctypes.c_int64 * len(so))(*so)
-        self._handle.call("speaker_mel", flat.data_ptr(), offs, len(wavs), mel.data_ptr(), None, 0)
+        self._handle.call("speaker_mel", flat.data_ptr(), so, B, mel.data_ptr(), None, 0)
         return mel[:fo[-1]], fo
 
     @torch.no_grad()

@@ -7,7 +7,6 @@ The device path implements n_fft 1024, hop 320 and win 1024 (configs/base.yaml);
 rejected.  A clip of n samples gives n // 320 frames; it needs more than 352 samples, the reflect padding."""
 from __future__ import annotations
 
-import ctypes
 from typing import List, Sequence
 
 import numpy as np
@@ -69,17 +68,8 @@ def spec_batch(audios: Sequence, hp, device="cuda") -> List[torch.Tensor]:
         return []
     for x in clips:
         _range_notice(x)
-    so = [0]
-    for x in clips:
-        so.append(so[-1] + int(x.numel()))
-    counts = [BINS * frames(x.numel()) for x in clips]
-    flat = torch.cat(clips).to(dev)
-    out = torch.empty(max(sum(counts), 1), dtype=torch.float32, device=dev)
-    offs = (ctypes.c_int64 * len(so))(*so)
-    _lib.call("linear_spec_ragged", flat.data_ptr(), offs, len(clips), out.data_ptr(), None, 0, device=dev)
-    host = out.cpu()
-    res, o = [], 0
-    for c in counts:
-        res.append(host[o:o + c].view(BINS, c // BINS))
-        o += c
-    return res
+    flat, so = _lib.ragged(clips, dev)
+    fo = _lib.offsets(BINS * frames(x.numel()) for x in clips)
+    out = torch.empty(max(fo[-1], 1), dtype=torch.float32, device=dev)
+    _lib.call("linear_spec_ragged", flat.data_ptr(), so, len(clips), out.data_ptr(), None, 0, device=dev)
+    return [s.view(BINS, s.numel() // BINS) for s in _lib.split(out.cpu(), fo)]

@@ -9,7 +9,7 @@ reaches the device: it has no windows, so no probabilities and no speech.
 """
 from __future__ import annotations
 
-import ctypes
+import ctypes  # noqa: F401  (callers build svcb_vad_probs offset arrays through vad_infer.ctypes)
 from typing import Dict, List, Sequence, Tuple
 
 import numpy as np
@@ -128,19 +128,15 @@ class VadB200:
     def speech_probs_device(self, wavs: Sequence, features: bool = False):
         """Ragged batch of 16 kHz waveforms -> (probs [sum W_b] on the device, window offsets [B + 1]) and, with
         `features`, the encoder outputs [sum W_b, 64]."""
-        wavs = [(w.float() if torch.is_tensor(w) else torch.as_tensor(np.asarray(w, np.float32))).reshape(-1) for w in wavs]
-        so, wo = [0], [0]
-        for w in wavs:
-            so.append(so[-1] + int(w.numel()))
-            wo.append(wo[-1] + windows(w.numel()))
+        flat, so = _lib.ragged(wavs, self.device)
+        B = len(so) - 1
+        wo = list(_lib.offsets(windows(so[b + 1] - so[b]) for b in range(B)))
         W = wo[-1]
         probs = torch.empty(max(W, 1), device=self.device, dtype=torch.float32)
         feat = torch.empty(max(W, 1), HIDDEN, device=self.device, dtype=torch.float32) if features else None
         if W > 0:
-            ws = self._handle.workspace(_lib.load().svcb_vad_workspace_bytes(self._handle, len(wavs), W))
-            flat = torch.cat(wavs).to(self.device)
-            offs = (ctypes.c_int64 * len(so))(*so)
-            self._handle.call("vad_probs", flat.data_ptr(), offs, len(wavs), probs.data_ptr(),
+            ws = self._handle.workspace(_lib.load().svcb_vad_workspace_bytes(self._handle, B, W))
+            self._handle.call("vad_probs", flat.data_ptr(), so, B, probs.data_ptr(),
                               feat.data_ptr() if features else None, ws.data_ptr(), ws.numel())
         out = (probs[:W], wo)
         return out + (feat[:W],) if features else out
@@ -149,13 +145,8 @@ class VadB200:
         """Ragged batch of 16 kHz waveforms -> a list of per-window fp32 probabilities (and of [W_b, 64] encoder
         outputs with `features`)."""
         r = self.speech_probs_device(wavs, features)
-        wo = r[1]
-        p = r[0].cpu().numpy()
-        probs = [p[wo[b]:wo[b + 1]] for b in range(len(wo) - 1)]
-        if not features:
-            return probs
-        f = r[2].cpu().numpy()
-        return probs, [f[wo[b]:wo[b + 1]] for b in range(len(wo) - 1)]
+        probs = _lib.split(r[0].cpu().numpy(), r[1])
+        return (probs, _lib.split(r[2].cpu().numpy(), r[1])) if features else probs
 
 
 def load_model(path: str, device="cuda") -> VadB200:
