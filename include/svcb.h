@@ -147,6 +147,20 @@ int svcb_infer(const svcb_model* m, const float* ppg, const float* vec, const fl
                float* wave, int32_t B, int32_t T, void* ws, size_t ws_bytes,
                const svcb_taps* taps, svcb_stream stream);
 
+/* svcb_infer for a ragged batch of chunks: the layouts of svcb_infer, padded to T frames.  Item b is the first
+ * n_b = n_frames_host[b] (1..T) frames of ppg, vec, pit and eps and the first n_b*hop samples of source; nothing past
+ * them reaches its result.  The first n_b*hop samples of item b's wave are bitwise those of a lone svcb_infer of the
+ * item (B = 1, T = n_b, lengths = {n_b}, same inputs); its later samples are zero.  (svcb_infer with lengths < T keeps
+ * the reference's padded-batch semantics instead: the generator there runs unmasked over all T frames.)
+ * The lengths are checked on the host before any launch.  SVCB_E_UNSUPPORTED, also before any launch, unless the model
+ * is at precision 3 and every generator stage takes a form with per-item ends at T and at every n_b: the tensor-core
+ * upsamplers (comb, fused, or tensor-core phases with the tensor-core noise conv), AMP_TC or space-to-depth AMP
+ * blocks, and the fused tail (a 16-byte aligned wave); configs/base.yaml's generator does at any length.
+ * ws_bytes >= svcb_workspace_bytes(m, B, T), which includes a region for the lengths.  No taps. */
+int svcb_infer_ragged(const svcb_model* m, const float* ppg, const float* vec, const float* pit, const float* spk,
+                      const int32_t* n_frames_host, const float* source, const float* eps, float* wave,
+                      int32_t B, int32_t T, void* ws, size_t ws_bytes, svcb_stream stream);
+
 /* Number of kernels enqueued by the most recent call on this thread (bench.py's gpu_launches). */
 int64_t svcb_last_launch_count(void);
 

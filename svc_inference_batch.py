@@ -6,7 +6,7 @@ The reference loads Whisper once, writes a .ppg.npy per file and then starts one
 checkpoint and re-spawning the HuBERT / pitch extractors every time.  Here the model is loaded
 once per GPU, files are sharded across the ranks of a `torchrun` launch (one process per GPU, one
 NCCL broadcast of the packed weights, no collective on the data path), and per rank the chunks of ALL its
-files are bucketed by length and run as full device batches (hostio.BatchEngine) while host threads read
+files are sorted by length and run as full ragged device batches (hostio.BatchEngine) while host threads read
 features and write WAVs.  Missing `<name>.ppg.npy` / `<name>.vec.npy` are extracted in-process by the H100 Whisper /
 HuBERT-Soft encoders (one model load per rank).  CREPE is outside the H100 hot path (SURVEY.md §8f-4):
 `<name>.pit.csv` must sit next to `<name>.wav` (or in --feat); a file without it is reported and skipped — the
@@ -39,7 +39,7 @@ def main():
     parser.add_argument('--feat', type=str, default=None, help="dir holding <name>.{ppg,vec}.npy / .pit.csv")
     parser.add_argument('--whisper', type=str, default=os.path.join("whisper_pretrain", "large-v2.pt"))
     parser.add_argument('--hubert', type=str, default=os.path.join("hubert_pretrain", "hubert-soft-0d54a1f4.pt"))
-    parser.add_argument('--max-batch', type=int, default=32, help="chunks per device call (equal-length chunks of all files)")
+    parser.add_argument('--max-batch', type=int, default=32, help="chunks per device call (chunks of all files, longest first)")
     args = parser.parse_args()
     wave_path = args.wave
     assert os.path.isdir(wave_path), f"{wave_path} is not folder"
@@ -111,7 +111,7 @@ def main():
     del hubert
 
     from concurrent.futures import ThreadPoolExecutor
-    engine = hostio.BatchEngine(model, hp, device, max_batch=args.max_batch)
+    engine = hostio.BatchEngine(model, hp, device, max_batch=args.max_batch, ragged=True)
     loaders, writers = ThreadPoolExecutor(max_workers=4), ThreadPoolExecutor(max_workers=4)
 
     def jobs():

@@ -134,6 +134,7 @@ SIGNATURES = {
     "svcb_flow": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, POINTER(Taps), c_void_p]),
     "svcb_generator": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, POINTER(Taps), c_void_p]),
     "svcb_infer": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, POINTER(Taps), c_void_p]),
+    "svcb_infer_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, c_void_p]),
     "svcb_op_conv1d": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int32] * 9 + [c_void_p]),
     "svcb_op_snake_alias": (c_int, [c_void_p] * 6 + [c_int32] * 3 + [c_void_p]),
     "svcb_op_layernorm_c": (c_int, [c_void_p] * 5 + [c_int32] * 4 + [c_float, c_void_p]),

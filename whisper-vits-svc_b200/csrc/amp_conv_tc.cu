@@ -40,13 +40,15 @@ int p8_rows(int L) { return p8_rows_of(L); }
 // of bf16 hi and 16 of lo) and the warp stores 512 contiguous bytes per part.
 constexpr int SP3_ROWS = 256;  // image rows per CTA (8 warps x 32)
 
+// wide: the interior test of the vector form (a dense batch: VEC; a ragged item: what a lone call of its own length
+// would choose, so that the same runs take the packed and the clamped arithmetic)
 template <bool VEC>
-__device__ __forceinline__ void sp3_run(const float* __restrict__ xr, int n0, int L, const SnakeTapsV& tp,
+__device__ __forceinline__ void sp3_run(const float* __restrict__ xr, int n0, int L, bool wide, const SnakeTapsV& tp,
                                         const float* f_up, const float* f_dn, float a_, float b_, float (&o)[8]) {
   // (the vector loads touch xr[n0-8 .. n0+16): keep them inside the row)
-  if (VEC ? (n0 - 8 >= 0 && n0 + 16 <= L) : (n0 - 6 >= 0 && n0 + 13 <= L - 1)) {
+  if (wide ? (n0 - 8 >= 0 && n0 + 16 <= L) : (n0 - 6 >= 0 && n0 + 13 <= L - 1)) {
     float x[24];  // xr[n0-8 .. n0+16)
-    if (VEC) {
+    if (VEC && (wide || (n0 - 8 >= 0 && n0 + 16 <= L))) {   // (a dense batch: wide is the same test)
 #pragma unroll
       for (int q = 0; q < 6; ++q) {
         const float4 t4 = __ldg(reinterpret_cast<const float4*>(xr + n0 - 8) + q);
@@ -79,11 +81,13 @@ __device__ __forceinline__ void sp3_run(const float* __restrict__ xr, int n0, in
   }
 }
 
-template <bool VEC, int MINB>
+// RAG: a ragged batch (lens): a separate instantiation, so that the dense ones fold `wide` and Lb at compile time
+template <bool VEC, int MINB, bool RAG>
 __global__ void __launch_bounds__(256, MINB)
 snake_pack3_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo,
                    const float* __restrict__ ea, const float* __restrict__ inv_b,
-                   const float* __restrict__ fu_g, const float* __restrict__ fd_g, const SnakeTapsV tp, int C, int L, int Lp) {
+                   const float* __restrict__ fu_g, const float* __restrict__ fd_g, const SnakeTapsV tp, int C, int L, int Lp,
+                   const int* __restrict__ lens, int lscale) {
   __shared__ float tile[8][32 * 9];   // per warp: [row][channel], row stride 9 -> conflict-free both ways
   __shared__ float f_up[12], f_dn[12];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -95,11 +99,14 @@ snake_pack3_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ hi, 
   const int c = lane >> 2, run = lane & 3;
   const int ch = oc * 8 + c;
   const int n0 = row0 - P8_PAD + 8 * run;
+  // a ragged item ends at Lb <= L: its rows past Lb are zero, as in the image of a lone call
+  const int Lb = RAG ? __ldg(lens + b) * lscale : L;
+  const bool wide = RAG ? (Lb & 3) == 0 : VEC;
   float o[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) o[i] = 0.f;
-  if (ch < C && n0 < L && n0 + 8 > 0) {
-    sp3_run<VEC>(x + ((long long)b * C + ch) * L, n0, L, tp, f_up, f_dn, __ldg(ea + ch), __ldg(inv_b + ch), o);
+  if (ch < C && n0 < Lb && n0 + 8 > 0) {
+    sp3_run<VEC>(x + ((long long)b * C + ch) * L, n0, Lb, wide, tp, f_up, f_dn, __ldg(ea + ch), __ldg(inv_b + ch), o);
   }
   float* tw = tile[warp];
 #pragma unroll
@@ -134,7 +141,8 @@ size_t p8_image_bytes(int B, int C, int L) {  // one of hi / lo
 }
 
 int launch_snake_pack(const float* x, void* hi, void* lo, const float* ea, const float* inv_b, const float* fu,
-                      const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps) {
+                      const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps, const int* lens,
+                      int lscale) {
   if (B <= 0 || C <= 0 || L <= 0) return SVCB_OK;
   SnakeTapsV tp;
   if (taps) tp = *taps;
@@ -150,8 +158,10 @@ int launch_snake_pack(const float* x, void* hi, void* lo, const float* ea, const
     const bool vec = (L & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
     // 64 registers -> four CTAs (32 warps) per SM: each warp lives for one tile, so residency is
     // what hides its initial load latency (10.8 vs 11.4 ms/step with two CTAs)
-    if (vec) snake_pack3_kernel<true, 4><<<grid3, 256, 0, s>>>(x, h, l, ea, inv_b, fu, fd, tp, C, L, Lp);
-    else snake_pack3_kernel<false, 4><<<grid3, 256, 0, s>>>(x, h, l, ea, inv_b, fu, fd, tp, C, L, Lp);
+    if (lens && vec) snake_pack3_kernel<true, 4, true><<<grid3, 256, 0, s>>>(x, h, l, ea, inv_b, fu, fd, tp, C, L, Lp, lens, lscale);
+    else if (lens) snake_pack3_kernel<false, 4, true><<<grid3, 256, 0, s>>>(x, h, l, ea, inv_b, fu, fd, tp, C, L, Lp, lens, lscale);
+    else if (vec) snake_pack3_kernel<true, 4, false><<<grid3, 256, 0, s>>>(x, h, l, ea, inv_b, fu, fd, tp, C, L, Lp, lens, lscale);
+    else snake_pack3_kernel<false, 4, false><<<grid3, 256, 0, s>>>(x, h, l, ea, inv_b, fu, fd, tp, C, L, Lp, lens, lscale);
     SVCB_LAUNCH_CHECK("snake_pack");
   }
   return SVCB_OK;

@@ -77,17 +77,18 @@ __device__ __forceinline__ void s2d_store_octet(__nv_bfloat16* hi, __nv_bfloat16
 __global__ void __launch_bounds__(256, 4)
 snake_pack_s2d_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo,
                       const float* __restrict__ ea, const float* __restrict__ inv_b,
-                      const SnakeTapsV tp, int C, int L, int r, int Rp) {
+                      const SnakeTapsV tp, int C, int L, int r, int Rp, const int* __restrict__ lens, int lscale) {
   const int run = blockIdx.x * 256 + threadIdx.x;
   const int c = blockIdx.y, b = blockIdx.z;
-  if (run * 8 >= L) return;
+  const int Lb = lens ? __ldg(lens + b) * lscale : L;   // a ragged item's end: its later rows stay zero
+  if (run * 8 >= Lb) return;
   const int opr = r >> 3;                       // octets per row of this channel (0 for r = 4: half an octet)
   const float* xr = x + ((long long)b * C + c) * L;
   const int n0 = run * 8;
   const float a_ = __ldg(ea + c), b_ = __ldg(inv_b + c);
   float out[8], xw[24];
-  const bool first = n0 == 0, last = n0 + 8 == L;
-  if (n0 - 8 >= 0 && n0 + 16 <= L) {
+  const bool first = n0 == 0, last = n0 + 8 == Lb;
+  if (n0 - 8 >= 0 && n0 + 16 <= Lb) {
 #pragma unroll
     for (int q = 0; q < 6; ++q) {
       const float4 t4 = __ldg(reinterpret_cast<const float4*>(xr + n0 - 8) + q);
@@ -95,7 +96,7 @@ snake_pack_s2d_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ h
     }
   } else {   // within 8 samples of a sequence end: replicate padding of x (alias/resample.py:28) = clamped loads
 #pragma unroll
-    for (int j = 0; j < 24; ++j) xw[j] = __ldg(xr + min(max(n0 - 8 + j, 0), L - 1));
+    for (int j = 0; j < 24; ++j) xw[j] = __ldg(xr + min(max(n0 - 8 + j, 0), Lb - 1));
   }
   snake8_packed(xw, tp, a_, 0.5f * b_, out, first, last);   // common.cuh: packed f32x2 FIRs
   if (opr) {
@@ -120,7 +121,8 @@ snake_pack_s2d_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ h
 }
 
 int launch_snake_pack_s2d(const float* x, void* hi, void* lo, const float* ea, const float* inv_b, const float* fu,
-                          const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps) {
+                          const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps, const int* lens,
+                          int lscale) {
   const int r = C > 0 ? s2d::N / C : 0;
   if (B <= 0 || L <= 0 || C * r != s2d::N || (r != 4 && r != 8 && r != 16) || L % 8 || (reinterpret_cast<uintptr_t>(x) & 15)) {
     set_error("snake_pack_s2d: unsupported shape");
@@ -134,7 +136,7 @@ int launch_snake_pack_s2d(const float* x, void* hi, void* lo, const float* ea, c
   KernelScope ks(kname, s, 0.0, 8.0 * B * C * (double)L, 70.0 * B * C * (double)L);
   dim3 grid((L / 8 + 255) / 256, C, B);
   snake_pack_s2d_kernel<<<grid, 256, 0, s>>>(x, static_cast<__nv_bfloat16*>(hi), static_cast<__nv_bfloat16*>(lo), ea,
-                                             inv_b, tp, C, L, r, s2d_rows(L, r));
+                                             inv_b, tp, C, L, r, s2d_rows(L, r), lens, lscale);
   SVCB_LAUNCH_CHECK("snake_pack_s2d");
   return SVCB_OK;
 }
@@ -167,7 +169,8 @@ int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, in
 //   12 epilogue warps = 3 column groups x 4 row quadrants: group g owns units u = g (mod 3), a unit
 //                  being one channel (r >= 8) or a channel pair (r = 4): 6-7 / 6-7 / 3-4 units per group for
 //                  C = 20 / 40 / 10 (13 warps leave the MMA warpgroups the registers of 160 accumulator columns)
-template <int R>
+// RAG: a ragged batch (p.lens): a separate instantiation, so that the dense one keeps its registers
+template <int R, bool RAG>
 __global__ void __launch_bounds__(s2d::THREADS, 1)
 amp_s2d_link_kernel(const AmpS2dParams p) {
   using namespace s2d;
@@ -249,7 +252,9 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
       const int b = tile / tpi, t = tile - b * tpi;
       const int tau0 = t * S - HS;
       const int tau = tau0 + row;
-      const bool valid = tau >= 0 && tau < nrows;
+      // a ragged item's last row: its later rows are neither read as residual, stored, nor written to the image
+      const int nrows_b = RAG ? __ldg(p.lens + b) * p.lscale / R : nrows;
+      const bool valid = tau >= 0 && tau < nrows_b, at_end = tau == nrows_b - 1;
       const bool useful = valid && row >= HS && row < TILE - HS;
       // residual rows are independent of the accumulator: the first unit's are requested before the wait,
       // every later unit's one unit ahead (their latency was 19 % of all stall samples)
@@ -374,7 +379,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
             float4 l4 = *reinterpret_cast<const float4*>(strip + row * RS - 4);    // previous row's last four (row 0 / 127
             float4 r4 = *reinterpret_cast<const float4*>(strip + row * RS + RS);   //  read outside the strip: halo rows, unused)
             if (tau == 0) l4 = make_float4(v[k * R], v[k * R], v[k * R], v[k * R]);
-            if (tau == nrows - 1) r4 = make_float4(v[k * R + R - 1], v[k * R + R - 1], v[k * R + R - 1], v[k * R + R - 1]);
+            if (at_end) r4 = make_float4(v[k * R + R - 1], v[k * R + R - 1], v[k * R + R - 1], v[k * R + R - 1]);
             xw[0] = l4.x; xw[1] = l4.y; xw[2] = l4.z; xw[3] = l4.w;
 #pragma unroll
             for (int j = 0; j < R; ++j) xw[4 + j] = v[k * R + j];
@@ -438,7 +443,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
 #pragma unroll
               for (int i = 0; i < 5; ++i) pv[i] = V[k][3].x;
             }
-            if (tau == nrows - 1) {
+            if (at_end) {
 #pragma unroll
               for (int i = 0; i < 5; ++i) nx[i] = V[k][R + 2].y;
             }
@@ -486,7 +491,7 @@ int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s) {
     set_error("amp_s2d_link: tap range exceeds the A panel, wrong image rows or missing operand");
     return SVCB_E_BAD_SHAPE;
   }
-  static DevSmemCache c4, c8, c16;
+  static DevSmemCache c4, c8, c16, g4, g8, g16;
   const int n_sm = device_sm_count();
   if (n_sm <= 0) { set_error("amp_s2d_link: cannot query the SM count"); return SVCB_E_CUDA; }
   const int S = s2d_tile_stride(r);
@@ -497,16 +502,21 @@ int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s) {
   const double el = (double)p.B * p.C * p.L;
   KernelScope ks(kname, s, 2.0 * p.C * p.K * el, el * (4.0 + (p.o_hi ? 4.0 : 0.0) + (p.res ? 4.0 : 0.0) + (p.y ? (p.accum ? 8.0 : 4.0) : 0.0)),
                  p.o_hi ? 70.0 * el : 0.0);
-  if (r == 4) {
-    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_s2d_link_kernel<4>, s2d::SMEM, c4));
-    amp_s2d_link_kernel<4><<<grid, s2d::THREADS, s2d::SMEM, s>>>(p);
-  } else if (r == 8) {
-    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_s2d_link_kernel<8>, s2d::SMEM, c8));
-    amp_s2d_link_kernel<8><<<grid, s2d::THREADS, s2d::SMEM, s>>>(p);
+#define SVCB_S2D_LINK(r_, rag, cache)                                                 \
+  do {                                                                                \
+    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_s2d_link_kernel<r_, rag>, s2d::SMEM, cache)); \
+    amp_s2d_link_kernel<r_, rag><<<grid, s2d::THREADS, s2d::SMEM, s>>>(p);            \
+  } while (0)
+  if (p.lens) {
+    if (r == 4) SVCB_S2D_LINK(4, true, g4);
+    else if (r == 8) SVCB_S2D_LINK(8, true, g8);
+    else SVCB_S2D_LINK(16, true, g16);
   } else {
-    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_s2d_link_kernel<16>, s2d::SMEM, c16));
-    amp_s2d_link_kernel<16><<<grid, s2d::THREADS, s2d::SMEM, s>>>(p);
+    if (r == 4) SVCB_S2D_LINK(4, false, c4);
+    else if (r == 8) SVCB_S2D_LINK(8, false, c8);
+    else SVCB_S2D_LINK(16, false, c16);
   }
+#undef SVCB_S2D_LINK
   SVCB_LAUNCH_CHECK("amp_s2d_link");
   return SVCB_OK;
 }

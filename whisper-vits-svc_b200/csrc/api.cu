@@ -223,6 +223,21 @@ static int launch_mask_mul(float* x, const long long* lengths, int B, int C, int
   return SVCB_OK;
 }
 
+// x[b, c, t] = 0 for lengths[b] <= t < T: the tails of a ragged batch, one thread per element of the longest tail
+// (no launch when every item fills T)
+__global__ void zero_tail_kernel(float* __restrict__ x, const long long* __restrict__ lengths, int C, int T) {
+  const long long t = lengths[blockIdx.z] + (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < T) x[((long long)blockIdx.z * C + blockIdx.y) * T + t] = 0.f;
+}
+static int launch_zero_tail(float* x, const long long* lengths, long long min_len, int B, int C, int T, cudaStream_t s) {
+  if (min_len >= T) return SVCB_OK;
+  dim3 grid((unsigned)((T - min_len + 127) / 128), C, B);
+  KernelScope ks("zero_tail", s, 0.0, 4.0 * B * C * (double)(T - min_len));
+  zero_tail_kernel<<<grid, 128, 0, s>>>(x, lengths, C, T);
+  SVCB_LAUNCH_CHECK("zero_tail");
+  return SVCB_OK;
+}
+
 // ----------------------------------------------------------------------------- upsampler finalize
 // The ConvTranspose1d upsamplers (generator.py:183) run as `rate` polyphase sub-convolutions.  Each
 // phase writes its outputs CONTIGUOUSLY into a phase-major scratch (coalesced stores); this kernel
@@ -271,21 +286,25 @@ static int launch_ups_finalize(const UpsFinalizeParams& p, int B, cudaStream_t s
   return SVCB_OK;
 }
 
-// source [B][Ltot] -> zero-padded copy [B][32 + Ltot + tail] for the space-to-depth noise convs
+// source [B][Ltot] -> zero-padded copy [B][32 + Ltot + tail] for the space-to-depth noise convs; a ragged item's source
+// ends at lens[b] * hop samples
 constexpr int SRC_PADF = 32;
 __global__ void pad_source_kernel(const float* __restrict__ src, float* __restrict__ dst, long long Ltot,
-                                  long long Lpad) {
+                                  long long Lpad, const int* __restrict__ lens, int hop) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (i >= Lpad) return;
   const long long si = i - SRC_PADF;
-  dst[(long long)b * Lpad + i] = (si >= 0 && si < Ltot) ? src[(long long)b * Ltot + si] : 0.f;
+  const long long n = lens ? (long long)lens[b] * hop : Ltot;
+  dst[(long long)b * Lpad + i] = (si >= 0 && si < n) ? src[(long long)b * Ltot + si] : 0.f;
 }
 
 // ----------------------------------------------------------------------------- prior encoder
+// ragged (svcb_infer_ragged): pre / hub also read ppg / vec as zero past each item's length, as a lone call's padding
+// (the reference convolves its padded batch unmasked there)
 static int run_prior(const svcb_model* m, Ctx& ctx, const float* ppg, const float* vec,
                      const float* pit, const long long* lengths, const float* eps, float* z_p, int B,
-                     int T) {
+                     int T, bool ragged = false) {
   const svcb_config& c = m->cfg;
   const int H = c.hidden_channels, C = c.inter_channels, Fc = c.filter_channels;
   cudaStream_t s = ctx.stream;
@@ -301,11 +320,11 @@ static int run_prior(const svcb_model* m, Ctx& ctx, const float* ppg, const floa
   {  // pre / hub on time-major inputs (vits/models.py:40-46)
     ConvParams p = std_conv(m->pre, ppg, x, B, T, T, 2);
     p.sxb = (long long)T * c.ppg_dim; p.sxc = 1; p.sxt = c.ppg_dim;
-    p.lengths = lengths; p.flags = CONV_OUT_MASK;
+    p.lengths = lengths; p.flags = CONV_OUT_MASK | (ragged ? CONV_IN_MASK : 0);
     RUN(run_conv(m, m->pre, p, s));
     ConvParams q = std_conv(m->hub, vec, x, B, T, T, 2);
     q.sxb = (long long)T * c.vec_dim; q.sxc = 1; q.sxt = c.vec_dim;
-    q.lengths = lengths; q.flags = CONV_OUT_MASK; q.res = x;
+    q.lengths = lengths; q.flags = p.flags; q.res = x;
     RUN(run_conv(m, m->hub, q, s));
   }
   RUN(launch_pitch_embed_add(x, pit, m->pit_emb, B, H, T, s));
@@ -390,6 +409,8 @@ struct AmpStage {
   void *img_hi, *img_lo;      // snake_pack operand images (AMP_TC)
   void* s2d[4];               // two ping-pong S2D images, hi and lo each (AMP_S2D)
   int B, C, L, nres, nsplit;
+  const int* lens;            // ragged batch (AMP_TC, AMP_S2D): item b ends at lens[b] * lscale samples, or null
+  int lscale;
   float* out(int d) const { return d == 0 ? RA : d == 1 ? RB : ACC; }
   bool accum(int d, int j) const { return d == 2 && j > 0; }
   float out_div(int d, int j) const { return d == 2 && j == nres - 1 ? (float)nres : 0.f; }
@@ -406,6 +427,7 @@ static AmpS2dParams s2d_link(const AmpStage& a, const ResBlock& R, int d, int ha
   q.a_hi = in[0]; q.a_lo = in[1];
   q.wpk = half ? R.c2_s2d[d] : R.c1_s2d[d]; q.bias = half ? R.c2[d].b : R.c1[d].b;
   q.ntaps = half ? R.s2d_nt2[d] : R.s2d_nt1[d]; q.mlo = half ? R.s2d_ml2[d] : R.s2d_ml1[d];
+  q.lens = a.lens; q.lscale = a.lscale;
   if (next < 6) {
     const SnakeW& act = R.act[next];
     q.o_hi = out[0]; q.o_lo = out[1];
@@ -418,7 +440,7 @@ static AmpS2dParams s2d_link(const AmpStage& a, const ResBlock& R, int d, int ha
 static int run_amp_s2d(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
   const SnakeW& s0 = R.act[0];
   const SnakeTapsV tv0 = s0.tapsv();
-  RUN(launch_snake_pack_s2d(a.X, a.s2d[0], a.s2d[1], s0.ea, s0.ib, s0.fu, s0.fd, a.B, a.C, a.L, ctx.stream, &tv0));
+  RUN(launch_snake_pack_s2d(a.X, a.s2d[0], a.s2d[1], s0.ea, s0.ib, s0.fu, s0.fd, a.B, a.C, a.L, ctx.stream, &tv0, a.lens, a.lscale));
   const float* cur = a.X;
   for (int d = 0; d < 3; ++d) {
     RUN(launch_amp_s2d_link(s2d_link(a, R, d, 0), ctx.stream));
@@ -456,10 +478,10 @@ static int run_amp_tc(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
     q.B = a.B; q.C = a.C; q.Cp = (a.C + 15) / 16 * 16; q.L = a.L; q.K = R.k; q.nsplit = a.nsplit;
     q.Lp = p8_rows(a.L); q.a_hi = a.img_hi; q.a_lo = lo;
     const SnakeTapsV tv1 = s1.tapsv(), tv2 = s2.tapsv();
-    RUN(launch_snake_pack(cur, a.img_hi, lo, s1.ea, s1.ib, s1.fu, s1.fd, a.B, a.C, a.L, ctx.stream, &tv1));
+    RUN(launch_snake_pack(cur, a.img_hi, lo, s1.ea, s1.ib, s1.fu, s1.fd, a.B, a.C, a.L, ctx.stream, &tv1, a.lens, a.lscale));
     q.y = a.T2; q.wpk = R.c1_tc[d]; q.bias = R.c1[d].b; q.dil = R.dil[d];
     RUN(launch_amp_conv_tc(q, ctx.stream));
-    RUN(launch_snake_pack(a.T2, a.img_hi, lo, s2.ea, s2.ib, s2.fu, s2.fd, a.B, a.C, a.L, ctx.stream, &tv2));
+    RUN(launch_snake_pack(a.T2, a.img_hi, lo, s2.ea, s2.ib, s2.fu, s2.fd, a.B, a.C, a.L, ctx.stream, &tv2, a.lens, a.lscale));
     q.wpk = R.c2_tc[d]; q.bias = R.c2[d].b; q.dil = 1; q.res = cur;
     q.y = a.out(d); q.accum = a.accum(d, j); q.out_div = a.out_div(d, j);
     RUN(launch_amp_conv_tc(q, ctx.stream));
@@ -484,8 +506,13 @@ static int run_amp_fp32(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
   return SVCB_OK;
 }
 
+// A ragged batch (svcb_infer_ragged) passes its lengths as lens (int32 frames, for the generator's own kernels) and
+// len64 ([n_ups + 1][B] int64: item b's length at the input rate of stage i in row i, for zero_tail and conv_tc) and has
+// been checked by ragged_forms(): every stage takes a form that reads them.  Item b then ends at its own length at
+// every rate, and what a conv reads past that end is zero, as in a lone call's padding.
 static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const float* z,
-                         const float* source, float* wave, int B, int T) {
+                         const float* source, float* wave, int B, int T, const long long* len64 = nullptr,
+                         const int* lens = nullptr, int min_n = 0) {
   const svcb_config& c = m->cfg;
   cudaStream_t s = ctx.stream;
   const int U = c.gen_input;
@@ -518,17 +545,19 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
   if (nsplit && !ctx.dry) {
     dim3 grid((unsigned)((Lpad + 255) / 256), B);
     KernelScope ks("pad_source", s, 0.0, 8.0 * B * (double)Lpad);
-    pad_source_kernel<<<grid, 256, 0, s>>>(source, SRCP, Ltot, Lpad);
+    pad_source_kernel<<<grid, 256, 0, s>>>(source, SRCP, Ltot, Lpad, lens, m->hop);
     SVCB_LAUNCH_CHECK("pad_source");
   }
   RUN(launch_linear_small(spk, m->ad_sw, m->ad_sb, sc, B, c.spk_dim, U, s));
   RUN(launch_linear_small(spk, m->ad_bw, m->ad_bb, bi, B, c.spk_dim, U, s));
   RUN(launch_layernorm_c(z, nullptr, sc, bi, xa, B, U, T, U, 1e-5f, s));
+  if (len64) RUN(launch_zero_tail(xa, len64, min_n, B, U, T, s));
   {
     ConvParams p = std_conv(m->conv_pre, xa, x0, B, T, T, 3);
     p.act = ACT_MISH;
     RUN(run_conv(m, m->conv_pre, p, s));
   }
+  if (len64) RUN(launch_zero_tail(x0, len64, min_n, B, c.gen_initial_channel, T, s));
   SVCB_TRY(tap(ctx, SVCB_TAP_GEN_PRE, x0, (size_t)B * c.gen_initial_channel * T));
 
   const float* x = x0;
@@ -548,6 +577,9 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
       q.Cin = ch; q.ilv = us.rate;
       q.x2 = SRCP + (SRC_PADF - sf / 2); q.sx2b = Lpad; q.sx2t = (long long)sf * us.rate;
       q.cin1 = us.comb_cin1; q.cin2 = us.comb_cin2;
+      // ragged: rows past an item's end read as zero in both inputs; a lone call's row bound (tau < Tin) also drops
+      // the source window of the row at its end, whose first sf/2 samples precede that end
+      if (len64) { q.lengths = len64 + (size_t)i * B; q.flags = CONV_IN_MASK; }
       RUN(launch_conv_tc(q, s));
     } else if (us.form == UPS_FUSED) {  // narrow stages: transposed conv + noise conv + biases in one fp32 pass
       UpsFusedParams q;
@@ -556,6 +588,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
       q.B = B; q.Cin = ch; q.Cout = chn; q.L = L; q.Ln = Ln; q.rate = us.rate; q.M = us.taps; q.pad = us.pad;
       q.cout_pad = us.phase[0].cout_pad; q.Kn = us.noise.k; q.sf = sf; q.padn = sf / 2;
       q.cout_pad_n = us.noise.cout_pad; q.Ltot = Ltot;
+      q.lens = lens; q.src_scale = m->hop;
       RUN(launch_ups_fused(q, s));
     } else {
       // `rate` polyphase sub-convolutions, each into its own contiguous slab of T1 (coalesced), interleaved + biased
@@ -598,7 +631,8 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
     SVCB_TRY(tap(ctx, SVCB_TAP_GEN_UP0 + i, X, (size_t)B * chn * Ln));
 
     const ResBlock* rb = &m->res[(size_t)i * c.n_res];
-    AmpStage a{X, ACC, T1, T2, RA, RB, IMG_HI, IMG_LO, {nullptr, nullptr, nullptr, nullptr}, B, chn, Ln, c.n_res, nsplit};
+    AmpStage a{X, ACC, T1, T2, RA, RB, IMG_HI, IMG_LO, {nullptr, nullptr, nullptr, nullptr}, B, chn, Ln, c.n_res, nsplit,
+               lens, Ln / T};
     // every block of a stage has the same channel count, so either all or none take the s2d form
     const bool s2d = rb[0].form == AMP_S2D && Ln % rb[0].s2d_r == 0 && Ln % 8 == 0;
     const size_t mark = ctx.off;
@@ -624,12 +658,15 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
       }
     }
     ctx.off = mark;
+    // the next upsampler reads the stage mean with zero padding past each ragged item's end (post_fused stops there)
+    if (len64 && i + 1 < c.n_ups) RUN(launch_zero_tail(ACC, len64 + (size_t)(i + 1) * B, (long long)min_n * (Ln / T), B, chn, Ln, s));
     SVCB_TRY(tap(ctx, SVCB_TAP_GEN_STAGE0 + i, ACC, (size_t)B * chn * Ln));
     x = ACC; ch = chn; L = Ln;
   }
   // activation_post + conv_post + tanh (generator.py:196-199)
   if (!m->conv_post.b && post_fused_supported(ch, L, m->conv_post.k, x, wave)) {
-    RUN(launch_post_fused(x, wave, m->post_act.ea, m->post_act.ib, m->post_act.tapsv(), m->conv_post_h.data(), B, ch, L, s));
+    RUN(launch_post_fused(x, wave, m->post_act.ea, m->post_act.ib, m->post_act.tapsv(), m->conv_post_h.data(), B, ch, L, s,
+                          lens, L / T));
     return SVCB_OK;
   }
   RUN(launch_snake_alias(x, T1, m->post_act.ea, m->post_act.ib, m->post_act.fu, m->post_act.fd, B, ch, L, s));
@@ -864,6 +901,59 @@ static int resolve(svcb_model* m, Resolver& R) {
   return SVCB_OK;
 }
 
+// svcb_infer_ragged: SVCB_E_UNSUPPORTED unless every generator stage takes, at T frames and at each item's own n[b], a
+// form that reads per-item ends (precision 3: the tensor-core upsamplers, AMP_TC or AMP_S2D, post_fused).
+static int ragged_forms(const svcb_model* m, const int32_t* n, int B, int T, const float* wave) {
+  const std::string who = "svcb_infer_ragged: ";
+  const svcb_config& c = m->cfg;
+  if (m->nsplit != 3) {
+    set_error(who + "needs a model at precision 3; this one has precision " + std::to_string(c.precision));
+    return SVCB_E_UNSUPPORTED;
+  }
+  int ch = c.gen_initial_channel;
+  long long f = 1;   // samples per frame after stage i
+  for (int i = 0; i < c.n_ups; ++i) {
+    const UpStage& us = m->ups[i];
+    ch /= 2; f *= us.rate;
+    bool ups = us.form == UPS_COMB || us.form == UPS_FUSED;
+    if (us.form == UPS_POLYPHASE && us.noise_form == NOISE_TC) {   // phases on conv_tc, source only through SRCP
+      ups = true;
+      for (bool tcp : us.phase_tc) ups = ups && tcp;
+    }
+    if (!ups) {
+      set_error(who + "generator stage " + std::to_string(i) + "'s upsampler has no ragged form");
+      return SVCB_E_UNSUPPORTED;
+    }
+    const ResBlock& R = m->res[(size_t)i * c.n_res];
+    if (R.form == AMP_S2D) {   // every block of a stage has the same form; the s2d test of run_generator per length
+      auto s2d = [&](long long L) { return L % R.s2d_r == 0 && L % 8 == 0; };
+      bool ok = s2d(T * f);
+      for (int b = 0; b < B && ok; ++b) ok = s2d(n[b] * f);
+      if (!ok) {
+        set_error(who + "generator stage " + std::to_string(i) + " would leave the space-to-depth form at some length");
+        return SVCB_E_UNSUPPORTED;
+      }
+    } else if (R.form != AMP_TC) {
+      set_error(who + "generator stage " + std::to_string(i) + "'s AMP blocks have no ragged form");
+      return SVCB_E_UNSUPPORTED;
+    }
+  }
+  bool post = !m->conv_post.b && post_fused_supported(ch, (int)(T * f), m->conv_post.k, wave, wave);
+  for (int b = 0; b < B && post; ++b) post = post_fused_supported(ch, (int)(n[b] * f), m->conv_post.k, wave, wave);
+  if (!post) {
+    set_error(who + "the generator's tail needs post_fused (a 16-byte aligned wave and 8 | samples)");
+    return SVCB_E_UNSUPPORTED;
+  }
+  return SVCB_OK;
+}
+
+// n64[i][b] = n[b] * f.v[i]: each item's length at the input rate of generator stage i (i = 0: frames)
+struct StageRates { long long v[SVCB_MAX_UPS + 1]; };
+__global__ void stage_lens_kernel(const int* __restrict__ n, long long* __restrict__ n64, StageRates f, int B, int rows) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < B * rows) n64[k] = n[k % B] * f.v[k / B];
+}
+
 static int validate_cfg(const svcb_config& c) {
   if (c.precision != 0 && c.precision != 1 && c.precision != 3) { set_error("config: precision must be 0, 1 or 3"); return SVCB_E_UNSUPPORTED; }
   if (c.n_ups < 1 || c.n_ups > SVCB_MAX_UPS || c.n_res < 1 || c.n_res > SVCB_MAX_RES) {
@@ -951,6 +1041,8 @@ size_t svcb_workspace_bytes(const svcb_model* m, int32_t B, int32_t T) {
   size_t peak = 0;
   {
     Ctx ctx; ctx.dry = true;
+    ctx.alloc<int>(ragged_lens_bytes(B) / sizeof(int));   // svcb_infer_ragged's lengths, int32 then int64 per rate
+    ctx.alloc<long long>((size_t)(m->cfg.n_ups + 1) * B);
     float* zp = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
     float* z = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
     const size_t mark = ctx.off;
@@ -1042,6 +1134,36 @@ int svcb_infer(const svcb_model* m, const float* ppg, const float* vec, const fl
   SVCB_TRY(run_flow(m, ctx, zp, len, spk, z, B, T));
   ctx.off = mark;
   return run_generator(m, ctx, spk, z, source, wave, B, T);
+}
+
+int svcb_infer_ragged(const svcb_model* m, const float* ppg, const float* vec, const float* pit, const float* spk,
+                      const int32_t* n_frames_host, const float* source, const float* eps, float* wave, int32_t B,
+                      int32_t T, void* ws, size_t ws_bytes, svcb_stream stream) {
+  g_launches = 0;
+  if (!m || B <= 0 || T <= 0 || !n_frames_host) { set_error("svcb_infer_ragged: bad shape or null lengths"); return SVCB_E_BAD_SHAPE; }
+  RaggedLens rl;
+  SVCB_TRY(rl.validate(n_frames_host, B, T, [](int n) { return n; }, "svcb_infer_ragged", "frames"));
+  SVCB_TRY(ragged_forms(m, n_frames_host, B, T, wave));
+  Ctx ctx;
+  SVCB_TRY(make_ctx(ctx, ws, ws_bytes, nullptr, stream));
+  const int rows = m->cfg.n_ups + 1;
+  int* lens = ctx.alloc<int>(ragged_lens_bytes(B) / sizeof(int));
+  long long* len64 = ctx.alloc<long long>((size_t)rows * B);
+  float* zp = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
+  float* z = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
+  SVCB_TRY(ctx.check());
+  SVCB_TRY(rl.stage(lens, ctx.stream));
+  StageRates f;
+  f.v[0] = 1;
+  for (int i = 0; i < m->cfg.n_ups; ++i) f.v[i + 1] = f.v[i] * m->cfg.up_rates[i];
+  stage_lens_kernel<<<(B * rows + 255) / 256, 256, 0, ctx.stream>>>(lens, len64, f, B, rows);
+  SVCB_LAUNCH_CHECK("stage_lens");
+  const size_t mark = ctx.off;
+  SVCB_TRY(run_prior(m, ctx, ppg, vec, pit, len64, eps, zp, B, T, true));
+  ctx.off = mark;
+  SVCB_TRY(run_flow(m, ctx, zp, len64, spk, z, B, T));
+  ctx.off = mark;
+  return run_generator(m, ctx, spk, z, source, wave, B, T, len64, lens, rl.min_out);
 }
 
 // ---- single-operator entry points

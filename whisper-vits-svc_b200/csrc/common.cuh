@@ -187,8 +187,9 @@ inline SnakeTapsV snake_taps_pack(const float* up12, const float* dn12) {
   return t;
 }
 bool post_fused_supported(int C, int L, int K, const float* x, const float* wave);
+// lens (device, may be null): a ragged batch, item b ending at lens[b] * lscale samples; its later samples of wave are zero
 int launch_post_fused(const float* x, float* wave, const float* ea, const float* inv_b, const SnakeTapsV& tp,
-                      const float* w_host, int B, int C, int L, cudaStream_t s);
+                      const float* w_host, int B, int C, int L, cudaStream_t s, const int* lens = nullptr, int lscale = 1);
 // device taps -> SnakeTapsV through a synchronous copy (unit-test entry points; the model keeps host copies)
 int snake_taps_from_device(const float* fu_dev, const float* fd_dev, SnakeTapsV* out);
 
@@ -335,8 +336,10 @@ int launch_amp_conv_tc(const AmpConvParams& p, cudaStream_t s);
 size_t amp_conv_tc_smem_bytes(int Cp, int K, int dil, int nsplit);
 // SnakeAlias(x[B,C,L]) -> bf16 hi (and lo, may be null) operand images
 // taps: host copy of the filter taps, or null (then read back from fu / fd with a synchronous copy: test entry points)
+// lens (device, may be null): a ragged batch, item b ending at lens[b] * lscale samples; its later image rows are zero
 int launch_snake_pack(const float* x, void* hi, void* lo, const float* ea, const float* inv_b, const float* fu,
-                      const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps = nullptr);
+                      const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps = nullptr,
+                      const int* lens = nullptr, int lscale = 1);
 size_t p8_image_bytes(int B, int C, int L);
 int p8_rows(int L);
 
@@ -358,6 +361,8 @@ struct AmpS2dParams {
   int ntaps = 0, mlo = 0;       // Toeplitz row offsets -mlo .. ntaps-1-mlo (pack.py:s2d_taps)
   int accum = 0;                // y = y_old + v
   float out_div = 0.f;          // then / out_div when != 0
+  const int* lens = nullptr;    // ragged batch: item b ends at lens[b] * lscale samples (a multiple of r), or null
+  int lscale = 1;
 };
 // Head-major QKV layout the Whisper attention kernel reads (written by the QKV GEMM's epilogue 4): per item
 // b, per w in {q, k, v}, per head h one block of Tp x 64 bf16 (Tp = T rounded up to 128 rows, pad rows zero);
@@ -371,7 +376,8 @@ __host__ __device__ inline size_t qkv_heads_off(int b, int w, int h, int t, int 
 }
 int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s);
 int launch_snake_pack_s2d(const float* x, void* hi, void* lo, const float* ea, const float* inv_b, const float* fu,
-                          const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps = nullptr);
+                          const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps = nullptr,
+                          const int* lens = nullptr, int lscale = 1);
 int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, int L, cudaStream_t s);
 int s2d_rows(int L, int r);
 size_t s2d_image_bytes(int B, int L, int r);
@@ -402,6 +408,8 @@ struct UpsFusedParams {
   int B = 0, Cin = 0, Cout = 0, L = 0, Ln = 0, rate = 0, M = 0, pad = 0, cout_pad = 0;
   int Kn = 0, sf = 1, padn = 0, cout_pad_n = 0;
   long long Ltot = 0;
+  const int* lens = nullptr;           // ragged batch: item b's source ends at lens[b] * src_scale samples, or null
+  int src_scale = 1;
 };
 int launch_ups_fused(const UpsFusedParams& p, cudaStream_t s);
 // lens (device, may be null): per-item sample counts of a ragged batch, each in [201, N]

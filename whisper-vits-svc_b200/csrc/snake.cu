@@ -90,12 +90,15 @@ struct PostTaps { float w[PF_MAXC][PF_K]; };
 
 __global__ void __launch_bounds__(PF_RUNS, 2)
 post_fused_kernel(const float* __restrict__ x, float* __restrict__ wave, const float* __restrict__ ea,
-                  const float* __restrict__ inv_b, const SnakeTapsV tp, const PostTaps pw, int C, int L) {
+                  const float* __restrict__ inv_b, const SnakeTapsV tp, const PostTaps pw, int C, int L,
+                  const int* __restrict__ lens, int lscale) {
   __shared__ __align__(16) float srow[2][PF_RUNS * 8];
   const int tid = threadIdx.x, b = blockIdx.y;
   const int n0 = blockIdx.x * (PF_OUT_RUNS * 8) - 8 + tid * 8;   // this thread's run of Snake values
-  const bool inside = n0 >= 0 && n0 < L;                          // outside the sequence: the conv's zero padding
-  const bool produces = tid >= 1 && tid <= PF_OUT_RUNS && inside;
+  const int Lb = lens ? __ldg(lens + b) * lscale : L;             // a ragged item's end (a multiple of 8)
+  const bool inside = n0 >= 0 && n0 < Lb;                         // outside the sequence: the conv's zero padding
+  const bool stores = tid >= 1 && tid <= PF_OUT_RUNS && n0 >= 0 && n0 < L;
+  const bool produces = stores && inside;
   float acc[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[i] = 0.f;
@@ -106,7 +109,7 @@ post_fused_kernel(const float* __restrict__ x, float* __restrict__ wave, const f
     if (inside) {
       const float* xr = x + ((long long)b * C + c) * L;
       float xw[24];
-      if (n0 - 8 >= 0 && n0 + 16 <= L) {
+      if (n0 - 8 >= 0 && n0 + 16 <= Lb) {
 #pragma unroll
         for (int q = 0; q < 6; ++q) {
           const float4 t4 = __ldg(reinterpret_cast<const float4*>(xr + n0 - 8) + q);
@@ -114,9 +117,9 @@ post_fused_kernel(const float* __restrict__ x, float* __restrict__ wave, const f
         }
       } else {   // replicate padding of x (alias/resample.py:28) = clamped loads
 #pragma unroll
-        for (int j = 0; j < 24; ++j) xw[j] = __ldg(xr + min(max(n0 - 8 + j, 0), L - 1));
+        for (int j = 0; j < 24; ++j) xw[j] = __ldg(xr + min(max(n0 - 8 + j, 0), Lb - 1));
       }
-      snake8_packed(xw, tp, __ldg(ea + c), 0.5f * __ldg(inv_b + c), v, n0 == 0, n0 + 8 == L);
+      snake8_packed(xw, tp, __ldg(ea + c), 0.5f * __ldg(inv_b + c), v, n0 == 0, n0 + 8 == Lb);
     }
     float* sr = srow[c & 1];
     *reinterpret_cast<float4*>(sr + tid * 8) = make_float4(v[0], v[1], v[2], v[3]);
@@ -138,6 +141,10 @@ post_fused_kernel(const float* __restrict__ x, float* __restrict__ wave, const f
     float* o = wave + (long long)b * L + n0;
     *reinterpret_cast<float4*>(o) = make_float4(tanhf(acc[0]), tanhf(acc[1]), tanhf(acc[2]), tanhf(acc[3]));
     *reinterpret_cast<float4*>(o + 4) = make_float4(tanhf(acc[4]), tanhf(acc[5]), tanhf(acc[6]), tanhf(acc[7]));
+  } else if (stores) {   // past a ragged item's end
+    float4* o = reinterpret_cast<float4*>(wave + (long long)b * L + n0);
+    o[0] = make_float4(0.f, 0.f, 0.f, 0.f);
+    o[1] = o[0];
   }
 }
 
@@ -147,7 +154,7 @@ bool post_fused_supported(int C, int L, int K, const float* x, const float* wave
 
 // w_host: the conv_post taps [C][7] on the host (out channel 0)
 int launch_post_fused(const float* x, float* wave, const float* ea, const float* inv_b, const SnakeTapsV& tp,
-                      const float* w_host, int B, int C, int L, cudaStream_t s) {
+                      const float* w_host, int B, int C, int L, cudaStream_t s, const int* lens, int lscale) {
   if (B <= 0 || L <= 0) return SVCB_OK;
   if (!post_fused_supported(C, L, PF_K, x, wave)) { set_error("post_fused: unsupported shape"); return SVCB_E_BAD_SHAPE; }
   PostTaps pw;
@@ -155,7 +162,7 @@ int launch_post_fused(const float* x, float* wave, const float* ea, const float*
     for (int k = 0; k < PF_K; ++k) pw.w[c][k] = c < C ? w_host[c * PF_K + k] : 0.f;
   dim3 grid((L / 8 + PF_OUT_RUNS - 1) / PF_OUT_RUNS, B);
   KernelScope ks("post_fused", s, 2.0 * PF_K * B * C * (double)L, 4.0 * B * (C + 1) * (double)L, 70.0 * B * C * (double)L);
-  post_fused_kernel<<<grid, PF_RUNS, 0, s>>>(x, wave, ea, inv_b, tp, pw, C, L);
+  post_fused_kernel<<<grid, PF_RUNS, 0, s>>>(x, wave, ea, inv_b, tp, pw, C, L, lens, lscale);
   SVCB_LAUNCH_CHECK("post_fused");
   return SVCB_OK;
 }

@@ -69,6 +69,7 @@ ups_fused_kernel(const UpsFusedParams p) {
       }
   }
   const float* sb = p.src + (long long)b * p.Ltot;
+  const long long nsrc = p.lens ? (long long)__ldg(p.lens + b) * p.src_scale : p.Ltot;   // a ragged item's source end
   float* yb = p.y + (long long)b * COUT * p.Ln;
 #pragma unroll
   for (int r = 0; r < RATE; ++r) {
@@ -76,7 +77,7 @@ ups_fused_kernel(const UpsFusedParams p) {
     if (n >= 0 && n < p.Ln) {
       for (int j = 0; j < p.Kn; ++j) {
         const long long si = (long long)n * p.sf + j - p.padn;
-        const float sv = (si >= 0 && si < p.Ltot) ? __ldg(sb + si) : 0.f;
+        const float sv = (si >= 0 && si < nsrc) ? __ldg(sb + si) : 0.f;
 #pragma unroll
         for (int co = 0; co < COUT; ++co) acc[r][co] = fmaf(sv, wns[j * CP + co], acc[r][co]);
       }

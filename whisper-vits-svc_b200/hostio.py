@@ -143,22 +143,34 @@ class BatchEngine:
     rank"; the reference runs one subprocess and batch-1 device calls per file, svc_inference_batch.py:39-43).
 
     Every utterance is cut by the reference's own chunk plan (svc_inference.py:101-131: 2500-frame chunks, +-10
-    frames of discarded overlap); chunks of ALL queued utterances are bucketed by exact length and run up to
-    `max_batch` at a time.  Only equal-length chunks share a batch: SnakeAlias pads by replication at the true
-    end of a chunk, so a chunk padded to a longer neighbour would differ from the reference's batch-1 result
-    in its last few hundred samples.  Host->device copies of the next batch and the device->host copy of the
-    previous result run on side streams and overlap the current batch's kernels.
+    frames of discarded overlap) and the chunks of ALL queued utterances run up to `max_batch` at a time.
+    Host->device copies of the next batch and the device->host copy of the previous result run on side streams and
+    overlap the current batch's kernels.
 
-        eng = BatchEngine(model, hp, device)
+    ragged=False (plan): only equal-length chunks share a batch.  The model's `inference` pads by replication and
+    convolves with zero padding at the end of the batch, so a chunk padded to a longer neighbour would differ from
+    the reference's batch-1 result in its last few hundred samples.  On real data almost every chunk has its own
+    length, so this runs about one chunk per call.
+    ragged=True (plan_ragged): chunks sorted by length, longest first, fill every batch, through the model's
+    `inference_ragged` (precision 3), which gives each chunk bitwise what a lone call of its own length gives.
+    The NSF sources of whole utterances come from padded `pitch2source` calls over groups of utterances sorted by
+    length; the source scan is causal, so each utterance's prefix is its lone source.
+
+        eng = BatchEngine(model, hp, device, ragged=True)
         for key, wave in eng.run(jobs):      # jobs: iterable of (key, spk, pit, ppg, vec) CPU tensors
             ...                              # wave: float32 numpy array of n_frames*hop - 1 samples
     """
 
-    def __init__(self, model, hp, device, max_batch: int = 32, window: int = 128):
+    # padded frames per padded pitch2source call: its [B, T*hop, n_harmonics] noise draw is 3.5 KB per frame
+    SOURCE_FRAMES = 32 * 2520
+
+    def __init__(self, model, hp, device, max_batch: int = 32, window: int = 128, ragged: bool = False):
         self.model, self.hp, self.device = model, hp, torch.device(device)
         self.max_batch, self.window = int(max_batch), int(window)
+        self.ragged = bool(ragged)
         self.hop = int(hp.data.hop_length)
         self.device_seconds = 0.0          # time spent inside device batches (CUDA events)
+        self.batches = 0                   # device batches (model inference calls)
         self.samples = 0
         self._events = []
         self._pinned = {}
@@ -183,6 +195,28 @@ class BatchEngine:
                 batches.append(idx[g0:g0 + max_batch])
         return chunks, batches
 
+    @staticmethod
+    def plan_ragged(lengths: Sequence[int], hop: int, max_batch: int):
+        """The chunks of plan(); batches = runs of up to max_batch chunks of any length, longest first (so a
+        batch pads its chunks to its first one's length, and lengths never increase from one batch to the next)."""
+        chunks, _ = BatchEngine.plan(lengths, hop, max_batch)
+        order = sorted(range(len(chunks)), key=lambda j: chunks[j][1] - chunks[j][2])   # stable: by length, descending
+        return chunks, [order[g0:g0 + max_batch] for g0 in range(0, len(order), max_batch)]
+
+    @staticmethod
+    def source_groups(lengths: Sequence[int], max_batch: int, max_frames: int):
+        """Utterance indices in groups for padded pitch2source calls: sorted by length, longest first, at most
+        max_batch per group and at most max_frames padded frames (a longer utterance gets a group of its own)."""
+        order = sorted(range(len(lengths)), key=lambda u: -int(lengths[u]))
+        groups = []
+        for u in order:
+            g = groups[-1] if groups else None
+            if g is None or len(g) == max_batch or (len(g) + 1) * int(lengths[g[0]]) > max_frames:
+                groups.append([u])
+            else:
+                g.append(u)
+        return groups
+
     def run(self, jobs):
         win = []
         for job in jobs:
@@ -203,18 +237,24 @@ class BatchEngine:
             n = min(pit.size(0), vec.size(0), ppg.size(0))       # svc_inference.py:78-81
             feats.append((key, spk, pit[:n], ppg[:n], vec[:n], n))
         lengths = [f[5] for f in feats]
-        chunks, batches = self.plan(lengths, hop, self.max_batch)
-        # NSF source of whole utterances (svc_inference.py:89-91), equal-length utterances in one call
+        chunks, batches = (self.plan_ragged if self.ragged else self.plan)(lengths, hop, self.max_batch)
+        # NSF source of whole utterances (svc_inference.py:89-91): equal-length utterances in one call, or (ragged)
+        # groups of any length padded with unvoiced frames, each utterance keeping its own prefix
         source = [None] * len(feats)
-        by_n = {}
-        for u, n in enumerate(lengths):
-            by_n.setdefault(n, []).append(u)
-        for n, us in by_n.items():
-            for g0 in range(0, len(us), self.max_batch):
-                grp = us[g0:g0 + self.max_batch]
-                src = model.pitch2source(torch.stack([feats[u][2] for u in grp]).to(dev, non_blocking=True))
-                for k, u in enumerate(grp):
-                    source[u] = src[k:k + 1]
+        if self.ragged:
+            groups = self.source_groups(lengths, self.max_batch, self.SOURCE_FRAMES)
+        else:
+            by_n = {}
+            for u, n in enumerate(lengths):
+                by_n.setdefault(n, []).append(u)
+            groups = [us[g0:g0 + self.max_batch] for us in by_n.values() for g0 in range(0, len(us), self.max_batch)]
+        for grp in groups:
+            f0 = torch.zeros(len(grp), lengths[grp[0]])
+            for k, u in enumerate(grp):
+                f0[k, :lengths[u]] = feats[u][2]
+            src = model.pitch2source(f0.to(dev, non_blocking=True))
+            for k, u in enumerate(grp):
+                source[u] = src[k:k + 1, :, :lengths[u] * hop]
         pieces = {u: [] for u in range(len(feats))}
 
         def pinned(name, slot, shape, dtype=torch.float32):
@@ -234,14 +274,14 @@ class BatchEngine:
             slot = bi & 1
             if h2d_done[slot] is not None:
                 h2d_done[slot].synchronize()          # the copy that last read this pinned set has finished
-            n = chunks[idx[0]][2] - chunks[idx[0]][1]
+            n = chunks[idx[0]][2] - chunks[idx[0]][1]    # (ragged: the longest; rows past a chunk's end are don't-care)
             B = len(idx)
             host = {"ppg": pinned("ppg", slot, (B, n, feats[0][3].shape[1])), "vec": pinned("vec", slot, (B, n, feats[0][4].shape[1])),
                     "pit": pinned("pit", slot, (B, n)), "spk": pinned("spk", slot, (B, feats[0][1].shape[0]))}
             for b, j in enumerate(idx):
                 u, cs, ce = chunks[j][0], chunks[j][1], chunks[j][2]
-                host["ppg"][b].copy_(feats[u][3][cs:ce]); host["vec"][b].copy_(feats[u][4][cs:ce])
-                host["pit"][b].copy_(feats[u][2][cs:ce]); host["spk"][b].copy_(feats[u][1])
+                host["ppg"][b, :ce - cs].copy_(feats[u][3][cs:ce]); host["vec"][b, :ce - cs].copy_(feats[u][4][cs:ce])
+                host["pit"][b, :ce - cs].copy_(feats[u][2][cs:ce]); host["spk"][b].copy_(feats[u][1])
             with torch.cuda.stream(copy_s):
                 d = {k: v.to(dev, non_blocking=True) for k, v in host.items()}
                 d["len"] = torch.full((B,), n, dtype=torch.int64, device=dev)
@@ -255,7 +295,7 @@ class BatchEngine:
             arr = res.numpy()
             for b, j in enumerate(batches[bi]):
                 u, cs, ce, so, eo = chunks[j]
-                pieces[u].append((cs, arr[b][so:eo].copy()))
+                pieces[u].append((cs, arr[b][:(ce - cs) * hop][so:eo].copy()))
 
         prev = None    # (batch index, pinned result, event) still in flight
         nxt = stage(0) if batches else None
@@ -265,13 +305,23 @@ class BatchEngine:
             if bi + 1 < len(batches):
                 nxt = stage(bi + 1)
             idx = batches[bi]
-            har = torch.cat([source[chunks[j][0]][:, :, chunks[j][1] * hop:chunks[j][2] * hop] for j in idx], 0)
+            if self.ragged:
+                n_frames = [chunks[j][2] - chunks[j][1] for j in idx]
+                har = torch.zeros(len(idx), 1, n_frames[0] * hop, device=dev)
+                for b, j in enumerate(idx):
+                    har[b, :, :n_frames[b] * hop] = source[chunks[j][0]][0, :, chunks[j][1] * hop:chunks[j][2] * hop]
+            else:
+                har = torch.cat([source[chunks[j][0]][:, :, chunks[j][1] * hop:chunks[j][2] * hop] for j in idx], 0)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(cur)
             for t in d.values():
                 t.record_stream(cur)
-            w = model.inference(d["ppg"], d["vec"], d["pit"], d["spk"], d["len"], har)
+            if self.ragged:
+                w = model.inference_ragged(d["ppg"], d["vec"], d["pit"], d["spk"], n_frames, har)
+            else:
+                w = model.inference(d["ppg"], d["vec"], d["pit"], d["spk"], d["len"], har)
             e1.record(cur)
+            self.batches += 1
             self._events.append((e0, e1))
             if prev is not None:
                 collect(*prev)                        # (its result buffer is the other slot)

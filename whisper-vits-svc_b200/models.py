@@ -166,6 +166,32 @@ class SynthesizerInfer(torch.nn.Module):
                           self._taps(taps))
         return wave
 
+    @torch.no_grad()
+    def inference_ragged(self, ppg, vec, pit, spk, n_frames, source, eps=None):
+        """`inference` for a batch of chunks of different lengths, padded to T (svcb_infer_ragged, precision 3).
+        ppg [B,T,ppg_dim], vec [B,T,vec_dim], pit [B,T], spk [B,spk_dim], n_frames: B host ints in 1..T,
+        source [B,1,T*hop], eps [B,inter_channels,T] or None -> wave [B,1,T*hop].  Item b is the first n_frames[b]
+        frames (n_frames[b]*hop source samples); its padding never reaches its result.  Its first n_frames[b]*hop
+        samples are bitwise those of a lone `inference` of it (T = ppg_l = n_frames[b]), the rest are zero."""
+        self._ensure()
+        dev = self._handle.device
+        ppg, vec, pit, spk, source = map(self._f32, (ppg, vec, pit, spk, source))
+        B, T, _ = ppg.shape
+        C = self._cfg["inter_channels"]
+        n = [int(v) for v in n_frames]
+        if eps is None:
+            eps = torch.randn(B, C, T, device=dev)
+        eps = self._f32(eps)
+        assert len(n) == B, "one length per item"
+        assert vec.shape[:2] == (B, T) and pit.shape == (B, T) and spk.shape[0] == B
+        assert source.shape == (B, 1, T * self.hop) and eps.shape == (B, C, T)
+        wave = torch.empty(B, 1, T * self.hop, device=dev, dtype=torch.float32)
+        ws = self._workspace(B, T)
+        self._handle.call("infer_ragged", ppg.data_ptr(), vec.data_ptr(), pit.data_ptr(), spk.data_ptr(),
+                          (ctypes.c_int32 * B)(*n), source.data_ptr(), eps.data_ptr(), wave.data_ptr(), B, T,
+                          ws.data_ptr(), ws.numel())
+        return wave
+
     # ---- stage entry points (parity tests, profiling) ---------------------------------------
     @torch.no_grad()
     def prior(self, ppg, vec, pit, ppg_l, eps, taps=None):
