@@ -1,0 +1,111 @@
+#!/usr/bin/env python
+"""The space-to-depth AMP links of generator stages 2-4 (csrc/amp_s2d.cu) at B = 32, T = 1000, one shape at a time
+through ops.amp_s2d_link.  A shape is (C, k, dilation, Snake output or not, residual or not); the step runs 54
+links over 15 distinct shapes per stage, each c1 link without a residual, each c2 link with one, every link but a
+block's last with the next SnakeAlias in its epilogue.  Every shape is also timed without the Snake output: that
+link is the MMA side plus a plain fp32 store, so the difference is what the Snake epilogue costs.
+
+ops.amp_s2d_link also clears the images, runs snake_pack_s2d and unpacks the output image; only the
+`amp_s2d_link_*` launches are counted (svcb_timing_enable / svcb_timing_report: CUDA events around each launch).
+ops.amp_s2d_link always writes the fp32 result, which the step's c1 links do not.
+
+Prints one JSON line: the card, its power limit and max SM clock (read in the same run) and, per shape, ms per
+launch, the launches per step, and the tensor work's share of the 989 TFLOP/s dense bf16 data-sheet peak (3 bf16
+products per tap and tile row, halo rows included).
+
+    python scripts/bench_s2d_link.py [--batch 32] [--frames 1000] [--iters 20]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import torch  # noqa: E402
+
+PEAK_BF16 = 989e12
+STAGES = [(40, 80), (20, 160), (10, 320)]   # (C, samples per frame) of generator stages 2-4
+KERNELS = (3, 7, 11)
+DILATIONS = (1, 3, 5)
+
+
+def gpu_info():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                        "-i", str(torch.cuda.current_device())], capture_output=True, text=True, check=True).stdout
+    name, pl, clk = [s.strip() for s in q.strip().splitlines()[0].split(",")]
+    return name, float(pl), float(clk)
+
+
+def link_ms(lib, call, iters):
+    """Summed duration and count of the amp_s2d_link_* launches of `iters` calls."""
+    lib.svcb_timing_enable(1)
+    for _ in range(iters):
+        call()
+    torch.cuda.synchronize()
+    rep = lib.svcb_timing_report().decode()
+    lib.svcb_timing_enable(0)
+    ms, n = 0.0, 0
+    for line in rep.strip().splitlines():
+        f = line.split()
+        if f[0].startswith("amp_s2d_link_"):
+            n += int(f[1]); ms += float(f[2])
+    assert n == iters, (n, iters, rep)
+    return ms / n
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--frames", type=int, default=1000)
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=2)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("bench_s2d_link.py needs a CUDA device")
+    from whisper_vits_svc_b200 import _lib, ops, pack
+    lib = _lib.load()
+    name, power, clk = gpu_info()
+    B = args.batch
+    g = torch.Generator().manual_seed(0)
+    gd = torch.Generator(device="cuda").manual_seed(0)
+    fu = (torch.randn(12, generator=g) * 0.1).cuda()
+    fd = (torch.randn(12, generator=g) * 0.1).cuda()
+    rows = []
+    for C, up in STAGES:
+        L = args.frames * up
+        r = pack.s2d_factor(C)
+        S = 128 - 2 * (1 if r >= 8 else 2)
+        ntiles = B * ((L // r + S - 1) // S)
+        x = torch.randn(B, C, L, device="cuda", generator=gd)
+        res = torch.randn(B, C, L, device="cuda", generator=gd)
+        a_in, b_in, a_out, b_out = (torch.randn(C, generator=g) * 0.3 for _ in range(4))
+        bias = (torch.randn(C, generator=g) * 0.1).cuda()
+        for k in KERNELS:
+            # (dilation, residual, launches per step with Snake output, without)
+            shapes = [(d, False, 1, 0) for d in DILATIONS] + [(1, True, 2, 1)]
+            for d, with_res, n_snake, n_plain in shapes:
+                w = torch.randn(C, C, k, generator=g) / (C * k) ** 0.5
+                mlo, mhi = pack.s2d_taps(k, d, r)
+                for snake, per_step in ((True, n_snake), (False, n_plain)):
+                    def call():
+                        ops.amp_s2d_link(x, a_in, b_in, fu, fd, w, bias, dilation=d, res=res if with_res else None,
+                                         alpha_out=a_out if snake else None, beta_out=b_out if snake else None)
+
+                    for _ in range(args.warmup):
+                        call()
+                    ms = link_ms(lib, call, args.iters)
+                    tensor_flop = 3 * 2.0 * 160 * 160 * (mlo + mhi + 1) * ntiles * 128
+                    rows.append({"C": C, "r": r, "k": k, "dilation": d, "ntaps": mlo + mhi + 1, "snake": snake,
+                                 "res": with_res, "launches_per_step": per_step, "ms": round(ms, 4),
+                                 "tensor_share_of_peak": round(tensor_flop / (ms * 1e-3) / PEAK_BF16, 3)})
+        del x, res
+        torch.cuda.empty_cache()
+    print(json.dumps({"gpu": name, "power_limit_w": power, "max_sm_clock_mhz": clk, "batch": B, "frames": args.frames,
+                      "iters": args.iters, "launches_per_step": sum(r["launches_per_step"] for r in rows),
+                      "family_ms_per_step": round(sum(r["ms"] * r["launches_per_step"] for r in rows), 3),
+                      "shapes": rows}))
+
+
+if __name__ == "__main__":
+    main()

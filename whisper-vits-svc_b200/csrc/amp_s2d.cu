@@ -46,8 +46,8 @@ constexpr uint32_t SMEM = 2 * A_PART + 2 * W_SLOT + STG_BYTES;
 static_assert(SMEM + 1024 <= 227 * 1024, "A panel + weight ring + strips must fit the 227 KB of one CTA");
 constexpr int EPI_WARPS = 4 * GROUPS;
 constexpr int THREADS = (EPI_WARPS + 1) * 32;
-constexpr int ACC_LD = N + 4;                   // floats per row of the staged accumulator (over the A panel)
-static_assert(TILE * ACC_LD * 4 <= 2 * A_PART, "the staged accumulator must fit over the A panel");
+constexpr int ACC_LD = N + 4;                   // floats per row of the staged accumulator (over the weight ring)
+static_assert(TILE * ACC_LD * 4 <= 2 * W_SLOT, "the staged accumulator must fit over the weight ring");
 }  // namespace s2d
 
 int s2d_halo_rows(int r) { return r >= 8 ? 1 : 2; }                 // SnakeAlias reaches +-5 samples
@@ -163,9 +163,12 @@ int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, in
 // ------------------------------------------------------------------------------------------------ link
 // Persistent: every CTA walks tiles (item, 126 useful rows) with a static stride.
 //   producer warp  A panel of the tile (40 bulk copies) and the (tap, hi|lo) weight matrices through a
-//                  2-slot ring (four bulk copies each)
+//                  2-slot ring (four bulk copies each).  The next tile's A panel is requested as soon as this
+//                  tile's MMAs retire (a_empty), so it loads under this tile's epilogue; its weights wait for
+//                  the epilogue to release the ring (ring_free)
 //   warpgroups 0-1 per tap: A_hi x W_hi, A_lo x W_hi, A_hi x W_lo — 30 wgmma m64n160k16 each for its 64 rows,
-//                  register accumulators, then staged as fp32 rows over the (consumed) A panel
+//                  register accumulators (the 10-20 wgmma of one matrix form one commit group), then staged
+//                  as fp32 rows over the (consumed) weight ring
 //   12 epilogue warps = 3 column groups x 4 row quadrants: group g owns units u = g (mod 3), a unit
 //                  being one channel (r >= 8) or a channel pair (r = 4): 6-7 / 6-7 / 3-4 units per group for
 //                  C = 20 / 40 / 10 (13 warps leave the MMA warpgroups the registers of 160 accumulator columns)
@@ -175,7 +178,7 @@ __global__ void __launch_bounds__(s2d::THREADS, 1)
 amp_s2d_link_kernel(const AmpS2dParams p) {
   using namespace s2d;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t a_full, a_empty, w_full[2], w_empty[2];
+  __shared__ __align__(8) uint64_t a_full, a_empty, ring_free, w_full[2], w_empty[2];
   __shared__ float s_par[3][40];      // bias | exp(alpha) | 1 / (exp(beta) + 1e-9) of every channel (C <= 40)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -193,10 +196,10 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
   uint8_t* Abase = smem;
   uint8_t* Wbase = smem + 2 * A_PART;
   float* Stg = reinterpret_cast<float*>(smem + 2 * A_PART + 2 * W_SLOT);
-  float* Acc = reinterpret_cast<float*>(smem);   // staged accumulator [TILE][ACC_LD], over the A panel
+  float* Acc = reinterpret_cast<float*>(Wbase);  // staged accumulator [TILE][ACC_LD], over the weight ring
 
   if (tid == 0) {
-    tc::mbar_init(&a_full, 1); tc::mbar_init(&a_empty, 1);
+    tc::mbar_init(&a_full, 1); tc::mbar_init(&a_empty, 1); tc::mbar_init(&ring_free, 1);
     for (int i = 0; i < 2; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 2); }
     tc::fence_barrier_init();
   }
@@ -210,12 +213,15 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
         const int b = tile / tpi, t = tile - b * tpi;
         const long long row0 = (long long)t * S - HS - A_OFF + PADR;     // image row of A-panel row 0 (>= 6)
+        // the A panel is free once the previous tile's MMAs have retired: its copies run under that tile's
+        // epilogue; the ring holds that epilogue's staged accumulator until the epilogue has read it
         if (it >= 1) tc::mbar_wait_parked(&a_empty, (uint32_t)((it - 1) & 1));
         tc::mbar_arrive_expect_tx(&a_full, 2 * A_PART);
         for (int part = 0; part < 2; ++part)
           for (int kc = 0; kc < KC; ++kc)
             tc::bulk_g2s(Abase + (size_t)part * A_PART + (size_t)kc * RA * 16,
                          img[part] + ((((long long)b * KC + kc) * p.Rp) + row0) * 16, RA * 16, &a_full);
+        if (it >= 1) tc::mbar_wait_parked(&ring_free, (uint32_t)((it - 1) & 1));
         for (int c = 0; c < 2 * p.ntaps; ++c, ++wi) {
           const int st = wi & 1;
           if (wi >= 2) tc::mbar_wait_parked(&w_empty[st], (uint32_t)(((wi >> 1) - 1) & 1));
@@ -233,7 +239,8 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
     // ------------------------------------------------------------------------------------ epilogue
     const int q = warp & 3, g = warp >> 2;
     const int row = q * 32 + lane;
-    const int wg = warp >> 2, tw = tid & 127;
+    // warp_u, not warp: ptxas must see the MMA branch (wg < 2) as warp-uniform, or it serialises every wgmma
+    const int wg = warp_u >> 2, tw = tid & 127;
     constexpr uint32_t LBO_A = RA * 16, LBO_B = N * 16;
     constexpr uint64_t KSA = (2 * LBO_A) >> 4, KSB = (2 * LBO_B) >> 4;      // descriptor step per K = 16
     const uint32_t a_h0 = tc::smem_u32(Abase) + (uint32_t)wg * 64u * 16u, a_l0 = a_h0 + A_PART, w_s0 = tc::smem_u32(Wbase);
@@ -278,6 +285,7 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const uint32_t arow_off = (uint32_t)(A_OFF - p.mlo + tap) * 16u;   // row shift
           const uint64_t ah = tc::smem_desc(a_h0 + arow_off, LBO_A), al = tc::smem_desc(a_l0 + arow_off, LBO_A);
+#pragma unroll   // part is a constant: each matrix is one branch-free commit group
           for (int part = 0; part < 2; ++part, ++wi) {   // W_hi: A_hi x W_hi, A_lo x W_hi;  W_lo: A_hi x W_lo
             const int st = wi & 1;
             tc::mbar_wait_parked(&w_full[st], (uint32_t)((wi >> 1) & 1));
@@ -290,12 +298,16 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
               for (int kk = 0; kk < N / 16; ++kk) tc::Wg<N, 0>::ss(acc, al + kk * KSA, bw + kk * KSB, 1u);
             }
             tc::wg_commit();
+            // drain before the next matrix: the ring is fed from L2 about as fast as the MMAs consume it, so
+            // the slot is released the moment its MMAs retire (releasing it one matrix later, under
+            // wgmma.wait_group 1, made the links 2-33 % slower on an H100 SXM at 700 W)
             tc::wg_wait<0>();
             if (tw == 0) tc::mbar_arrive(&w_empty[st]);
           }
         }
         tc::wg_hold(acc);
-        tc::named_sync(6, 256);                   // both warpgroups' MMAs are done: the A panel is free
+        tc::named_sync(6, 256);                   // both warpgroups' MMAs have retired: A panel and ring are free
+        if (tid == 0) tc::mbar_arrive(&a_empty);
         tc::acc_to_smem<N>(acc, Acc + wg * 64 * ACC_LD, ACC_LD, 0, N / 8);
       }
       tc::named_sync(7, EPI_WARPS * 32);          // accumulator rows staged
@@ -473,9 +485,9 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
           }
         }
       }
-      tc::fence_proxy_async_smem();               // staged rows (generic proxy) -> the next tile's bulk copies
+      tc::fence_proxy_async_smem();               // staged rows (generic proxy) -> the next tile's weight copies
       tc::named_sync(7, EPI_WARPS * 32);
-      if (tid == 0) tc::mbar_arrive(&a_empty);
+      if (tid == 0) tc::mbar_arrive(&ring_free);
     }
   }
 }
