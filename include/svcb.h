@@ -446,7 +446,8 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
  * generator stages (C = 20 or 10; vits_decoder/bigv.py:50-58) in space-to-depth form (csrc/amp_s2d.cu):
  * snake_pack_s2d, then the block-Toeplitz wgmma convolution whose epilogue writes y (fp32, may be NULL)
  * and — when y_act != NULL — SnakeAlias_out(result) as the next link's bf16 hi/lo operand image, returned
- * here decoded to fp32 [B,C,L].  w_s2d = pack.py:pack_conv_s2d image; L % (160/C) == 0. */
+ * here decoded to fp32 [B,C,L].  w_s2d = pack.py:pack_conv_s2d_slots image (output columns in the kernel's
+ * phase-slot order); L % (160/C) == 0. */
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L);
 int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                          const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,

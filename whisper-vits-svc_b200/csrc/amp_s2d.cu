@@ -42,12 +42,16 @@ constexpr int GROUPS = 3;                       // epilogue column groups (x 4 r
 constexpr int STRIP = TILE * 8;                 // floats of one group's strip: 128 rows x (first 4 | last 4 samples) of one channel,
                                                 // or 128 rows x 4 samples of two channels (r = 4)
 constexpr uint32_t STG_BYTES = 64 + GROUPS * STRIP * 4 + 64 + GROUPS * 128 * 4;  // sample strips (+ guards) + edge buffers
-constexpr uint32_t SMEM = 2 * A_PART + 2 * W_SLOT + STG_BYTES;
-static_assert(SMEM + 1024 <= 227 * 1024, "A panel + weight ring + strips must fit the 227 KB of one CTA");
+constexpr uint32_t RES_W = 20 * 40 * 16;       // 12,800 B: the first tap's W_hi over its 40 reached columns, packed
+constexpr uint32_t SMEM = 2 * A_PART + 2 * W_SLOT + STG_BYTES + RES_W;
+static_assert(SMEM + 1024 <= 227 * 1024, "A panel + weight ring + strips + resident matrix must fit the 227 KB of one CTA");
 constexpr int EPI_WARPS = 4 * GROUPS;
 constexpr int THREADS = (EPI_WARPS + 1) * 32;
 constexpr int ACC_LD = N + 4;                   // floats per row of the staged accumulator (over the weight ring)
 static_assert(TILE * ACC_LD * 4 <= 2 * W_SLOT, "the staged accumulator must fit over the weight ring");
+constexpr uint32_t LBO_A = RA * 16, LBO_B = N * 16;
+constexpr uint64_t KSA = (2 * LBO_A) >> 4;      // A descriptor step per K = 16
+constexpr int GCOLS = N / 4;                    // output columns of one phase group
 }  // namespace s2d
 
 int s2d_halo_rows(int r) { return r >= 8 ? 1 : 2; }                 // SnakeAlias reaches +-5 samples
@@ -57,6 +61,26 @@ int s2d_rows(int L, int r) {                                         // Rp of an
   return ((nrows + S - 1) / S) * S + 160;
 }
 size_t s2d_image_bytes(int B, int L, int r) { return (size_t)B * s2d::KC * s2d_rows(L, r) * 16; }
+
+// Output columns of the weights and the accumulator come in four slots of 40, n = 40 s + g c + j: slot s holds
+// the g = r / 4 phases p = g q + j of every channel c of phase group q = {0, 1, 3, 2}[s] (pack.py:
+// s2d_column_order).  Row tap m reaches the phases [max(0, r m - P), min(r - 1, r m + r - 1 + P)] only, so the
+// matrix of an edge tap is zero outside the groups {0}, {0, 1} (m < 0) or {3}, {3, 2} (m > 0), that is outside
+// columns [0, 40), [0, 80), [80, 120) or [80, 160).  Per tap 3 bits: code 1-4 = those ranges, 0 = all columns.
+bool s2d_tap_plan(int k, int dil, int r, int& mlo, int& ntaps, uint64_t& tap_cols) {
+  const int P = dil * (k - 1) / 2, g = r / 4;
+  mlo = (P + r - 1) / r;
+  ntaps = mlo + (r - 1 + P) / r + 1;
+  tap_cols = 0;
+  if (g < 1 || ntaps > 21) return false;
+  for (int t = 0; t < ntaps; ++t) {
+    const int m = t - mlo;
+    const int q0 = std::max(0, r * m - P) / g, q1 = std::min(r - 1, r * m + r - 1 + P) / g;
+    const int code = q0 == 0 && q1 <= 1 ? 1 + q1 : q1 == 3 && q0 >= 2 ? 3 + (3 - q0) : 0;
+    tap_cols |= (uint64_t)code << (3 * t);
+  }
+  return true;
+}
 
 __device__ __forceinline__ void s2d_store_octet(__nv_bfloat16* hi, __nv_bfloat16* lo, long long row_elem,
                                                 const float (&o)[8]) {
@@ -161,24 +185,95 @@ int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, in
 }
 
 // ------------------------------------------------------------------------------------------------ link
+// One (tap, hi|lo) matrix over the output columns [N0, N0 + W) it reaches: the accumulator registers of those
+// columns (4j .. 4j+3 hold columns 8j .. 8j+7) and the B panel from its row N0 (16 B = one descriptor unit).
+// The skipped products are exact zeros, so every output sums the same products in the same order as at W = 160.
+// LB: bytes between the K-chunks of the B panel (LBO_B in the ring; W * 16 for a matrix packed to its columns).
+template <int W, int N0, bool ALO, uint32_t LB = s2d::LBO_B>
+__device__ __forceinline__ void s2d_mma(float (&acc)[s2d::N / 2], uint64_t ah, uint64_t al, uint64_t bw) {
+  using namespace s2d;
+  constexpr uint64_t KS = (2 * LB) >> 4;
+  float(&d)[W / 2] = *reinterpret_cast<float(*)[W / 2]>(acc + N0 / 2);
+#pragma unroll
+  for (int kk = 0; kk < N / 16; ++kk) tc::Wg<W, 0>::ss(d, ah + kk * KSA, bw + N0 + kk * KS, 1u);
+  if constexpr (ALO) {
+#pragma unroll
+    for (int kk = 0; kk < N / 16; ++kk) tc::Wg<W, 0>::ss(d, al + kk * KSA, bw + N0 + kk * KS, 1u);
+  }
+}
+// The accumulator is two independent 80-column halves, lower (slots 0, 1) and upper (slots 2, 3), each of which
+// a wgmma only ever addresses from its first register: ptxas serialises every wgmma of the kernel once one of
+// them starts inside another's register range.  `code` (s2d_tap_plan) is warp-uniform.
+// TRIM = false (a link without edge taps to trim): one m64n160 over the whole accumulator per K step.
+template <bool ALO, bool TRIM>
+__device__ __forceinline__ void s2d_mma_tap(float (&acc)[s2d::N / 2], uint64_t ah, uint64_t al, uint64_t bw, int code) {
+  if constexpr (!TRIM) {
+    s2d_mma<s2d::N, 0, ALO>(acc, ah, al, bw);
+    return;
+  }
+  switch (code) {
+    case 1: s2d_mma<40, 0, ALO>(acc, ah, al, bw); break;
+    case 2: s2d_mma<80, 0, ALO>(acc, ah, al, bw); break;
+    case 3: s2d_mma<40, 80, ALO>(acc, ah, al, bw); break;
+    case 4: s2d_mma<80, 80, ALO>(acc, ah, al, bw); break;
+    default: s2d_mma<80, 0, ALO>(acc, ah, al, bw); s2d_mma<80, 80, ALO>(acc, ah, al, bw); break;
+  }
+}
+
+// Accumulator fragment (64 rows x 160 columns in slot order, see s2d_tap_plan; phase p = g q + j, g = R / 4) ->
+// rows buf[row * ACC_LD + c * R + p] in the channel-major order the epilogue reads.  A thread holds the columns
+// 8 i + 2 (l & 3) + {0, 1}, i = 5 s + i5, of rows rr and rr + 8: for R = 4 and 8 these are all R phases of its
+// channels (float4 runs), for R = 16 pairs of phases (float2).  With the row stride of 164 floats (+4 banks per
+// row) every store is free of bank conflicts.
+template <int R>
+__device__ __forceinline__ void s2d_stage_acc(const float (&d)[s2d::N / 2], float* buf) {
+  using namespace s2d;
+  const int t = threadIdx.x & 127, lq = t & 3;
+  const int rr = 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* row = buf + (rr + 8 * h) * ACC_LD;
+#pragma unroll
+    for (int i5 = 0; i5 < 5; ++i5) {
+      auto a = [&](int q, int e) { return d[4 * (5 * (q < 2 ? q : 5 - q) + i5) + 2 * h + e]; };   // group q, slot s
+      if constexpr (R == 4) {          // channel 8 i5 + 2 lq + e, phase q
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          *reinterpret_cast<float4*>(row + 4 * (8 * i5 + 2 * lq + e)) = make_float4(a(0, e), a(1, e), a(2, e), a(3, e));
+      } else if constexpr (R == 8) {   // channel 4 i5 + lq, phase 2 q + e
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+          *reinterpret_cast<float4*>(row + 8 * (4 * i5 + lq) + 4 * hh) =
+              make_float4(a(2 * hh, 0), a(2 * hh, 1), a(2 * hh + 1, 0), a(2 * hh + 1, 1));
+      } else {                         // channel 2 i5 + lq / 2, phase 4 q + 2 (lq & 1) + e
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          *reinterpret_cast<float2*>(row + 16 * (2 * i5 + (lq >> 1)) + 4 * q + 2 * (lq & 1)) = make_float2(a(q, 0), a(q, 1));
+      }
+    }
+  }
+}
+
 // Persistent: every CTA walks tiles (item, 126 useful rows) with a static stride.
 //   producer warp  A panel of the tile (40 bulk copies) and the (tap, hi|lo) weight matrices through a
-//                  2-slot ring (four bulk copies each).  The next tile's A panel is requested as soon as this
-//                  tile's MMAs retire (a_empty), so it loads under this tile's epilogue; its weights wait for
-//                  the epilogue to release the ring (ring_free)
-//   warpgroups 0-1 per tap: A_hi x W_hi, A_lo x W_hi, A_hi x W_lo — 30 wgmma m64n160k16 each for its 64 rows,
-//                  register accumulators (the 10-20 wgmma of one matrix form one commit group), then staged
-//                  as fp32 rows over the (consumed) weight ring
+//                  2-slot ring (four bulk copies each; an edge tap's 20 runs of its reached columns).  The next
+//                  tile's A panel is requested as soon as this tile's MMAs retire (a_empty), so it loads under
+//                  this tile's epilogue; its weights wait for the epilogue to release the ring (ring_free)
+//   warpgroups 0-1 per tap: A_hi x W_hi, A_lo x W_hi, A_hi x W_lo — 30 pairs of wgmma m64n80k16 (one per
+//                  accumulator half; one m64n160 when the link has no edge tap to trim) each for its 64 rows, or
+//                  30 m64n40 / m64n80 over the reached columns of an edge tap; register accumulators (the wgmma of one matrix form one commit group), then
+//                  staged as fp32 rows over the (consumed) weight ring
 //   12 epilogue warps = 3 column groups x 4 row quadrants: group g owns units u = g (mod 3), a unit
 //                  being one channel (r >= 8) or a channel pair (r = 4): 6-7 / 6-7 / 3-4 units per group for
 //                  C = 20 / 40 / 10 (13 warps leave the MMA warpgroups the registers of 160 accumulator columns)
 // RAG: a ragged batch (p.lens): a separate instantiation, so that the dense one keeps its registers
-template <int R, bool RAG>
+// TRIM: the link has edge taps to trim (p.tap_cols != 0); without, one m64n160 per K step as before
+template <int R, bool RAG, bool TRIM>
 __global__ void __launch_bounds__(s2d::THREADS, 1)
 amp_s2d_link_kernel(const AmpS2dParams p) {
   using namespace s2d;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t a_full, a_empty, ring_free, w_full[2], w_empty[2];
+  __shared__ __align__(8) uint64_t a_full, a_empty, ring_free, w_full[2], w_empty[2], res_full;
   __shared__ float s_par[3][40];      // bias | exp(alpha) | 1 / (exp(beta) + 1e-9) of every channel (C <= 40)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -196,11 +291,17 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
   uint8_t* Abase = smem;
   uint8_t* Wbase = smem + 2 * A_PART;
   float* Stg = reinterpret_cast<float*>(smem + 2 * A_PART + 2 * W_SLOT);
+  uint8_t* Res = smem + 2 * A_PART + 2 * W_SLOT + STG_BYTES;
+  // The first matrix of every tile waits for the epilogue to release the ring, and its L2 fetch is exposed.
+  // When it is a 40-column edge tap (tap 0 reaching phase group 0 only) its W_hi is the same 12,800 B for every
+  // tile: it is loaded once, packed to its columns, and stays resident outside the ring.
+  const bool res0 = TRIM && (p.tap_cols & 7) == 1;
   float* Acc = reinterpret_cast<float*>(Wbase);  // staged accumulator [TILE][ACC_LD], over the weight ring
 
   if (tid == 0) {
     tc::mbar_init(&a_full, 1); tc::mbar_init(&a_empty, 1); tc::mbar_init(&ring_free, 1);
     for (int i = 0; i < 2; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 2); }
+    tc::mbar_init(&res_full, 1);
     tc::fence_barrier_init();
   }
   __syncthreads();
@@ -210,6 +311,10 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
     if (tc::elect_one()) {
       const uint8_t* img[2] = {reinterpret_cast<const uint8_t*>(p.a_hi), reinterpret_cast<const uint8_t*>(p.a_lo)};
       int it = 0, wi = 0;
+      if (res0) {
+        tc::mbar_arrive_expect_tx(&res_full, RES_W);
+        for (int kc = 0; kc < KC; ++kc) tc::bulk_g2s(Res + kc * GCOLS * 16, p.wpk + kc * LBO_B, GCOLS * 16, &res_full);
+      }
       for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
         const int b = tile / tpi, t = tile - b * tpi;
         const long long row0 = (long long)t * S - HS - A_OFF + PADR;     // image row of A-panel row 0 (>= 6)
@@ -222,14 +327,22 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
             tc::bulk_g2s(Abase + (size_t)part * A_PART + (size_t)kc * RA * 16,
                          img[part] + ((((long long)b * KC + kc) * p.Rp) + row0) * 16, RA * 16, &a_full);
         if (it >= 1) tc::mbar_wait_parked(&ring_free, (uint32_t)((it - 1) & 1));
-        for (int c = 0; c < 2 * p.ntaps; ++c, ++wi) {
+        for (int c = res0 ? 1 : 0; c < 2 * p.ntaps; ++c, ++wi) {
           const int st = wi & 1;
           if (wi >= 2) tc::mbar_wait_parked(&w_empty[st], (uint32_t)(((wi >> 1) - 1) & 1));
-          tc::mbar_arrive_expect_tx(&w_full[st], W_SLOT);
+          const int code = (int)(p.tap_cols >> (3 * (c >> 1))) & 7;
+          uint8_t* dst = Wbase + (size_t)st * W_SLOT;
+          const uint8_t* src = p.wpk + (size_t)c * W_SLOT;
+          if (code) {        // an edge tap: only its reached columns, one run of w rows per octet
+            const uint32_t w = (code & 1 ? 1u : 2u) * GCOLS, off = (code >= 3 ? 2u * GCOLS : 0u) * 16u;
+            tc::mbar_arrive_expect_tx(&w_full[st], KC * w * 16);
+            for (int kc = 0; kc < KC; ++kc) tc::bulk_g2s(dst + kc * LBO_B + off, src + kc * LBO_B + off, w * 16, &w_full[st]);
+          } else {
+            tc::mbar_arrive_expect_tx(&w_full[st], W_SLOT);
 #pragma unroll
-          for (int piece = 0; piece < 4; ++piece)    // four requests in flight per matrix instead of one long one
-            tc::bulk_g2s(Wbase + (size_t)st * W_SLOT + piece * (W_SLOT / 4), p.wpk + (size_t)c * W_SLOT + piece * (W_SLOT / 4),
-                         W_SLOT / 4, &w_full[st]);
+            for (int piece = 0; piece < 4; ++piece)    // four requests in flight per matrix instead of one long one
+              tc::bulk_g2s(dst + piece * (W_SLOT / 4), src + piece * (W_SLOT / 4), W_SLOT / 4, &w_full[st]);
+          }
         }
       }
     }
@@ -241,9 +354,8 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
     const int row = q * 32 + lane;
     // warp_u, not warp: ptxas must see the MMA branch (wg < 2) as warp-uniform, or it serialises every wgmma
     const int wg = warp_u >> 2, tw = tid & 127;
-    constexpr uint32_t LBO_A = RA * 16, LBO_B = N * 16;
-    constexpr uint64_t KSA = (2 * LBO_A) >> 4, KSB = (2 * LBO_B) >> 4;      // descriptor step per K = 16
     const uint32_t a_h0 = tc::smem_u32(Abase) + (uint32_t)wg * 64u * 16u, a_l0 = a_h0 + A_PART, w_s0 = tc::smem_u32(Wbase);
+    const uint64_t b_res = tc::smem_desc(tc::smem_u32(Res), GCOLS * 16);
     const float* arow = Acc + row * ACC_LD;
     int wi = 0;
     constexpr int CU = R >= 8 ? R : 8;            // accumulator columns per unit: whole channels, >= one image octet
@@ -285,30 +397,36 @@ amp_s2d_link_kernel(const AmpS2dParams p) {
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const uint32_t arow_off = (uint32_t)(A_OFF - p.mlo + tap) * 16u;   // row shift
           const uint64_t ah = tc::smem_desc(a_h0 + arow_off, LBO_A), al = tc::smem_desc(a_l0 + arow_off, LBO_A);
+          const int code = (int)(p.tap_cols >> (3 * tap)) & 7;
 #pragma unroll   // part is a constant: each matrix is one branch-free commit group
-          for (int part = 0; part < 2; ++part, ++wi) {   // W_hi: A_hi x W_hi, A_lo x W_hi;  W_lo: A_hi x W_lo
+          for (int part = 0; part < 2; ++part) {   // W_hi: A_hi x W_hi, A_lo x W_hi;  W_lo: A_hi x W_lo
+            if (part == 0 && tap == 0 && res0) {     // the resident first matrix: no ring slot
+              tc::mbar_wait_parked(&res_full, 0u);
+              tc::wg_fence();
+              s2d_mma<GCOLS, 0, true, GCOLS * 16>(acc, ah, al, b_res);
+              tc::wg_commit();
+              tc::wg_wait<0>();
+              continue;
+            }
             const int st = wi & 1;
             tc::mbar_wait_parked(&w_full[st], (uint32_t)((wi >> 1) & 1));
             const uint64_t bw = tc::smem_desc(w_s0 + (uint32_t)st * W_SLOT, LBO_B);
             tc::wg_fence();
-#pragma unroll
-            for (int kk = 0; kk < N / 16; ++kk) tc::Wg<N, 0>::ss(acc, ah + kk * KSA, bw + kk * KSB, 1u);
-            if (part == 0) {
-#pragma unroll
-              for (int kk = 0; kk < N / 16; ++kk) tc::Wg<N, 0>::ss(acc, al + kk * KSA, bw + kk * KSB, 1u);
-            }
+            if (part == 0) s2d_mma_tap<true, TRIM>(acc, ah, al, bw, code);
+            else s2d_mma_tap<false, TRIM>(acc, ah, al, bw, code);
             tc::wg_commit();
             // drain before the next matrix: the ring is fed from L2 about as fast as the MMAs consume it, so
             // the slot is released the moment its MMAs retire (releasing it one matrix later, under
             // wgmma.wait_group 1, made the links 2-33 % slower on an H100 SXM at 700 W)
             tc::wg_wait<0>();
             if (tw == 0) tc::mbar_arrive(&w_empty[st]);
+            ++wi;
           }
         }
         tc::wg_hold(acc);
         tc::named_sync(6, 256);                   // both warpgroups' MMAs have retired: A panel and ring are free
         if (tid == 0) tc::mbar_arrive(&a_empty);
-        tc::acc_to_smem<N>(acc, Acc + wg * 64 * ACC_LD, ACC_LD, 0, N / 8);
+        s2d_stage_acc<R>(acc, Acc + wg * 64 * ACC_LD);
       }
       tc::named_sync(7, EPI_WARPS * 32);          // accumulator rows staged
       auto ld_acc = [&](int col, uint32_t* dst, int n) {
@@ -503,7 +621,12 @@ int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s) {
     set_error("amp_s2d_link: tap range exceeds the A panel, wrong image rows or missing operand");
     return SVCB_E_BAD_SHAPE;
   }
-  static DevSmemCache c4, c8, c16, g4, g8, g16;
+  for (int t = 0; t < p.ntaps; ++t)
+    if (((p.tap_cols >> (3 * t)) & 7) > 4) {
+      set_error("amp_s2d_link: a tap's column range is empty");
+      return SVCB_E_BAD_SHAPE;
+    }
+  static DevSmemCache c4, c8, c16, g4, g8, g16, u4, u8, u16, v4, v8, v16;
   const int n_sm = device_sm_count();
   if (n_sm <= 0) { set_error("amp_s2d_link: cannot query the SM count"); return SVCB_E_CUDA; }
   const int S = s2d_tile_stride(r);
@@ -514,19 +637,29 @@ int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s) {
   const double el = (double)p.B * p.C * p.L;
   KernelScope ks(kname, s, 2.0 * p.C * p.K * el, el * (4.0 + (p.o_hi ? 4.0 : 0.0) + (p.res ? 4.0 : 0.0) + (p.y ? (p.accum ? 8.0 : 4.0) : 0.0)),
                  p.o_hi ? 70.0 * el : 0.0);
-#define SVCB_S2D_LINK(r_, rag, cache)                                                 \
-  do {                                                                                \
-    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_s2d_link_kernel<r_, rag>, s2d::SMEM, cache)); \
-    amp_s2d_link_kernel<r_, rag><<<grid, s2d::THREADS, s2d::SMEM, s>>>(p);            \
+#define SVCB_S2D_LINK(r_, rag, trim, cache)                                                 \
+  do {                                                                                      \
+    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_s2d_link_kernel<r_, rag, trim>, s2d::SMEM, cache)); \
+    amp_s2d_link_kernel<r_, rag, trim><<<grid, s2d::THREADS, s2d::SMEM, s>>>(p);            \
   } while (0)
-  if (p.lens) {
-    if (r == 4) SVCB_S2D_LINK(4, true, g4);
-    else if (r == 8) SVCB_S2D_LINK(8, true, g8);
-    else SVCB_S2D_LINK(16, true, g16);
+  // links without a trimmed tap keep the single 160-column accumulator (one m64n160 per K step)
+  const bool trim = p.tap_cols != 0;
+  if (p.lens && trim) {
+    if (r == 4) SVCB_S2D_LINK(4, true, true, g4);
+    else if (r == 8) SVCB_S2D_LINK(8, true, true, g8);
+    else SVCB_S2D_LINK(16, true, true, g16);
+  } else if (p.lens) {
+    if (r == 4) SVCB_S2D_LINK(4, true, false, v4);
+    else if (r == 8) SVCB_S2D_LINK(8, true, false, v8);
+    else SVCB_S2D_LINK(16, true, false, v16);
+  } else if (trim) {
+    if (r == 4) SVCB_S2D_LINK(4, false, true, c4);
+    else if (r == 8) SVCB_S2D_LINK(8, false, true, c8);
+    else SVCB_S2D_LINK(16, false, true, c16);
   } else {
-    if (r == 4) SVCB_S2D_LINK(4, false, c4);
-    else if (r == 8) SVCB_S2D_LINK(8, false, c8);
-    else SVCB_S2D_LINK(16, false, c16);
+    if (r == 4) SVCB_S2D_LINK(4, false, false, u4);
+    else if (r == 8) SVCB_S2D_LINK(8, false, false, u8);
+    else SVCB_S2D_LINK(16, false, false, u16);
   }
 #undef SVCB_S2D_LINK
   SVCB_LAUNCH_CHECK("amp_s2d_link");

@@ -100,9 +100,10 @@ struct UpStage {
 struct ResBlock {
   ConvW c1[3], c2[3];
   const uint8_t *c1_tc[3], *c2_tc[3];  // bf16 hi/lo tensor-core images of the same weights
-  // narrow stages (C * r = 160, r = s2d_r): block-Toeplitz matrices of the same convs (pack.py:pack_conv_s2d)
+  // narrow stages (C * r = 160, r = s2d_r): block-Toeplitz matrices of the same convs (pack.py:pack_conv_s2d_slots)
   const uint8_t *c1_s2d[3] = {nullptr, nullptr, nullptr}, *c2_s2d[3] = {nullptr, nullptr, nullptr};
   int s2d_r = 0, s2d_ml1[3], s2d_nt1[3], s2d_ml2[3], s2d_nt2[3];
+  uint64_t s2d_tc1[3], s2d_tc2[3];      // the output columns each tap reaches (s2d_tap_plan)
   SnakeW act[6];
   int k, dil[3];
   AmpForm form = AMP_FP32;
@@ -110,13 +111,8 @@ struct ResBlock {
                                  // AMP_S2D needs L % s2d_r == 0 and L % 8 == 0
 };
 
-// must match pack.py:s2d_factor / s2d_taps
+// must match pack.py:s2d_factor
 static int s2d_link_factor(int ch) { return ch == 40 ? 4 : ch == 20 ? 8 : ch == 10 ? 16 : 0; }
-static void s2d_taps(int k, int dil, int r, int& mlo, int& ntaps) {
-  const int P = dil * (k - 1) / 2;
-  mlo = (P + r - 1) / r;
-  ntaps = mlo + (r - 1 + P) / r + 1;
-}
 
 }  // namespace svcb
 
@@ -427,6 +423,7 @@ static AmpS2dParams s2d_link(const AmpStage& a, const ResBlock& R, int d, int ha
   q.a_hi = in[0]; q.a_lo = in[1];
   q.wpk = half ? R.c2_s2d[d] : R.c1_s2d[d]; q.bias = half ? R.c2[d].b : R.c1[d].b;
   q.ntaps = half ? R.s2d_nt2[d] : R.s2d_nt1[d]; q.mlo = half ? R.s2d_ml2[d] : R.s2d_ml1[d];
+  q.tap_cols = half ? R.s2d_tc2[d] : R.s2d_tc1[d];
   q.lens = a.lens; q.lscale = a.lscale;
   if (next < 6) {
     const SnakeW& act = R.act[next];
@@ -874,8 +871,8 @@ static int resolve(svcb_model* m, Resolver& R) {
       }
       rb.s2d_r = s2d_link_factor(ch);
       for (int d = 0; d < 3 && rb.s2d_r; ++d) {
-        s2d_taps(rb.k, rb.dil[d], rb.s2d_r, rb.s2d_ml1[d], rb.s2d_nt1[d]);
-        s2d_taps(rb.k, 1, rb.s2d_r, rb.s2d_ml2[d], rb.s2d_nt2[d]);
+        s2d_tap_plan(rb.k, rb.dil[d], rb.s2d_r, rb.s2d_ml1[d], rb.s2d_nt1[d], rb.s2d_tc1[d]);
+        s2d_tap_plan(rb.k, 1, rb.s2d_r, rb.s2d_ml2[d], rb.s2d_nt2[d], rb.s2d_tc2[d]);
         const uint64_t per_tap = 2ull * 160 * 160 / 2;   // fp32-typed elements of one (hi, lo) pair
         rb.c1_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c1." + std::to_string(d) + ".s2d", per_tap * rb.s2d_nt1[d]));
         rb.c2_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c2." + std::to_string(d) + ".s2d", per_tap * rb.s2d_nt2[d]));
@@ -1237,7 +1234,7 @@ int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_ac
     SVCB_TRY(snake_taps_from_device(fu, fd, &q.taps));
   }
   q.wpk = static_cast<const uint8_t*>(w_s2d); q.bias = bias; q.res = res; q.y = y;
-  s2d_taps(K, dilation, r, q.mlo, q.ntaps);
+  if (!s2d_tap_plan(K, dilation, r, q.mlo, q.ntaps, q.tap_cols)) { set_error("svcb_op_amp_s2d_link: too many taps"); return SVCB_E_BAD_SHAPE; }
   SVCB_TRY(launch_amp_s2d_link(q, s));
   if (y_act) SVCB_TRY(launch_s2d_unpack(q.o_hi, q.o_lo, y_act, B, C, L, s));
   return SVCB_OK;

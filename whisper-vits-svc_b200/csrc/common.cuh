@@ -349,7 +349,8 @@ struct AmpS2dParams {
   const void* a_lo = nullptr;
   void* o_hi = nullptr;         // output S2D image = SnakeAlias_next(result), or null
   void* o_lo = nullptr;
-  const uint8_t* wpk = nullptr; // bf16 [ntaps][2 (hi, lo)][20][160][8]  (pack.py:pack_conv_s2d)
+  const uint8_t* wpk = nullptr; // bf16 [ntaps][2 (hi, lo)][20][160][8], output columns in phase-group order
+                                // (pack.py:pack_conv_s2d_slots)
   const float* bias = nullptr;  // [C]
   const float* res = nullptr;   // residual [B, C, L] fp32 or null
   float* y = nullptr;           // fp32 result [B, C, L] or null
@@ -359,7 +360,8 @@ struct AmpS2dParams {
   int B = 0, C = 0, L = 0, K = 0;   // K = taps of the original conv (bookkeeping only)
   int Rp = 0;                   // image rows per (item, octet) = s2d_rows(L, r)
   int ntaps = 0, mlo = 0;       // Toeplitz row offsets -mlo .. ntaps-1-mlo (pack.py:s2d_taps)
-  int accum = 0;                // y = y_old + v
+  uint64_t tap_cols = 0;        // 3 bits per tap (s2d_tap_plan): the output columns its matrix can reach
+  int accum = 0;               // y = y_old + v
   float out_div = 0.f;          // then / out_div when != 0
   const int* lens = nullptr;    // ragged batch: item b ends at lens[b] * lscale samples (a multiple of r), or null
   int lscale = 1;
@@ -381,6 +383,9 @@ int launch_snake_pack_s2d(const float* x, void* hi, void* lo, const float* ea, c
 int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, int L, cudaStream_t s);
 int s2d_rows(int L, int r);
 size_t s2d_image_bytes(int B, int L, int r);
+// Toeplitz taps of a 'same' Conv1d(k, dil) over rows of r samples (pack.py:s2d_taps) and, per tap, the output
+// columns it reaches (pack.py:s2d_tap_cols) as AmpS2dParams::tap_cols; false when there are more taps than fit
+bool s2d_tap_plan(int k, int dil, int r, int& mlo, int& ntaps, uint64_t& tap_cols);
 
 // ----------------------------------------------------------------------------- fused AMP block (C = 10, 20)
 struct AmpBlockParams {

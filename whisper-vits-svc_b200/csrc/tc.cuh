@@ -107,7 +107,8 @@ __device__ __forceinline__ void wg_hold(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- wgmma wrappers, m64nNk16, bf16 x bf16 -> fp32, N = 16 .. 256 in steps of 16 (A from registers: N = 64, 96)
+// ---- wgmma wrappers, m64nNk16, bf16 x bf16 -> fp32, N = 16 .. 256 in steps of 16, and 24, 40 (A from
+// registers: N = 64, 96)
 #define SVCB_F4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
 #define SVCB_F8(i) SVCB_F4(i), SVCB_F4(i + 4)
 #define SVCB_R8_0 "%0, %1, %2, %3, %4, %5, %6, %7"
@@ -143,6 +144,12 @@ template <int TB> struct Wg<32, TB> {
   static __device__ __forceinline__ void ss(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\nwgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {" SVCB_R8_0 ", " SVCB_R8_8
                  "}, %16, %17, p, 1, 1, 0, %19;\n}\n" : SVCB_F8(0), SVCB_F8(8) : "l"(da), "l"(db), "r"(acc), "n"(TB));
+  }
+};
+template <int TB> struct Wg<40, TB> {
+  static __device__ __forceinline__ void ss(float (&d)[20], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %22, 0;\nwgmma.mma_async.sync.aligned.m64n40k16.f32.bf16.bf16 {" SVCB_R8_0 ", " SVCB_R8_8
+                 ", %16, %17, %18, %19}, %20, %21, p, 1, 1, 0, %23;\n}\n" : SVCB_F8(0), SVCB_F8(8), SVCB_F4(16) : "l"(da), "l"(db), "r"(acc), "n"(TB));
   }
 };
 template <int TB> struct Wg<48, TB> {

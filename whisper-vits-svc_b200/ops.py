@@ -103,7 +103,7 @@ def amp_s2d_link(x, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=Non
     ea_i, ib_i = snake_params(alpha_in, beta_in)
     ea_o, ib_o = snake_params(alpha_out, beta_out) if alpha_out is not None else (None, None)
     fu, fd = _c(fu.reshape(-1).to(x.device)), _c(fd.reshape(-1).to(x.device))
-    w = pack.pack_conv_s2d(weight.detach().cpu().float(), dilation, r).to(x.device)
+    w = pack.pack_conv_s2d_slots(weight.detach().cpu().float(), dilation, r).to(x.device)
     b = _c(bias)
     rs = _c(res) if res is not None else None
     y = torch.empty_like(x)

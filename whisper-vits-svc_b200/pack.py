@@ -111,6 +111,48 @@ def pack_conv_s2d(w: torch.Tensor, dil: int, r: int) -> torch.Tensor:
     return img.view(torch.float32).reshape(-1)
 
 
+S2D_SLOT_GROUPS = (0, 1, 3, 2)   # phase group held by each 40-column slot of csrc/amp_s2d.cu
+
+
+def s2d_column_order(r: int) -> torch.Tensor:
+    """Output column n of the kernel's slot order -> column c*r + p of conv_s2d_matrices.  Slot s = n // 40 holds
+    the g = r/4 phases p = g*q + j of phase group q = S2D_SLOT_GROUPS[s], channel by channel: n = 40 s + g c + j.
+    Every edge tap then reaches only the first 40 or 80 columns of a half (s2d_tap_cols)."""
+    g = r // 4
+    n = torch.arange(S2D_WIDTH)
+    q = torch.tensor(S2D_SLOT_GROUPS)[n // 40]
+    c, j = (n % 40) // g, (n % 40) % g
+    return c * r + g * q + j
+
+
+def s2d_tap_cols(k: int, dil: int, r: int):
+    """Per Toeplitz tap m = -mlo .. mhi, the output columns [n0, n1) of the slot order its matrix can reach.
+    Tap m reaches the phases max(0, r m - P) .. min(r - 1, r m + r - 1 + P); an edge tap that reaches only
+    phase groups {0}, {0, 1}, {3} or {3, 2} keeps [0, 40), [0, 80), [80, 120) or [80, 160), every other tap
+    all 160 columns (csrc/amp_s2d.cu:s2d_tap_plan)."""
+    P = dil * (k - 1) // 2
+    mlo, mhi = s2d_taps(k, dil, r)
+    g = r // 4
+    cols = []
+    for m in range(-mlo, mhi + 1):
+        q0, q1 = max(0, r * m - P) // g, min(r - 1, r * m + r - 1 + P) // g
+        if q0 == 0 and q1 <= 1:
+            cols.append((0, 40 * (q1 + 1)))
+        elif q1 == 3 and q0 >= 2:
+            cols.append((80, 80 + 40 * (4 - q0)))
+        else:
+            cols.append((0, S2D_WIDTH))
+    return cols
+
+
+def pack_conv_s2d_slots(w: torch.Tensor, dil: int, r: int) -> torch.Tensor:
+    """pack_conv_s2d's image with the output (N') index in the slot order of s2d_column_order: the layout
+    csrc/amp_s2d.cu reads, so that an edge tap's reached columns are one contiguous run per octet."""
+    T = sum(s2d_taps(w.shape[-1], dil, r)) + 1
+    img = pack_conv_s2d(w, dil, r).view(torch.bfloat16).view(T, 2, S2D_WIDTH // 8, S2D_WIDTH, 8)
+    return img[:, :, :, s2d_column_order(r)].contiguous().view(torch.float32).reshape(-1)
+
+
 def tc_tiling(cout: int, cin: int):
     """(kch, cin_pad, bn, ntiles) — must match csrc/api.cu:tc_tiling."""
     kch = 32
@@ -291,8 +333,8 @@ def pack_svc_state_dict(sd: Dict[str, torch.Tensor], cfg: dict) -> List[Tuple[st
             put(f"dec.res.{n}.c1.{d}.tc", pack_conv_tc(w1))
             put(f"dec.res.{n}.c2.{d}.tc", pack_conv_tc(w2))
             if r:   # narrow stages: block-Toeplitz matrices for csrc/amp_s2d.cu
-                put(f"dec.res.{n}.c1.{d}.s2d", pack_conv_s2d(w1, cfg["res_dilations"][j][d], r))
-                put(f"dec.res.{n}.c2.{d}.s2d", pack_conv_s2d(w2, 1, r))
+                put(f"dec.res.{n}.c1.{d}.s2d", pack_conv_s2d_slots(w1, cfg["res_dilations"][j][d], r))
+                put(f"dec.res.{n}.c2.{d}.s2d", pack_conv_s2d_slots(w2, 1, r))
         for a in range(6):
             _snake(put, f"dec.res.{n}.act.{a}", sd, f"{p}.activations.{a}")
     _snake(put, "dec.post.act", sd, "dec.activation_post")
