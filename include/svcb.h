@@ -257,6 +257,15 @@ int svcb_resample_ragged(const float* x, const int64_t* in_offsets_host, int32_t
 int svcb_pcm16_normalise_ragged(const float* y, const int64_t* offsets_host, int32_t B, int16_t* out, float* peak,
                                 svcb_stream stream);
 
+/* ------------------------------------------------------------------ cutting the lowest STFT bins (training data) */
+/* Replaces prepare/preprocess_cdc.py:16-25 (cut_direct_content) for a ragged batch of mono clips: item b is
+ * x[offsets_host[b] .. offsets_host[b+1]) (fp32, as torchaudio.load gives it, finite), n_b >= 513, B >= 1.  Its
+ * 1024 / 256 periodic-Hann STFT (center, reflect padding of 512) with bins 0 and 1 set to zero, inverted by the
+ * overlap-add over the window envelope and computed in fp64 without a transform, rounded to fp32, x 32768, clamped to
+ * [-32768, 32767] and truncated toward zero.  out: int16, item b's 256*(n_b/256) samples following item b-1's from
+ * out[0].  Each item is bitwise that of a lone call. */
+int svcb_cdc_ragged(const float* x, const int64_t* offsets_host, int32_t B, int16_t* out, svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */

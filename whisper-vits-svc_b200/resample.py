@@ -19,16 +19,21 @@ from . import _lib
 _TAPS = {}   # (up, down, device) -> (device fp64 taps, pre_remove)
 
 
-def decode_wav(path: str) -> Tuple[int, np.ndarray]:
-    """(rate, float32 mono) of a .wav as librosa decodes it: integer PCM scaled to [-1, 1) (8-bit is unsigned around
-    128), float PCM as stored, channels averaged."""
-    from scipy.io import wavfile
-    rate, x = wavfile.read(path)
+def scale_pcm(x: np.ndarray) -> np.ndarray:
+    """Samples as scipy reads them -> float32, as librosa and torchaudio decode them: integer PCM scaled to [-1, 1)
+    (8-bit is unsigned around 128), float PCM as stored."""
     if x.dtype == np.uint8:     # 8-bit WAV is unsigned with the zero level at 128
         x = (x.astype(np.float32) - 128.0) / 128.0
     elif x.dtype.kind in "iu":
         x = x.astype(np.float32) / float(np.iinfo(x.dtype).max + 1)
-    x = x.astype(np.float32)
+    return x.astype(np.float32)
+
+
+def decode_wav(path: str) -> Tuple[int, np.ndarray]:
+    """(rate, float32 mono) of a .wav as librosa decodes it: `scale_pcm`, channels averaged."""
+    from scipy.io import wavfile
+    rate, x = wavfile.read(path)
+    x = scale_pcm(x)
     if x.ndim > 1:
         x = x.mean(axis=1)
     return int(rate), x
