@@ -31,19 +31,7 @@ def main(args):
                          "(use the reference's pitch/inference.py to produce it)")
     if not torch.cuda.is_available():
         raise SystemExit("this build has no CPU path: a CUDA (sm_90a) device is required")
-    if args.vec is None:   # svc_inference.py:144-148 of the reference, in-process
-        from whisper_vits_svc_b200 import hubert_infer
-        args.vec = "svc_tmp.vec.npy"
-        print(f"Auto run : H100 hubert-soft encoder -w {args.wave} -v {args.vec}")
-        hm = hubert_infer.load_model(os.path.join("hubert_pretrain", "hubert-soft-0d54a1f4.pt"), "cuda")
-        hubert_infer.pred_vec(hm, args.wave, args.vec)
-        del hm
-    if args.ppg is None:
-        from whisper_vits_svc_b200 import whisper_infer
-        args.ppg = "svc_tmp.ppg.npy"
-        print(f"Auto run : H100 whisper encoder -w {args.wave} -p {args.ppg}")
-        wm = whisper_infer.load_model(os.path.join("whisper_pretrain", "large-v2.pt"), "cuda")
-        whisper_infer.pred_ppg(wm, args.wave, args.ppg, "cuda")
+    args.ppg, args.vec = hostio.extract_missing_features(args.wave, args.ppg, args.vec)
     logging.basicConfig(level=logging.DEBUG if args.debug else logging.INFO)
     device = torch.device("cuda")
     hp = hparams.load_hparams(args.config)

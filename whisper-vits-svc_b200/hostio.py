@@ -58,18 +58,40 @@ def save_csv_pitch(pitch: Sequence[float], path: str):
             print(f"{minute}m {seconds}s {millisecond:3d},{int(pitch[i])}", file=f)
 
 
+def shift_pitch(pit: Sequence[int], shift: int) -> torch.Tensor:
+    """svc_inference.py:187-200 and svc_inference_shift.py:63-65: the CSV pitch times 2^(shift/12) in float64, then
+    rounded once to float32.  (At shift 0 the factor is exactly 1, so the integer pitch passes unchanged.)"""
+    return torch.FloatTensor(np.array(pit) * (2 ** (shift / 12)))
+
+
 def prepare_features(ppg_path: str, vec_path: str, pit_path: str, shift: int = 0):
     """svc_inference.py:172-199: 20 ms rows repeated x2, CSV pitch, optional 2^(k/12) shift."""
     # (torch.from_numpy on the repeated float32 array: the same values as the reference's torch.FloatTensor(...)
     #  without a second 5 MB copy per utterance)
     ppg = torch.from_numpy(np.ascontiguousarray(np.repeat(np.load(ppg_path), 2, 0), dtype=np.float32))
     vec = torch.from_numpy(np.ascontiguousarray(np.repeat(np.load(vec_path), 2, 0), dtype=np.float32))
-    pit = load_csv_pitch(pit_path)
-    if shift != 0:
-        pit = np.array(pit)
-        pit = pit * (2 ** (shift / 12))
-    pit = torch.FloatTensor(pit)
-    return ppg, vec, pit
+    return ppg, vec, shift_pitch(load_csv_pitch(pit_path), shift)
+
+
+def extract_missing_features(wave: str, ppg: str | None, vec: str | None) -> Tuple[str, str]:
+    """svc_inference.py:138-148, in process: a missing `vec` / `ppg` path is extracted from `wave` by the device
+    HuBERT-Soft / Whisper encoders into svc_tmp.vec.npy / svc_tmp.ppg.npy, with the checkpoints
+    hubert_pretrain/hubert-soft-0d54a1f4.pt and whisper_pretrain/large-v2.pt of the working directory.
+    Returns the (ppg, vec) paths."""
+    if vec is None:
+        from . import hubert_infer
+        vec = "svc_tmp.vec.npy"
+        print(f"Auto run : H100 hubert-soft encoder -w {wave} -v {vec}")
+        hm = hubert_infer.load_model(os.path.join("hubert_pretrain", "hubert-soft-0d54a1f4.pt"), "cuda")
+        hubert_infer.pred_vec(hm, wave, vec)
+        del hm                      # (its device weights are freed before Whisper large-v2 loads)
+    if ppg is None:
+        from . import whisper_infer
+        ppg = "svc_tmp.ppg.npy"
+        print(f"Auto run : H100 whisper encoder -w {wave} -p {ppg}")
+        wm = whisper_infer.load_model(os.path.join("whisper_pretrain", "large-v2.pt"), "cuda")
+        whisper_infer.pred_ppg(wm, wave, ppg, "cuda")
+    return ppg, vec
 
 
 def chunk_plan(all_frame: int, hop_size: int, out_chunk: int = 2500, hop_frame: int = 10
