@@ -373,22 +373,39 @@ int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_of
                    float* feat_out, void* ws, size_t ws_bytes, svcb_stream stream);
 
 /* Operator entry points of the encoder (unit tests):
- * out[M,N] = A[M,K] . W[N,K]^T + bias with epilogue 0: bf16 row-major out, 1: GELU(erf) then bf16
- * out as the GEMM tile image ([ceil(M/128)][N/64][8][128][8], the A operand of a following GEMM),
- * 2: + res (fp32 [M,N]) -> fp32 out.  A, W bf16 row-major (converted to tile images in `scratch`);
- * N % 256 == 0, K % 64 == 0. */
+ * acc[M,N] = A[M,K] . W[N,K]^T + bias through epilogue 1..7 of csrc/whisper_gemm.cu, with its res_mod and aux
+ * arguments as the encoders pass them: 1 GELU(erf) -> bf16 tile image of out ([ceil(M/128)][N/64][8][128][8]),
+ * 2 + res -> fp32 [M,N], 3 GELU + res[m % res_mod], 4 bf16 head-major QKV (common.cuh qkv_heads_off), 5 GELU
+ * scattered into the next stride-2 conv's im2col image, 6 the stride-2 valid scatter, 7 GELU + res over the first
+ * res_mod columns of rows aux apart.  A, W bf16 row-major (converted to tile images in `scratch`); N % 256 == 0,
+ * K % 64 == 0.  lens_host (may be NULL, epilogue 5 only): the frame count of each of the M / res_mod items, staged
+ * into `scratch`.  `out` is only written where the epilogue stores: the caller sets its initial contents. */
 size_t svcb_op_gemm_bf16_scratch_bytes(int32_t M, int32_t N, int32_t K);
 int svcb_op_gemm_bf16(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
-                      int32_t M, int32_t N, int32_t K, int32_t epilogue, void* scratch, size_t scratch_bytes,
-                      svcb_stream stream);
+                      int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t res_mod, int32_t aux, const int32_t* lens_host,
+                      void* scratch, size_t scratch_bytes, svcb_stream stream);
 /* softmax(q k^T / sqrt(64)) v per head as the encoder runs it (csrc/whisper_attn_tc.cu): qkv bf16 [B*T, 3*D] rows
  * (q|k|v), out bf16 [B*T, D].  q k^T and p v as wgmma MMAs with S and O in registers, operands taken from the
  * head-major layout the QKV GEMM writes (built here from the row-major input).
  * v_layout: 0 = the V panel read as an MN-major operand with LBO = 128 B between 8-key groups (what the encoder
- * uses), 1 = LBO / SBO exchanged (kept for the descriptor unit test).  scratch: 256-byte aligned. */
+ * uses), 1 = LBO / SBO exchanged (kept for the descriptor unit test).  lens_host (may be NULL): item b attends over
+ * its first lens_host[b] keys (1..T), its query rows past that are zeros or finite.  scratch: 256-byte aligned. */
 size_t svcb_op_attention_tc_bf16_scratch_bytes(int32_t B, int32_t T, int32_t D);
 int svcb_op_attention_tc_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, int32_t T, int32_t D, int32_t heads,
-                              int32_t v_layout, void* scratch, size_t scratch_bytes, svcb_stream stream);
+                              int32_t v_layout, const int32_t* lens_host, void* scratch, size_t scratch_bytes, svcb_stream stream);
+/* Row LayerNorm (eps 1e-5) of fp32 x [M, D] as the encoders run it: out_bf16 = 1 writes y as the bf16 GEMM tile image
+ * of [M, D] (rows of the last tile past M are not written) and, when y32 is not NULL, the fp32 rows [M, D] too;
+ * out_bf16 = 0 writes fp32 rows [M, D] to y.  D % 128 == 0, D <= 2048. */
+int svcb_op_ln_rows(const float* x, const float* gamma, const float* beta, void* y, float* y32, int32_t M, int32_t D,
+                    int32_t out_bf16, svcb_stream stream);
+/* The im2col tile image of Whisper's conv1 (k = 3, pad 1) over mel [B, n_mels, n] fp32: img[b*n + t][j*n_mels + ci] =
+ * bf16(mel[b][ci][t + j - 1]), K padded with zero columns to a multiple of 64, pad rows of the last tile zero. */
+int svcb_op_im2col_s1_image(const float* mel, void* img, int32_t B, int32_t n_mels, int32_t n, svcb_stream stream);
+/* The im2col tile image of one channel group of a 'same' convolution over time-major fp32 rows x [B*T, ld]:
+ * img[b*T + t][j*cg + ci] = bf16(x[b*T + t + j - pad][c0 + ci]), zero outside [0, T) or, with lens_host (may be NULL),
+ * outside [0, lens_host[b]); pad rows of the last tile zero.  scratch: 4 B bytes when lens_host is given. */
+int svcb_op_im2col_rows_image(const float* x, void* img, const int32_t* lens_host, int32_t B, int32_t T, int32_t ld, int32_t c0,
+                              int32_t cg, int32_t taps, int32_t pad, void* scratch, size_t scratch_bytes, svcb_stream stream);
 
 /* Per-kernel timing for roofline reports: after svcb_timing_enable(1) every launch is bracketed
  * by CUDA events on its stream; after the caller synchronises, svcb_timing_report() returns

@@ -127,8 +127,8 @@ def test_last_stage_of_rate_4_has_no_combined_image(hp):
 
 
 def test_whisper_conv2_weight_image_layout():
-    """The stem's stride-2 conv runs as a GEMM over an im2col image (csrc/whisper_gemm.cu:
-    im2col_s2_image): its weight must reach the kernel as W2[co][j*D + ci] = w[co][ci][j] in the bf16
+    """The stem's stride-2 conv runs as a GEMM over an im2col image (written by conv1's epilogue 5 in
+    csrc/whisper_gemm.cu): its weight must reach the kernel as W2[co][j*D + ci] = w[co][ci][j] in the bf16
     GEMM tile image [N/256][K/64][8][256][8]."""
     from whisper_vits_svc_b200 import synth, whisper_infer
     dims = dict(synth.WHISPER_LARGE_V2_DIMS, n_audio_state=256, n_audio_head=4, n_audio_layer=4)
@@ -148,7 +148,7 @@ def test_whisper_conv2_weight_image_layout():
 
 
 def test_stem_conv2_im2col_equivalence():
-    """The identity the device path relies on (csrc/whisper_gemm.cu:im2col_s2_image + epilogue 3):
+    """The identity the device path relies on (csrc/whisper_gemm.cu epilogues 5 and 3):
     Conv1d(D, D, k=3, stride=2, padding=1)(h)[b, :, t2] == A[b*n2 + t2, :] @ W2^T with
     A[m, j*D + ci] = h[b, ci, 2*t2 + j - 1] (zero outside) and W2[co, j*D + ci] = w[co, ci, j]."""
     g = torch.Generator().manual_seed(4)

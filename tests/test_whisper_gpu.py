@@ -2,8 +2,6 @@
 The encoder computes GEMMs/attention with bf16 operands (fp32 accumulate); the reference itself
 runs fp16 on GPU (whisper/inference.py:22-23), so the gate is relative: rel-L2 <= 2e-2 and
 cosine >= 0.999 against the fp32 oracle (SURVEY.md §8c tolerance plan)."""
-import ctypes
-
 import numpy as np
 
 import pytest
@@ -15,77 +13,6 @@ from tests.util import max_abs, rel_l2
 from whisper_vits_svc_b200 import synth
 
 pytestmark = pytest.mark.gpu
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _from_image(img, M, N):
-    """GEMM tile image [ceil(M/128)][N/64][8][128][8] -> row-major [M, N]"""
-    mt = (M + 127) // 128
-    t = img.view(mt, N // 64, 8, 128, 8).permute(0, 3, 1, 2, 4).reshape(mt * 128, N)
-    return t[:M]
-
-
-@pytest.mark.parametrize("M,N,K,epi", [(128, 256, 64, 0), (300, 256, 128, 0), (1000, 512, 1280, 1), (257, 1280, 320, 2),
-                                       (3000, 3840, 1280, 0), (24000, 1280, 1280, 2)])
-def test_gemm_bf16(M, N, K, epi):
-    from whisper_vits_svc_b200 import _lib
-    g = torch.Generator().manual_seed(M + N + K)
-    A = (torch.randn(M, K, generator=g)).bfloat16()
-    Wt = (torch.randn(N, K, generator=g) / K ** 0.5).bfloat16()
-    bias = torch.randn(N, generator=g)
-    res = torch.randn(M, N, generator=g)
-    Ad, Wd, bd, rd = A.cuda(), Wt.cuda(), bias.cuda(), res.cuda()
-    ref = Ad.float() @ Wd.float().t() + bd          # fp32 reference on the device (same bf16 inputs)
-    if epi == 1:
-        ref = F.gelu(ref)
-    if epi == 2:
-        ref = ref + rd
-    Mp = (M + 127) // 128 * 128
-    lib = _lib.load()
-    scratch = torch.empty(int(lib.svcb_op_gemm_bf16_scratch_bytes(M, N, K)), dtype=torch.uint8, device="cuda")
-    if epi == 2:
-        out = torch.zeros(M, N, device="cuda", dtype=torch.float32)
-    else:
-        out = torch.zeros(Mp if epi == 1 else M, N, device="cuda", dtype=torch.bfloat16)
-    st = lib.svcb_op_gemm_bf16(Ad.data_ptr(), Wd.data_ptr(), bd.data_ptr(), out.data_ptr(),
-                               rd.data_ptr() if epi == 2 else None, M, N, K, epi, scratch.data_ptr(),
-                               scratch.numel(), _s())
-    _lib.check(st, "svcb_op_gemm_bf16")
-    torch.cuda.synchronize()
-    got = _from_image(out, M, N) if epi == 1 else out
-    tol = 2e-4 * K ** 0.5 if epi == 2 else 3e-2   # bf16 output rounding dominates for epi 0/1
-    assert max_abs(got.float(), ref) <= tol
-
-
-@pytest.mark.parametrize("B,T,heads,v_layout", [(2, 100, 2, 0), (1, 64, 4, 0), (2, 1500, 2, 0), (1, 333, 20, 0), (3, 129, 4, 0),
-                                                (2, 100, 2, 1)])
-def test_attention_tc_bf16(B, T, heads, v_layout):
-    """The encoder's attention kernel (wgmma: S and O in registers, P fed from registers, V read as an MN-major operand) on its
-    own, fed through the same tile image the QKV GEMM writes.  v_layout 1 exchanges LBO / SBO of the V
-    descriptor: it must NOT match (pins the descriptor semantics the kernel relies on)."""
-    from whisper_vits_svc_b200 import _lib
-    D = heads * 64
-    g = torch.Generator().manual_seed(T + heads)
-    qkv = torch.randn(B, T, 3 * D, generator=g).bfloat16()
-    q, k, v = [t.float().view(B, T, heads, 64).permute(0, 2, 1, 3) for t in qkv.split(D, dim=-1)]
-    ref = (F.softmax(q @ k.transpose(-1, -2) / 8.0, dim=-1) @ v).permute(0, 2, 1, 3).reshape(B, T, D)
-    qd = qkv.cuda()
-    out = torch.zeros(B, T, D, device="cuda", dtype=torch.bfloat16)
-    lib = _lib.load()
-    scratch = torch.empty(int(lib.svcb_op_attention_tc_bf16_scratch_bytes(B, T, D)), dtype=torch.uint8, device="cuda")
-    st = lib.svcb_op_attention_tc_bf16(qd.data_ptr(), out.data_ptr(), B, T, D, heads, v_layout, scratch.data_ptr(),
-                                       scratch.numel(), _s())
-    _lib.check(st, "svcb_op_attention_tc_bf16")
-    torch.cuda.synchronize()
-    err = max_abs(out.float(), ref)
-    print(f"attention_tc B={B} T={T} heads={heads} v_layout={v_layout}: max-abs {err:.3e}")
-    if v_layout == 0:
-        assert err <= 2e-2
-    else:
-        assert err > 2e-2
 
 
 @pytest.mark.parametrize("state,heads,layers,B,n", [(256, 4, 4, 2, 200), (512, 8, 4, 1, 301), (1280, 20, 4, 1, 400)])

@@ -120,9 +120,12 @@ SIGNATURES = {
     "svcb_vad_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int64]),
     "svcb_vad_probs": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "svcb_op_gemm_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
-    "svcb_op_gemm_bf16": (c_int, [c_void_p] * 5 + [c_int32] * 4 + [c_void_p, c_size_t, c_void_p]),
+    "svcb_op_gemm_bf16": (c_int, [c_void_p] * 5 + [c_int32] * 6 + [POINTER(c_int32), c_void_p, c_size_t, c_void_p]),
     "svcb_op_attention_tc_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
-    "svcb_op_attention_tc_bf16": (c_int, [c_void_p, c_void_p] + [c_int32] * 5 + [c_void_p, c_size_t, c_void_p]),
+    "svcb_op_attention_tc_bf16": (c_int, [c_void_p, c_void_p] + [c_int32] * 5 + [POINTER(c_int32), c_void_p, c_size_t, c_void_p]),
+    "svcb_op_ln_rows": (c_int, [c_void_p] * 5 + [c_int32] * 3 + [c_void_p]),
+    "svcb_op_im2col_s1_image": (c_int, [c_void_p, c_void_p] + [c_int32] * 3 + [c_void_p]),
+    "svcb_op_im2col_rows_image": (c_int, [c_void_p, c_void_p, POINTER(c_int32)] + [c_int32] * 7 + [c_void_p, c_size_t, c_void_p]),
     "svcb_timing_enable": (None, [c_int32]),
     "svcb_timing_report": (c_char_p, []),
     "svcb_model_create": (c_int, [c_void_p, c_size_t, POINTER(TensorEntry), c_int32, POINTER(Config), POINTER(c_void_p)]),

@@ -493,13 +493,12 @@ int launch_source2wav(const float* src, int16_t* out, size_t n, cudaStream_t s);
 
 // ----------------------------------------------------------------------------- Whisper / HuBERT transformer kernels
 // bf16 wgmma GEMM over tile images with fused epilogues (each one is described in whisper_gemm.cu)
-enum GemmEpi : int { EPI_BF16_ROWMAJOR = 0, EPI_GELU_BF16_IMAGE = 1, EPI_RESID_F32 = 2, EPI_GELU_ADD_F32 = 3, EPI_QKV_HEADS = 4,
+enum GemmEpi : int { EPI_GELU_BF16_IMAGE = 1, EPI_RESID_F32 = 2, EPI_GELU_ADD_F32 = 3, EPI_QKV_HEADS = 4,
                      EPI_GELU_CONV2_IMG = 5, EPI_GELU_VALID_S2_IMG = 6, EPI_GELU_ADD_F32_LD = 7, EPI_IVF_TOPK = 8 };
 // lens (device, may be null): per-item frame counts of a ragged batch, read by epilogue 5 only
 int launch_gemm_tc(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
                    int M, int N, int K, GemmEpi epi, cudaStream_t s, int res_mod = 0, int aux = 0, const int* lens = nullptr);
 int launch_im2col_s1_image(const float* mel, void* img, int B, int n_mels, int n, cudaStream_t s);
-int launch_im2col_s2_image(const float* h1, void* img, int B, int D, int n, int n2, cudaStream_t s, int taps = 3, int pad = 1);
 int launch_im2col_rows_image(const float* x, void* img, int B, int T, int ld, int c0, int cg, int taps, int pad, cudaStream_t s,
                              const int* lens = nullptr);
 // ragged batches: host ints -> device dst[0, n), stream-ordered, without a host-to-device copy

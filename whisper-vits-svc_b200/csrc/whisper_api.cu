@@ -178,31 +178,53 @@ int svcb_whisper_log_mel_ragged(const float* audio, const int32_t* n_samples_hos
   return launch_log_mel(audio, mel_filters, nullptr, 0.f, mel, mx, B, n_samples, n_mels, s, d_lens);
 }
 
+// unit-test entry points: per-item lengths from the host, each in [1, max_len], staged into `dst` on the stream
+static int op_stage_lens(const int32_t* lens_host, int n, int max_len, void* dst, cudaStream_t s, const char* who) {
+  for (int b = 0; b < n; ++b)
+    if (lens_host[b] < 1 || lens_host[b] > max_len) {
+      set_error(std::string(who) + ": item " + std::to_string(b) + " has length " + std::to_string(lens_host[b]) + "; need 1.." +
+                std::to_string(max_len));
+      return SVCB_E_BAD_SHAPE;
+    }
+  return launch_stage_ints(lens_host, n, static_cast<int*>(dst), s);
+}
+
 size_t svcb_op_gemm_bf16_scratch_bytes(int32_t M, int32_t N, int32_t K) {
-  return ((size_t)(M + 127) / 128 * 128 * K + (size_t)N * K) * 2 + 1024;
+  return ((size_t)(M + 127) / 128 * 128 * K + (size_t)N * K) * 2 + align256(4 * (size_t)M) + 1024;
 }
 
 int svcb_op_gemm_bf16(const void* A_bf16, const void* W_bf16, const float* bias, void* out, const float* res,
-                      int32_t M, int32_t N, int32_t K, int32_t epilogue, void* scratch, size_t scratch_bytes,
-                      svcb_stream stream) {
-  // row-major operands in, converted to tile images in `scratch`; epilogue 1 writes the tile image of out
+                      int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t res_mod, int32_t aux, const int32_t* lens_host,
+                      void* scratch, size_t scratch_bytes, svcb_stream stream) {
+  // row-major operands in, converted to tile images in `scratch`; `out` is written by the epilogue as it is
   if (!scratch || scratch_bytes < svcb_op_gemm_bf16_scratch_bytes(M, N, K)) { set_error("gemm scratch too small"); return SVCB_E_WORKSPACE; }
+  if (epilogue < EPI_GELU_BF16_IMAGE || epilogue > EPI_GELU_ADD_F32_LD) {
+    set_error("svcb_op_gemm_bf16: epilogue must be 1..7 (the IVF search, 8, has its own entry point)");
+    return SVCB_E_BAD_SHAPE;
+  }
+  if (lens_host && (epilogue != EPI_GELU_CONV2_IMG || res_mod <= 0 || M % res_mod)) {
+    set_error("svcb_op_gemm_bf16: lengths are read by epilogue 5 only, with rows = items x res_mod frames");
+    return SVCB_E_BAD_SHAPE;
+  }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* a_img = static_cast<char*>(scratch);
   char* w_img = a_img + align256((size_t)(M + 127) / 128 * 128 * K * 2);
+  char* lens = w_img + align256((size_t)N * K * 2);
+  if (lens_host) SVCB_TRY(op_stage_lens(lens_host, M / res_mod, res_mod, lens, s, "svcb_op_gemm_bf16"));
   SVCB_TRY(launch_rowmajor_to_image(A_bf16, a_img, M, K, 128, s));
   SVCB_TRY(launch_rowmajor_to_image(W_bf16, w_img, N, K, 256, s));
-  return launch_gemm_tc(a_img, w_img, bias, out, res, M, N, K, static_cast<GemmEpi>(epilogue), s);
+  return launch_gemm_tc(a_img, w_img, bias, out, res, M, N, K, static_cast<GemmEpi>(epilogue), s, res_mod, aux,
+                        lens_host ? reinterpret_cast<const int*>(lens) : nullptr);
 }
 
 size_t svcb_op_attention_tc_bf16_scratch_bytes(int32_t B, int32_t T, int32_t D) {
   if (B <= 0 || T <= 0 || D <= 0) return 0;
   const size_t Mp = ((size_t)B * T + 127) / 128 * 128;
-  return align256((size_t)B * qkv_heads_tp(T) * 3 * D * 2) + align256(Mp * D * 2) + 512;
+  return align256((size_t)B * qkv_heads_tp(T) * 3 * D * 2) + align256(Mp * D * 2) + align256(4 * (size_t)B) + 512;
 }
 
 int svcb_op_attention_tc_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, int32_t T, int32_t D, int32_t heads,
-                              int32_t v_layout, void* scratch, size_t scratch_bytes, svcb_stream stream) {
+                              int32_t v_layout, const int32_t* lens_host, void* scratch, size_t scratch_bytes, svcb_stream stream) {
   // row-major q|k|v in, converted to the GEMM tile image the encoder produces; result converted back
   SVCB_TRY(check_workspace(scratch, scratch_bytes, svcb_op_attention_tc_bf16_scratch_bytes(B, T, D), "attention_tc"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -210,10 +232,34 @@ int svcb_op_attention_tc_bf16(const void* qkv_bf16, void* out_bf16, int32_t B, i
   char* qimg = static_cast<char*>(scratch);
   const size_t qbytes = (size_t)B * qkv_heads_tp(T) * 3 * D * 2;
   char* oimg = qimg + align256(qbytes);
+  char* lens = oimg + align256((M + 127) / 128 * 128 * D * 2);
+  if (lens_host) SVCB_TRY(op_stage_lens(lens_host, B, T, lens, s, "svcb_op_attention_tc_bf16"));
   SVCB_CUDA_CHECK(cudaMemsetAsync(qimg, 0, qbytes, s));
   SVCB_TRY(launch_qkv_rowmajor_to_heads(qkv_bf16, qimg, B, T, D, s));
-  SVCB_TRY(launch_whisper_attention_tc(qimg, oimg, B, T, D, heads, v_layout, s));
+  SVCB_TRY(launch_whisper_attention_tc(qimg, oimg, B, T, D, heads, v_layout, s, lens_host ? reinterpret_cast<const int*>(lens) : nullptr));
   return launch_image_to_rowmajor(oimg, out_bf16, (int)M, D, s);
+}
+
+int svcb_op_ln_rows(const float* x, const float* gamma, const float* beta, void* y, float* y32, int32_t M, int32_t D,
+                    int32_t out_bf16, svcb_stream stream) {
+  if (!x || !gamma || !beta || !y || M <= 0 || (y32 && !out_bf16)) { set_error("svcb_op_ln_rows: bad argument"); return SVCB_E_BAD_SHAPE; }
+  return launch_ln_rows(x, gamma, beta, y, M, D, out_bf16 != 0, static_cast<cudaStream_t>(stream), y32);
+}
+
+int svcb_op_im2col_s1_image(const float* mel, void* img, int32_t B, int32_t n_mels, int32_t n, svcb_stream stream) {
+  if (!mel || !img || B <= 0 || n_mels <= 0 || n <= 0) { set_error("svcb_op_im2col_s1_image: bad argument"); return SVCB_E_BAD_SHAPE; }
+  return launch_im2col_s1_image(mel, img, B, n_mels, n, static_cast<cudaStream_t>(stream));
+}
+
+int svcb_op_im2col_rows_image(const float* x, void* img, const int32_t* lens_host, int32_t B, int32_t T, int32_t ld, int32_t c0,
+                              int32_t cg, int32_t taps, int32_t pad, void* scratch, size_t scratch_bytes, svcb_stream stream) {
+  if (!x || !img || B <= 0 || T <= 0) { set_error("svcb_op_im2col_rows_image: bad argument"); return SVCB_E_BAD_SHAPE; }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (lens_host) {
+    SVCB_TRY(check_workspace(scratch, scratch_bytes, 4 * (size_t)B, "im2col_rows_image"));
+    SVCB_TRY(op_stage_lens(lens_host, B, T, scratch, s, "svcb_op_im2col_rows_image"));
+  }
+  return launch_im2col_rows_image(x, img, B, T, ld, c0, cg, taps, pad, s, lens_host ? static_cast<const int*>(scratch) : nullptr);
 }
 
 }  // extern "C"

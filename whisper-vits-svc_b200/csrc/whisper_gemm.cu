@@ -14,8 +14,8 @@
 //   producer thread   3-deep ring of (A 16 KB + W BN*128 B) k-tiles, running ahead across tiles
 //   2 warpgroups      64 rows each: wgmma m64nBNk16 x4 per k-tile into register accumulators, then the
 //                     epilogue through a per-warpgroup shared-memory strip (64 columns at a time):
-//                     bias / GELU / residual -> stores (row-major bf16, tile-image bf16 for the next
-//                     GEMM, or fp32 residual stream)
+//                     bias / GELU / residual -> stores (tile-image bf16 for the next GEMM, the
+//                     attention kernel's head-major QKV, scatters into im2col images, or fp32 rows)
 // The row LayerNorm that writes the GEMMs' A images (ln_rows) is at the end of this file.
 #include <algorithm>
 
@@ -227,14 +227,10 @@ gemm_tc_kernel(const __nv_bfloat16* __restrict__ Aimg, const __nv_bfloat16* __re
               const size_t o = qkv_heads_off(bi, w, hd, t, d, Dm >> 6, qkv_heads_tp(res_mod));
               *reinterpret_cast<uint4*>(ob + o) = *reinterpret_cast<const uint4*>(h);
               *reinterpret_cast<uint4*>(ob + o + (w == 0 ? 1024 : 512)) = *reinterpret_cast<const uint4*>(h + 8);
-            } else if (EPI == EPI_GELU_BF16_IMAGE) {  // A operand of the next GEMM
+            } else {   // EPI_GELU_BF16_IMAGE: A operand of the next GEMM
               __nv_bfloat16* ob = static_cast<__nv_bfloat16*>(out);
               *reinterpret_cast<uint4*>(ob + img_off(m, n0 + c0, N / GM_BK)) = *reinterpret_cast<const uint4*>(h);
               *reinterpret_cast<uint4*>(ob + img_off(m, n0 + c0 + 8, N / GM_BK)) = *reinterpret_cast<const uint4*>(h + 8);
-            } else {
-              __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out) + (size_t)m * N + n0 + c0;
-              *reinterpret_cast<uint4*>(o) = *reinterpret_cast<const uint4*>(h);
-              *reinterpret_cast<uint4*>(o + 8) = *reinterpret_cast<const uint4*>(h + 8);
             }
           }
         }
@@ -270,7 +266,6 @@ int launch_gemm_tc(const void* A_img, const void* W_img, const float* bias, void
   const __nv_bfloat16* A = static_cast<const __nv_bfloat16*>(A_img);
   const __nv_bfloat16* W = static_cast<const __nv_bfloat16*>(W_img);
   switch (epi) {
-    case EPI_BF16_ROWMAJOR: return launch_gemm_t<256, EPI_BF16_ROWMAJOR>(A, W, bias, out, res, M, N, K, 0, s);
     case EPI_GELU_BF16_IMAGE: return launch_gemm_t<256, EPI_GELU_BF16_IMAGE>(A, W, bias, out, res, M, N, K, 0, s);
     case EPI_RESID_F32: return launch_gemm_t<256, EPI_RESID_F32>(A, W, bias, out, res, M, N, K, 0, s);
     case EPI_GELU_CONV2_IMG:
@@ -357,39 +352,6 @@ int launch_ivf_pack(const float* x, void* img, int M, int d, cudaStream_t s) {
   ivf_pack_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, static_cast<__nv_bfloat16*>(img), M, Mp, d);
   SVCB_LAUNCH_CHECK("ivf_pack");
   return SVCB_OK;
-}
-
-// Stem conv2 (Conv1d(D, D, k=3, stride 2, pad 1), whisper/model.py:150) as a GEMM: this kernel builds
-// the A tile image of its im2col matrix, A[m = b*n2 + t2][k = j*D + ci] = h1[b][ci][2*t2 + j - 1]
-// (zero outside the sequence and in the rows that pad M to whole 128-row tiles), bf16.
-// One CTA = one (row tile, k tile): a k tile of 64 lies inside one tap j because D % 64 == 0.
-__global__ void __launch_bounds__(256)
-im2col_s2_image_kernel(const float* __restrict__ h1, __nv_bfloat16* __restrict__ img, int D, int n, int n2, int M, int taps,
-                       int pad) {
-  __shared__ float tile[64][129];
-  const int mt = blockIdx.x, kt = blockIdx.y, tid = threadIdx.x;
-  const int j = (kt * 64) / D, ci0 = (kt * 64) % D;
-  for (int idx = tid; idx < 64 * 128; idx += 256) {
-    const int cc = idx >> 7, r = idx & 127;
-    const int m = mt * 128 + r;
-    float v = 0.f;
-    if (m < M) {
-      const int b = m / n2, t2 = m - b * n2;
-      const int t = 2 * t2 + j - pad;
-      if (t >= 0 && t < n) v = __ldg(h1 + ((size_t)b * D + ci0 + cc) * n + t);
-    }
-    tile[cc][r] = v;
-  }
-  __syncthreads();
-  const int KT = taps * D / 64;
-  __nv_bfloat16* dst = img + ((size_t)mt * KT + kt) * (GM_BM * GM_BK);
-  for (int idx = tid; idx < 8 * 128; idx += 256) {
-    const int kc = idx >> 7, r = idx & 127;
-    __align__(16) __nv_bfloat16 h[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) h[e] = __float2bfloat16_rn(tile[kc * 8 + e][r]);
-    *reinterpret_cast<uint4*>(dst + (size_t)(kc * 128 + r) * 8) = *reinterpret_cast<const uint4*>(h);
-  }
 }
 
 // Stem conv1 (Conv1d(n_mels, D, k=3, pad 1), whisper/model.py:149) as a GEMM: the A tile image of ITS im2col matrix,
@@ -506,17 +468,6 @@ int launch_zero_tail_rows(float* out, const int* lens, int B, int T, int width, 
   KernelScope ks("zero_tail_rows", s, 0.0, 4.0 * B * (double)(T - min_len) * width);
   zero_tail_rows_kernel<<<dim3(T - min_len, B), 256, 0, s>>>(out, lens, T, width);
   SVCB_LAUNCH_CHECK("zero_tail_rows");
-  return SVCB_OK;
-}
-
-// taps / pad: 3 / 1 for Whisper's conv2; 3 / 0 for the first stride-2 conv of the HuBERT stem (valid convolution)
-int launch_im2col_s2_image(const float* h1, void* img, int B, int D, int n, int n2, cudaStream_t s, int taps, int pad) {
-  if (D % 64) { set_error("im2col_s2_image: D must be a multiple of 64"); return SVCB_E_BAD_SHAPE; }
-  const int M = B * n2;
-  dim3 grid((M + 127) / 128, taps * D / 64);
-  KernelScope ks("im2col_s2_image", s, 0.0, (double)M * taps * D * 2 + 4.0 * B * D * (double)n);
-  im2col_s2_image_kernel<<<grid, 256, 0, s>>>(h1, static_cast<__nv_bfloat16*>(img), D, n, n2, M, taps, pad);
-  SVCB_LAUNCH_CHECK("im2col_s2_image");
   return SVCB_OK;
 }
 
