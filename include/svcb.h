@@ -14,7 +14,8 @@
  *   - a model handle is immutable after creation: concurrent calls on different streams
  *     are fine when their workspaces differ;
  *   - sm_90a only, no fallback: svcb_model_create, svcb_whisper_create, svcb_hubert_create,
- *     svcb_ivf_create, svcb_speaker_create and svcb_vad_create fail with SVCB_E_UNSUPPORTED elsewhere.
+ *     svcb_ivf_create, svcb_speaker_create, svcb_vad_create and svcb_crepe_create fail with SVCB_E_UNSUPPORTED
+ *     elsewhere.
  */
 #ifndef SVCB_H_
 #define SVCB_H_
@@ -371,6 +372,45 @@ size_t svcb_vad_workspace_bytes(const svcb_vad* v, int32_t B, int64_t total_wind
  * receives the encoder output of each window (may be NULL).  All fp32.  An item's result does not depend on the batch. */
 int svcb_vad_probs(const svcb_vad* v, const float* wav, const int64_t* sample_offsets_host, int32_t B, float* probs_out,
                    float* feat_out, void* ws, size_t ws_bytes, svcb_stream stream);
+
+/* ------------------------------------------------------------------ pitch extractor (CREPE, 16 kHz) */
+typedef struct svcb_crepe svcb_crepe;
+/* Replaces crepe.load.model + Crepe(model) (crepe/load.py, crepe/model.py:14-92).  capacity 0 = 'full' (bf16 wgmma
+ * convolutions, fp32 accumulation), 1 = 'tiny' (fp32 CUDA cores).  Blob names/layouts:
+ * whisper-vits-svc_b200/crepe_infer.py:pack_crepe.  Fails with SVCB_E_UNSUPPORTED unless the device is sm_90. */
+int svcb_crepe_create(const void* dev_blob, size_t blob_bytes, const svcb_tensor_entry* table_host, int32_t n_entries,
+                      int32_t capacity, svcb_crepe** out);
+void svcb_crepe_destroy(svcb_crepe* c);
+/* frames of n_samples of 16 kHz audio at `hop`: 1 + n_samples / hop (crepe/core.py:663) */
+int64_t svcb_crepe_frames(int64_t n_samples, int32_t hop);
+/* scratch for svcb_crepe_probs on total_frames frames in all: frames run through the network in chunks of up to 4096,
+ * about 0.5 MB per frame of a chunk at full capacity (conv1's output is 384 KB of it) */
+size_t svcb_crepe_workspace_bytes(const svcb_crepe* c, int64_t total_frames);
+/* Replaces crepe.preprocess (crepe/core.py:626-702, pad = True) and the noise line of pitch/inference.py:78 for a ragged
+ * batch: item b is wav[sample_offsets_host[b] .. sample_offsets_host[b+1]) (offsets non-decreasing, checked before any
+ * launch; an empty item has one frame) + 0.001 * noise (same layout, may be NULL), zero-padded by 512 on both sides ->
+ * frames_out [sum_b F_b, 1024] fp32, F_b = svcb_crepe_frames(n_b, hop): each frame less its mean, over
+ * max(1e-10, its unbiased standard deviation). */
+int svcb_crepe_frame(const float* wav, const int64_t* sample_offsets_host, int32_t B, int32_t hop, const float* noise,
+                     float* frames_out, svcb_stream stream);
+/* Replaces crepe.infer (crepe/core.py:539-564; crepe/model.py:94-134: pad, conv, ReLU, BatchNorm (eval), max-pool 2, six
+ * times, the classifier over (position, channel) features, sigmoid) and the range mask of crepe.postprocess
+ * (crepe/core.py:597-603, fmin 50, fmax 1000) on the frames of svcb_crepe_frame: probs_out [sum_b F_b, 360] fp32,
+ * bins outside [39, 299) = -inf.  A frame's row does not depend on the batch. */
+int svcb_crepe_probs(const svcb_crepe* c, const float* wav, const int64_t* sample_offsets_host, int32_t B, int32_t hop,
+                     const float* noise, float* probs_out, void* ws, size_t ws_bytes, svcb_stream stream);
+/* scratch for svcb_crepe_decode: the back-pointers, 720 bytes per frame */
+size_t svcb_crepe_decode_workspace_bytes(int64_t total_frames);
+/* Replaces crepe.decode.viterbi + bins_to_frequency + crepe.periodicity (crepe/decode.py:55-80, crepe/convert.py:12-33,
+ * crepe/core.py:710-722) as crepe.predict applies them (crepe/core.py:117-149): item b is rows
+ * frame_offsets_host[b] .. frame_offsets_host[b+1] of probs [.., 360] (each item at least one frame) and is decoded in
+ * independent segments of `segment` (1..512) frames: softmax over the bins, then the Viterbi path of
+ * librosa.sequence.viterbi under transition[i][j] ~ max(12 - |i - j|, 0) with a uniform start, in fp64, the first maximum
+ * on ties.  bins_out int32, pitch_out = 10 * 2^((20 bin + 1997.3794 + dither) / 1200) Hz (dither: cents per frame, may
+ * be NULL), periodicity_out = probs[t][bin] (may be NULL); all indexed like the rows of probs. */
+int svcb_crepe_decode(const float* probs, const int64_t* frame_offsets_host, int32_t B, int32_t segment, const float* dither,
+                      int32_t* bins_out, float* pitch_out, float* periodicity_out, void* ws, size_t ws_bytes,
+                      svcb_stream stream);
 
 /* Operator entry points of the encoder (unit tests):
  * acc[M,N] = A[M,K] . W[N,K]^T + bias through epilogue 1..7 of csrc/whisper_gemm.cu, with its res_mod and aux

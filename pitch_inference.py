@@ -1,0 +1,33 @@
+#!/usr/bin/env python
+"""Drop-in for the reference's pitch/inference.py (same flags): the F0 of one recording by CREPE-full on the H100
+(`compute_f0_sing`: 20 ms hop, Viterbi in 512-frame segments, every value twice, mean over 5), written as the `.pit.csv`
+the inference command lines read, one line per 10 ms.  The weights are crepe/assets/full.pth, where the reference keeps
+them.  The wav is read as `hubert_infer.load_audio` reads it (16 kHz)."""
+import argparse
+import os
+import sys
+
+sys.path.append(os.path.dirname(os.path.abspath(__file__)))
+
+MODEL = os.path.join("crepe", "assets", "full.pth")
+
+
+def require_cuda():
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("this build has no CPU path: a CUDA (sm_90a) device is required")
+
+
+if __name__ == "__main__":
+    parser = argparse.ArgumentParser()
+    parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
+    parser.add_argument("-p", "--pit", help="pit", dest="pit", required=True)  # csv for excel
+    args = parser.parse_args()
+    print(args.wav)
+    print(args.pit)
+    require_cuda()
+    from whisper_vits_svc_b200 import crepe_infer, hostio, hubert_infer
+
+    model = crepe_infer.load_model(MODEL, "cuda")
+    audio = hubert_infer.load_audio(args.wav, crepe_infer.SAMPLE_RATE)
+    hostio.save_csv_pitch(crepe_infer.compute_f0_sing(model, audio), args.pit)

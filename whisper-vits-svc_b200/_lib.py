@@ -119,6 +119,14 @@ SIGNATURES = {
     "svcb_vad_windows": (c_int64, [c_int64]),
     "svcb_vad_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int64]),
     "svcb_vad_probs": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "svcb_crepe_create": (c_int, [c_void_p, c_size_t, POINTER(TensorEntry), c_int32, c_int32, POINTER(c_void_p)]),
+    "svcb_crepe_destroy": (None, [c_void_p]),
+    "svcb_crepe_frames": (c_int64, [c_int64, c_int32]),
+    "svcb_crepe_workspace_bytes": (c_size_t, [c_void_p, c_int64]),
+    "svcb_crepe_frame": (c_int, [c_void_p, POINTER(c_int64), c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    "svcb_crepe_probs": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "svcb_crepe_decode_workspace_bytes": (c_size_t, [c_int64]),
+    "svcb_crepe_decode": (c_int, [c_void_p, POINTER(c_int64), c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "svcb_op_gemm_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_gemm_bf16": (c_int, [c_void_p] * 5 + [c_int32] * 6 + [POINTER(c_int32), c_void_p, c_size_t, c_void_p]),
     "svcb_op_attention_tc_bf16_scratch_bytes": (c_size_t, [c_int32] * 3),

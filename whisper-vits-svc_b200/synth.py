@@ -247,3 +247,25 @@ def speaker_checkpoint(seed: int = 1234):
         sd[b + "lstm.bias_hh_l0"] = r.n(4 * H, std=0.1)
         sd[b + "linear.weight"] = r.n(P, H, std=math.sqrt(2.0 / (P + H)))
     return {"model": {k: v.float().contiguous() for k, v in sd.items()}}
+
+
+def crepe_checkpoint(seed: int = 1234, capacity: str = "full") -> Dict[str, torch.Tensor]:
+    """Seeded CREPE weights in the layout of crepe/assets/{full,tiny}.pth (crepe/model.py:14-92).  Conv weights are
+    scaled by their fan-in so that activations stay O(1) through conv2's K = 65,536; BatchNorm running statistics sit
+    away from (0, 1) and a third of its weights are negative, which swaps the order of the pair being pooled."""
+    channels = {"full": [1, 1024, 128, 128, 128, 256, 512], "tiny": [1, 128, 16, 16, 16, 32, 64]}[capacity]
+    g = _Gen(seed)
+    sd: Dict[str, torch.Tensor] = {}
+    for i in range(6):
+        cin, cout, taps = channels[i], channels[i + 1], 512 if i == 0 else 64
+        p = f"conv{i + 1}"
+        sd[p + ".weight"] = g.n(cout, cin, taps, 1, std=1.6 / math.sqrt(cin * taps))
+        sd[p + ".bias"] = g.n(cout, std=0.1)
+        sign = torch.where(torch.rand(cout, generator=g.g) < 1 / 3, -1.0, 1.0)
+        sd[p + "_BN.weight"] = sign * (0.7 + 0.6 * torch.rand(cout, generator=g.g))
+        sd[p + "_BN.bias"] = g.n(cout, std=0.3)
+        sd[p + "_BN.running_mean"] = 0.2 + 0.4 * torch.rand(cout, generator=g.g)
+        sd[p + "_BN.running_var"] = 0.4 + 0.8 * torch.rand(cout, generator=g.g)
+    sd["classifier.weight"] = g.n(360, 4 * channels[6], std=2.0 / math.sqrt(4 * channels[6]))
+    sd["classifier.bias"] = g.n(360, std=0.5)
+    return sd
