@@ -26,8 +26,6 @@ if __name__ == "__main__":
     print(args.wav)
     print(args.pit)
     require_cuda()
-    from whisper_vits_svc_b200 import crepe_infer, hostio, hubert_infer
+    from whisper_vits_svc_b200 import crepe_infer
 
-    model = crepe_infer.load_model(MODEL, "cuda")
-    audio = hubert_infer.load_audio(args.wav, crepe_infer.SAMPLE_RATE)
-    hostio.save_csv_pitch(crepe_infer.compute_f0_sing(model, audio), args.pit)
+    crepe_infer.pred_pit(crepe_infer.load_model(MODEL, "cuda"), args.wav, args.pit)

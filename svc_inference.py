@@ -4,12 +4,13 @@ svc_out.wav float32 @ hp.data.sampling_rate and svc_out_pit.wav int16 in the CWD
 device path running in libsvc_b200.so.
 
 Differences, by design (SURVEY.md §8 scope): the reference shells out to its Whisper / HuBERT /
-CREPE extractors when --ppg/--vec/--pit are missing (svc_inference.py:138-154).  Here --ppg and
---vec are produced in-process by the H100 Whisper encoder / HuBERT-Soft encoder when their
-checkpoints are available (whisper_pretrain/large-v2.pt, hubert_pretrain/hubert-soft-0d54a1f4.pt);
-CREPE is out of scope (SURVEY.md §8f-4), so --pit must be given.  --enable-retrieval reads the
-reference's faiss IVF-Flat indexes without faiss and runs the search and blend on the device
-(whisper-vits-svc_b200/retrieval.py); svc_train_retrieval.py builds those indexes on the device."""
+CREPE extractors when --ppg/--vec/--pit are missing (svc_inference.py:138-154).  Here they are produced in-process on
+the device, in the order --vec, --ppg, --pit, each model freed before the next loads: the HuBERT-Soft and Whisper
+encoders with hubert_pretrain/hubert-soft-0d54a1f4.pt and whisper_pretrain/large-v2.pt, and the CREPE-full pitch
+extractor with crepe/assets/full.pth (all in the working directory), which writes svc_tmp.pit.csv exactly as
+pitch_inference.py would.  The pitch is read back from that CSV, as in the reference, so --shift applies to it as to a
+given --pit.  --enable-retrieval reads the reference's faiss IVF-Flat indexes without faiss and runs the search and
+blend on the device (whisper-vits-svc_b200/retrieval.py); svc_train_retrieval.py builds those indexes on the device."""
 import argparse
 import logging
 import os
@@ -20,18 +21,17 @@ import numpy as np
 import torch
 from scipy.io.wavfile import write
 
+from pitch_inference import MODEL as CREPE_MODEL
 from whisper_vits_svc_b200 import hostio, hparams, models, retrieval
 
 logger = logging.getLogger(__name__)
 
 
 def main(args):
-    if args.pit is None:
-        raise SystemExit("--pit is required: the CREPE pitch extractor is out of scope of this build "
-                         "(use the reference's pitch/inference.py to produce it)")
     if not torch.cuda.is_available():
         raise SystemExit("this build has no CPU path: a CUDA (sm_90a) device is required")
     args.ppg, args.vec = hostio.extract_missing_features(args.wave, args.ppg, args.vec)
+    args.pit = hostio.extract_missing_pitch(args.wave, args.pit, CREPE_MODEL)
     logging.basicConfig(level=logging.DEBUG if args.debug else logging.INFO)
     device = torch.device("cuda")
     hp = hparams.load_hparams(args.config)

@@ -7,10 +7,15 @@ checkpoint and re-spawning the HuBERT / pitch extractors every time.  Here the m
 once per GPU, files are sharded across the ranks of a `torchrun` launch (one process per GPU, one
 NCCL broadcast of the packed weights, no collective on the data path), and per rank the chunks of ALL its
 files are sorted by length and run as full ragged device batches (hostio.BatchEngine) while host threads read
-features and write WAVs.  Missing `<name>.ppg.npy` / `<name>.vec.npy` are extracted in-process by the H100 Whisper /
-HuBERT-Soft encoders (one model load per rank).  CREPE is outside the H100 hot path (SURVEY.md §8f-4):
-`<name>.pit.csv` must sit next to `<name>.wav` (or in --feat); a file without it is reported and skipped — the
-reference would silently produce nothing for it either (subprocess exit codes are ignored there).
+features and write WAVs.
+
+Features are read from --feat (default: the wav folder) as `<stem>.ppg.npy`, `<stem>.vec.npy` and `<stem>.pit.csv`.
+Those that are missing are extracted in-process into ./_svc_out/<name>.{ppg.npy,vec.npy,pit.csv}, one model load per
+rank and only if some file needs it: first the F0 by CREPE-full (crepe/assets/full.pth, as pitch_inference.py writes it)
+in ragged device batches of whole files, then the PPG by Whisper and the units by HuBERT-Soft, file by file.  A
+`.pit.csv` in --feat, such as a hand-edited F0, is used as it is and never overwritten.  A file whose features cannot
+be made or read is reported and counted as failed, the other files are still converted, and the exit code is 1; the
+reference ignores its subprocesses' exit codes and silently produces nothing for such a file.
 
     python svc_inference_batch.py --config configs/base.yaml --model sovits5.0.pth --wave waves/ --spk singer.npy
     python -m torch.distributed.run --nproc-per-node 8 svc_inference_batch.py ...   # 8 GPUs
@@ -24,9 +29,46 @@ import numpy as np
 import torch
 from scipy.io.wavfile import write
 
-from whisper_vits_svc_b200 import hostio, hparams, models, shard
+from pitch_inference import MODEL as CREPE_MODEL
+from preprocess_crepe import MAX_PADDED
+from whisper_vits_svc_b200 import dataset, hostio, hparams, models, shard
 
 out_path = "./_svc_out"
+
+
+def feature_path(feat: str, name: str, ext: str) -> str:
+    """Where the features of wav `name` are read: `<feat>/<stem><ext>` if that file exists, else
+    `./_svc_out/<name><ext>`, where the extraction passes write them."""
+    given = os.path.join(feat, name[:-4] + ext)
+    return given if os.path.isfile(given) else os.path.join(out_path, name + ext)
+
+
+def missing_pitch(waves, mine, feat: str):
+    """The files of `mine` (indices into `waves`) whose F0 must be extracted: those without `<feat>/<stem>.pit.csv`."""
+    return [i for i in mine if not os.path.isfile(os.path.join(feat, waves[i][:-4] + ".pit.csv"))]
+
+
+def extract_pitch(model, wavs, csvs, noises=None, dithers=None, threads: int = 4, batch: int = 32):
+    """`crepe_infer.pred_pit(model, wavs[k], csvs[k])` for every k, in ragged device batches of whole files
+    (`dataset.run_batched`, as preprocess_crepe.py runs them).  `noises[k]` / `dithers[k]` are file k's random draws
+    (drawn per file when left out).  Returns the indices k that failed, each reported on stderr."""
+    from whisper_vits_svc_b200 import crepe_infer, hubert_infer
+    index = {w: k for k, w in enumerate(wavs)}
+    saved = set()
+
+    def run(items):
+        ks = [k for k, _ in items]
+        return crepe_infer.compute_f0_sing_batch(model, [a for _, a in items],
+                                                 None if noises is None else [noises[k] for k in ks],
+                                                 None if dithers is None else [dithers[k] for k in ks])
+
+    def save(wav, f0):
+        hostio.save_csv_pitch(f0, csvs[index[wav]])
+        saved.add(index[wav])
+
+    dataset.run_batched(list(wavs), lambda w: (index[w], hubert_infer.load_audio(w, crepe_infer.SAMPLE_RATE)), run, save,
+                        threads, batch, size=lambda item: item[1].shape[0], max_padded=MAX_PADDED)
+    return [k for k in range(len(wavs)) if k not in saved]
 
 
 def main():
@@ -70,20 +112,31 @@ def main():
     spk = torch.FloatTensor(np.load(args.spk))
     whisper = None
     done, failed = 0, []
+    no_pitch = set()
 
     def load(i):
         """Features of one utterance (host threads: file reads overlap the device batches)."""
         name = waves[i]
-        stem = os.path.join(feat, name[:-4])
-        ppg_p, vec_p, pit_p = stem + ".ppg.npy", stem + ".vec.npy", stem + ".pit.csv"
-        if not os.path.isfile(pit_p):
-            raise FileNotFoundError(f"{pit_p} missing (the CREPE pitch extractor is out of scope)")
-        if not os.path.isfile(ppg_p):
-            ppg_p = os.path.join(out_path, name + ".ppg.npy")     # written by the extractor pass below
-        if not os.path.isfile(vec_p):
-            vec_p = os.path.join(out_path, name + ".vec.npy")
-        ppg, vec, pit = hostio.prepare_features(ppg_p, vec_p, pit_p, args.shift)
+        if i in no_pitch:
+            raise RuntimeError("F0 extraction failed")
+        ppg, vec, pit = hostio.prepare_features(*(feature_path(feat, name, e) for e in (".ppg.npy", ".vec.npy", ".pit.csv")),
+                                                args.shift)
         return name, spk, pit, ppg, vec
+
+    # F0 pass for files that have no pitch file (one CREPE load per rank; whole files in ragged device batches)
+    bare = missing_pitch(waves, mine, feat)
+    if bare:
+        from whisper_vits_svc_b200 import crepe_infer
+        try:
+            crepe = crepe_infer.load_model(CREPE_MODEL, device)
+        except Exception as e:
+            print(f"[rank {rank}] F0 extraction FAILED ({len(bare)} files): {e}")
+            no_pitch.update(bare)
+        else:
+            lost = extract_pitch(crepe, [os.path.join(wave_path, waves[i]) for i in bare],
+                                 [os.path.join(out_path, waves[i] + ".pit.csv") for i in bare])
+            no_pitch.update(bare[k] for k in lost)
+            del crepe                   # (its device weights are freed before Whisper large-v2 loads)
 
     # PPG pass for files that have none yet (one Whisper load per rank; chunks of a file run as one batch)
     for i in mine:

@@ -15,7 +15,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from . import _lib, pack
+from . import _lib, hostio, hubert_infer, pack
 
 SAMPLE_RATE = 16000
 WINDOW = 1024
@@ -237,6 +237,13 @@ def compute_f0_sing_batch(model: CrepeB200, audios: Sequence, noises=None, dithe
 
 def compute_f0_sing(model: CrepeB200, audio, noise=None, dither=None) -> torch.Tensor:
     return compute_f0_sing_batch(model, [audio], None if noise is None else [noise], None if dither is None else [dither])[0]
+
+
+def pred_pit(model: CrepeB200, wavPath: str, pitPath: str, noise=None, dither=None):
+    """pitch/inference.py:120-130 (its __main__): the wav read at 16 kHz by `hubert_infer.load_audio`, `compute_f0_sing`,
+    and the `.pit.csv` written by `hostio.save_csv_pitch`."""
+    audio = hubert_infer.load_audio(wavPath, SAMPLE_RATE)
+    hostio.save_csv_pitch(compute_f0_sing(model, audio, noise, dither), pitPath)
 
 
 def finish_f0(pitch: torch.Tensor, periodicity: torch.Tensor) -> np.ndarray:

@@ -94,6 +94,20 @@ def extract_missing_features(wave: str, ppg: str | None, vec: str | None) -> Tup
     return ppg, vec
 
 
+def extract_missing_pitch(wave: str, pit: str | None, crepe_path: str) -> str:
+    """svc_inference.py:150-154, in process: a missing `pit` path is extracted from `wave` by the device CREPE-full
+    model (`crepe_path`, the checkpoint pitch_inference.py reads) into svc_tmp.pit.csv, as pitch_inference.py writes
+    it.  The model is freed before returning.  Returns the pit path."""
+    if pit is None:
+        from . import crepe_infer
+        pit = "svc_tmp.pit.csv"
+        print(f"Auto run : H100 CREPE pitch extractor -w {wave} -p {pit}")
+        cm = crepe_infer.load_model(crepe_path, "cuda")
+        crepe_infer.pred_pit(cm, wave, pit)
+        del cm
+    return pit
+
+
 def chunk_plan(all_frame: int, hop_size: int, out_chunk: int = 2500, hop_frame: int = 10
                ) -> List[Tuple[int, int, int, int]]:
     """The reference's chunk arithmetic (svc_inference.py:94-115,129-131) as data:
