@@ -501,12 +501,13 @@ int svcb_op_conv_tc(const float* x, const void* w_tc, const float* bias, float* 
 /* One `SnakeAlias -> Conv1d(C->C, K, dilation, same padding) + bias (+ res)` link of
  * AMPBlock.forward (vits_decoder/bigv.py:50-58) on the tensor cores: snake_pack (bf16 hi/lo operand
  * image in `scratch`) followed by the wgmma convolution.  w_tc = pack.py:pack_conv_tc image;
- * nsplit 1 = bf16, 3 = bf16x3 (parity grade). */
+ * nsplit 1 = bf16, 3 = bf16x3 (parity grade).  accum != 0: y = y_old + (conv + res), as the AMP blocks of a
+ * stage add up their outputs; out_div != 0: then y / out_div (the stage mean). */
 size_t svcb_op_amp_conv_tc_scratch_bytes(int32_t B, int32_t C, int32_t L);
 int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float* ea, const float* inv_b,
                         const float* fu, const float* fd, const void* w_tc, const float* bias, int32_t B,
-                        int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t nsplit, void* scratch,
-                        size_t scratch_bytes, svcb_stream stream);
+                        int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t nsplit, int32_t accum,
+                        float out_div, void* scratch, size_t scratch_bytes, svcb_stream stream);
 
 /* One `SnakeAlias_in -> Conv1d(C->C, K, dilation) + bias (+ res) [-> SnakeAlias_out]` link of the narrow
  * generator stages (C = 20 or 10; vits_decoder/bigv.py:50-58) in space-to-depth form (csrc/amp_s2d.cu):

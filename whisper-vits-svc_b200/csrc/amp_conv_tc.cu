@@ -168,25 +168,32 @@ int launch_snake_pack(const float* x, void* hi, void* lo, const float* ea, const
 }
 
 // ------------------------------------------------------------------------------------ amp_conv_tc
-// Persistent: each CTA walks tiles (item, 128 samples) with a static stride.
-//   producer thread  A image rows of tile i+1 (bulk copies, 1-2 buffers) and the weight tiles
-//                    (all taps resident in shared memory when they fit, else a 2-slot ring per tile)
-//   2 warpgroups     64 rows each: all taps x split parts of tile i as wgmma m64nCpk16 into register
-//                    accumulators, then +bias (+res, +stage accumulation, /3) through a shared-memory strip
-//                    (64 columns at a time) -> coalesced stores
-struct AmpPlan { int resident, nabuf, nw; size_t smem; };
-constexpr int AMP_WMAX = 2;     // weight ring depth when the taps do not stay resident
-constexpr int AMP_EPI_LD = 72;  // floats per row of an epilogue strip
-constexpr int AMP_THREADS = 288;
-constexpr size_t AMP_STRIP_BYTES = 2 * 64 * AMP_EPI_LD * 4;
+// Persistent and warp-specialised: each CTA walks tiles (item, 128 samples) with a static stride.
+//   warp 0 (one lane)  the A image rows of each tile (bulk copies, one buffer per tile in flight)
+//   warp 1 (one lane)  the weight matrices: all resident in shared memory when they fit, else a ring of 2-8 slots
+//   warpgroups 1-2     all taps x split parts as wgmma m64nCpk16 into register accumulators, then
+//                      + bias (+res, +stage accumulation, /3) stored straight from the accumulator fragments
+// Two schedules (amp_plan):
+//   ping-pong    (PP) each consumer warpgroup owns whole 128-row tiles, as two m64 accumulators: warpgroup 0 the even
+//                tiles of the CTA's walk, warpgroup 1 the odd ones, each with its own A buffer.  One warpgroup's
+//                epilogue runs while the other's MMAs keep the tensor pipe busy.
+//   cooperative  both warpgroups on one tile, 64 rows each, when two A buffers and two weight slots do not fit
+//                (C = 160) or two 128-row accumulators would not fit the registers.
+// Either way every output row sees the same wgmma sequence (tap, weight part, A part, K step) into one accumulator.
+struct AmpPlan { int pingpong, resident, nabuf, nw; size_t smem; };
+constexpr int AMP_WMAX = 8;       // weight ring depth (max) when the taps do not stay resident
+constexpr int AMP_THREADS = 384;
+constexpr int AMP_PRODUCER_REGS = 40, AMP_CONSUMER_REGS = 232;   // 128 * 40 + 256 * 232 <= 64 K registers
+constexpr int AMP_PP_MAX_C = 112;  // ping-pong: two 64 x C accumulators per warpgroup (at C = 128 they spill)
 
-template <int NC>
+template <int NC, bool PP>
 __global__ void __launch_bounds__(AMP_THREADS, 1)
 amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, const int nw) {
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t a_full[2], a_empty[2], w_full[AMP_WMAX], w_empty[AMP_WMAX], w_res;
+  __shared__ __align__(8) uint64_t a_full[2], a_empty[2], w_full[AMP_WMAX], w_empty[AMP_WMAX], w_res, order[2];
+  constexpr int MB = PP ? 2 : 1;    // 64-row accumulators per consumer warpgroup
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tc::warp_uniform_idx();
   const int P = p.dil * (p.K - 1) / 2;
   const int R = TC_M + (p.K - 1) * p.dil;
   const int KC = NC / 8;
@@ -197,152 +204,173 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
   const int nch = p.K * parts;
   uint8_t* Abase = smem;
   uint8_t* Wbase = smem + (size_t)nabuf * a_buf;
-  float* Strips = reinterpret_cast<float*>(Wbase + (size_t)(resident ? nch : nw) * wb);
   const int tpi = (p.L + TC_M - 1) / TC_M;
   const int ntiles = p.B * tpi;
 
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&a_full[i], 1); tc::mbar_init(&a_empty[i], 2); }
-    for (int i = 0; i < AMP_WMAX; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], 2); }
+    for (int i = 0; i < 2; ++i) { tc::mbar_init(&a_full[i], 1); tc::mbar_init(&a_empty[i], PP ? 1 : 2); }
+    for (int i = 0; i < AMP_WMAX; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], PP ? 1 : 2); }
     tc::mbar_init(&w_res, 1);
+    for (int i = 0; i < 2; ++i) tc::mbar_init(&order[i], 1);
     tc::fence_barrier_init();
   }
   __syncthreads();
 
-  if (tid == 256) {
-    // ---------------------------------------------------------------- producer
-    if (resident) {
-      tc::mbar_arrive_expect_tx(&w_res, wb * (uint32_t)nch);
-      for (int i = 0; i < nch; ++i)
-        tc::bulk_g2s(Wbase + (size_t)i * wb, p.wpk + ((size_t)(i / parts) * 2 + (i % parts)) * wb, wb, &w_res);
-    }
-    const uint32_t run = (uint32_t)R * 16u;
-    int it = 0, wi = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int buf = it % nabuf;
-      if (it >= nabuf) tc::mbar_wait(&a_empty[buf], (uint32_t)(((it / nabuf) - 1) & 1));
-      const int b = tile / tpi, t0 = (tile - b * tpi) * TC_M;
-      tc::mbar_arrive_expect_tx(&a_full[buf], run * KC * parts);
-      const long long row = P8_PAD + t0 - P;
-      for (int part = 0; part < parts; ++part) {
-        const uint8_t* src = reinterpret_cast<const uint8_t*>(part == 0 ? p.a_hi : p.a_lo);
-        uint8_t* dst = Abase + (size_t)buf * a_buf + (size_t)part * a_part;
-        for (int kc = 0; kc < KC; ++kc)
-          tc::bulk_g2s(dst + (size_t)kc * run, src + (((long long)b * KC + kc) * p.Lp + row) * 16, run, &a_full[buf]);
+  if (warp < 4) {
+    // ------------------------------------------------------------------ producers
+    tc::setmaxnreg_dec<AMP_PRODUCER_REGS>();
+    if (warp == 0 && tc::elect_one()) {
+      const uint32_t run = (uint32_t)R * 16u;
+      int it = 0;
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+        const int buf = it % nabuf;   // ping-pong: the buffer of the warpgroup that owns the tile
+        if (it >= nabuf) tc::mbar_wait(&a_empty[buf], (uint32_t)(((it / nabuf) - 1) & 1));
+        const int b = tile / tpi, t0 = (tile - b * tpi) * TC_M;
+        tc::mbar_arrive_expect_tx(&a_full[buf], run * KC * parts);
+        const long long row = P8_PAD + t0 - P;
+        for (int part = 0; part < parts; ++part) {
+          const uint8_t* src = reinterpret_cast<const uint8_t*>(part == 0 ? p.a_hi : p.a_lo);
+          uint8_t* dst = Abase + (size_t)buf * a_buf + (size_t)part * a_part;
+          for (int kc = 0; kc < KC; ++kc)
+            tc::bulk_g2s(dst + (size_t)kc * run, src + (((long long)b * KC + kc) * p.Lp + row) * 16, run, &a_full[buf]);
+        }
       }
-      if (!resident) {
-        for (int i = 0; i < nch; ++i, ++wi) {
-          const int st = wi % nw;
-          if (wi >= nw) tc::mbar_wait(&w_empty[st], (uint32_t)(((wi / nw) - 1) & 1));
-          tc::mbar_arrive_expect_tx(&w_full[st], wb);
-          tc::bulk_g2s(Wbase + (size_t)st * wb, p.wpk + ((size_t)(i / parts) * 2 + (i % parts)) * wb, wb, &w_full[st]);
+    } else if (warp == 1 && tc::elect_one()) {
+      if (resident) {
+        tc::mbar_arrive_expect_tx(&w_res, wb * (uint32_t)nch);
+        for (int i = 0; i < nch; ++i)
+          tc::bulk_g2s(Wbase + (size_t)i * wb, p.wpk + ((size_t)(i / parts) * 2 + (i % parts)) * wb, wb, &w_res);
+      } else {
+        // one pass over the nch matrices per tile, in the order the tiles' MMAs consume them
+        int wi = 0;
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+          for (int i = 0; i < nch; ++i, ++wi) {
+            const int st = wi % nw;
+            if (wi >= nw) tc::mbar_wait(&w_empty[st], (uint32_t)(((wi / nw) - 1) & 1));
+            tc::mbar_arrive_expect_tx(&w_full[st], wb);
+            tc::bulk_g2s(Wbase + (size_t)st * wb, p.wpk + ((size_t)(i / parts) * 2 + (i % parts)) * wb, wb, &w_full[st]);
+          }
         }
       }
     }
-  } else if (warp < 8) {
-    // ---------------------------------------------------------------- MMA + epilogue (warpgroup wg: rows 64 wg ..)
-    const int wg = warp >> 2, t = tid & 127;
-    float* strip = Strips + wg * 64 * AMP_EPI_LD;
-    const uint32_t a0 = tc::smem_u32(Abase), w0 = tc::smem_u32(Wbase);
-    const uint32_t lbo_a = (uint32_t)R * 16u, lbo_b = (uint32_t)NC * 16u;
-    const uint64_t ks_a = (2u * lbo_a) >> 4, ks_b = (2u * lbo_b) >> 4;
-    constexpr int NK = NC / 16;
-    const bool do_div = p.out_div != 0.f;
-    if (resident) tc::mbar_wait(&w_res, 0);
-    int it = 0, wi = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int buf = it % nabuf;
-      const int b = tile / tpi, t0 = (tile - b * tpi) * TC_M;
-      tc::mbar_wait(&a_full[buf], (uint32_t)((it / nabuf) & 1));
-      const uint32_t a_hi = a0 + (uint32_t)buf * a_buf + (uint32_t)wg * 64u * 16u, a_lo = a_hi + a_part;
-      float acc[NC / 2];
-#pragma unroll
-      for (int i = 0; i < NC / 2; ++i) acc[i] = 0.f;
-      int i = 0;
-      for (int tap = 0; tap < p.K; ++tap) {
-        const uint32_t tap_off = (uint32_t)(tap * p.dil) * 16u;
-        for (int part = 0; part < parts; ++part, ++i) {
-          uint32_t wbase;
-          int st = 0;
-          if (resident) {
-            wbase = w0 + (uint32_t)i * wb;
-          } else {
-            st = wi % nw;
-            tc::mbar_wait(&w_full[st], (uint32_t)((wi / nw) & 1));
-            wbase = w0 + (uint32_t)st * wb;
-          }
-          const int n_a = (part == 0 && parts == 2) ? 2 : 1;  // Wh meets Ah and Al; Wl meets Ah
-          const uint64_t bd = tc::smem_desc(wbase, lbo_b);
-          tc::wg_fence();
-          for (int ap = 0; ap < n_a; ++ap) {
-            const uint64_t ad = tc::smem_desc((ap == 0 ? a_hi : a_lo) + tap_off, lbo_a);
-#pragma unroll
-            for (int kk = 0; kk < NK; ++kk) tc::Wg<NC, 0>::ss(acc, ad + kk * ks_a, bd + kk * ks_b, 1u);
-          }
-          tc::wg_commit();
-          if (!resident) {
-            tc::wg_wait<0>();
-            if (t == 0) tc::mbar_arrive(&w_empty[st]);
-            ++wi;
-          }
-        }
-      }
-      tc::wg_wait<0>();
-      tc::wg_hold(acc);
-      if (t == 0) tc::mbar_arrive(&a_empty[buf]);
+    return;
+  }
 
-      // epilogue: thread = (row t % 64, 32-column half t / 64) of every 64-column chunk
-      const int tt = t0 + wg * 64 + (t & 63);
-      const bool live = tt < p.L;
-      const long long rowb = (long long)b * p.C * p.L + tt;
-#pragma unroll 1
-      for (int ch = 0; ch < (NC + 63) / 64; ++ch) {
-        tc::named_sync(1 + wg, 128);
-        tc::acc_to_smem<NC>(acc, strip, AMP_EPI_LD, 8 * ch, 8 * ch + 8);
-        tc::named_sync(1 + wg, 128);
-#pragma unroll 1
-        for (int sub = 0; sub < 2; ++sub) {
-          const int cl = (t >> 6) * 32 + sub * 16, c0 = ch * 64 + cl;
-          if (c0 >= NC || !live) continue;
+  // -------------------------------------------------------------------- MMA + epilogue (warpgroups 1-2)
+  tc::setmaxnreg_inc<AMP_CONSUMER_REGS>();
+  const int wg = (warp - 4) >> 2, t = tid & 127;
+  const uint32_t a0 = tc::smem_u32(Abase), w0 = tc::smem_u32(Wbase);
+  const uint32_t lbo_a = (uint32_t)R * 16u, lbo_b = (uint32_t)NC * 16u;
+  const uint64_t ks_a = (2u * lbo_a) >> 4, ks_b = (2u * lbo_b) >> 4;
+  constexpr int NK = NC / 16;
+  const bool do_div = p.out_div != 0.f;
+  if (resident) tc::mbar_wait(&w_res, 0);
+  for (int it = PP ? wg : 0;; it += PP ? 2 : 1) {
+    const int tile = blockIdx.x + it * gridDim.x;
+    if (tile >= ntiles) break;
+    const int buf = it % nabuf;
+    const int b = tile / tpi, t0 = (tile - b * tpi) * TC_M;
+    tc::mbar_wait(&a_full[buf], (uint32_t)((it / nabuf) & 1));
+    // Ping-pong: wait until the other warpgroup has issued every MMA of tile it - 1 (its ((it - 1) / 2)-th arrival
+    // here).  The two then do not share the tensor pipe, and they consume the weight stream strictly in tile order,
+    // which its parity waits need: a warpgroup that ran a tile ahead could take a slot's earlier phase for its own.
+    if (PP && it > 0) tc::mbar_wait(&order[wg], (uint32_t)(((it - 1) >> 1) & 1));
+    const uint32_t a_hi = a0 + (uint32_t)buf * a_buf + (PP ? 0u : (uint32_t)wg * 64u * 16u), a_lo = a_hi + a_part;
+    float acc[MB][NC / 2];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int co = c0 + j;
-            if (co < p.C) {
-              const long long off = rowb + (long long)co * p.L;
-              float a = 0.f;
-              if (p.res) a = p.res[off];
-              if (p.accum) a += p.y[off];
-              float o = strip[(t & 63) * AMP_EPI_LD + cl + j] + __ldg(p.bias + co) + a;
-              // a real (uniform) branch: if-converted, the division would run its x/0 slow path per element
-              if (do_div) { asm volatile(""); o = o / p.out_div; }
-              p.y[off] = o;
-            }
-          }
+    for (int m = 0; m < MB; ++m)
+#pragma unroll
+      for (int i = 0; i < NC / 2; ++i) acc[m][i] = 0.f;
+    int i = 0;
+    for (int tap = 0; tap < p.K; ++tap) {
+      const uint32_t tap_off = (uint32_t)(tap * p.dil) * 16u;
+      for (int part = 0; part < parts; ++part, ++i) {
+        uint32_t wbase;
+        int st = 0;
+        if (resident) {
+          wbase = w0 + (uint32_t)i * wb;
+        } else {
+          const int wi = it * nch + i;   // position in the weight stream
+          st = wi % nw;
+          tc::mbar_wait(&w_full[st], (uint32_t)((wi / nw) & 1));
+          wbase = w0 + (uint32_t)st * wb;
+        }
+        const int n_a = (part == 0 && parts == 2) ? 2 : 1;  // Wh meets Ah and Al; Wl meets Ah
+        const uint64_t bd = tc::smem_desc(wbase, lbo_b);
+        tc::wg_fence();
+        for (int ap = 0; ap < n_a; ++ap) {
+          const uint64_t ad = tc::smem_desc((ap == 0 ? a_hi : a_lo) + tap_off, lbo_a);
+#pragma unroll
+          for (int m = 0; m < MB; ++m)
+#pragma unroll
+            for (int kk = 0; kk < NK; ++kk) tc::Wg<NC, 0>::ss(acc[m], ad + 64u * m + kk * ks_a, bd + kk * ks_b, 1u);   // + 64 rows (address >> 4)
+        }
+        tc::wg_commit();
+        if (!resident) {
+          tc::wg_wait<0>();
+          if (t == 0) tc::mbar_arrive(&w_empty[st]);
         }
       }
+    }
+    if (PP && t == 0) tc::mbar_arrive(&order[wg ^ 1]);
+    tc::wg_wait<0>();
+#pragma unroll
+    for (int m = 0; m < MB; ++m) tc::wg_hold(acc[m]);
+    if (t == 0) tc::mbar_arrive(&a_empty[buf]);
+
+    // epilogue from the fragments: d[4 j + e] is row 16 w + l/4 + 8 (e/2), column 8 j + 2 (l%4) + e%2, so the 8 lanes
+    // of a column cover 8 consecutive samples, one 32-byte sector of [B][C][L].  All residual / stage loads are
+    // issued before the first store.
+    const int w = t >> 5, l = t & 31;
+    const long long yb = (long long)b * p.C * p.L;
+#pragma unroll
+    for (int m = 0; m < MB; ++m) {
+      const int r0 = t0 + (PP ? 64 * m : 64 * wg) + 16 * w + (l >> 2);
+      float add[NC / 2];
+#pragma unroll
+      for (int j = 0; j < NC / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int co = 8 * j + 2 * (l & 3) + (e & 1), tt = r0 + 8 * (e >> 1);
+          float a = 0.f;
+          if (co < p.C && tt < p.L) {
+            const long long off = yb + (long long)co * p.L + tt;
+            if (p.res) a = p.res[off];
+            if (p.accum) a += p.y[off];
+          }
+          add[4 * j + e] = a;
+        }
+#pragma unroll
+      for (int j = 0; j < NC / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int co = 8 * j + 2 * (l & 3) + (e & 1), tt = r0 + 8 * (e >> 1);
+          if (co < p.C && tt < p.L) {
+            float o = acc[m][4 * j + e] + __ldg(p.bias + co) + add[4 * j + e];
+            // a real (uniform) branch: if-converted, the division would run its x/0 slow path per element
+            if (do_div) { asm volatile(""); o = o / p.out_div; }
+            p.y[yb + (long long)co * p.L + tt] = o;
+          }
+        }
     }
   }
 }
 
+// Resident weights when all nch matrices fit beside two A buffers; else a weight ring of as many slots as fit
+// (2-8) beside two A buffers, or beside one (C = 160).  Ping-pong needs the two A buffers.
 static AmpPlan amp_plan(int Cp, int K, int dil, int nsplit) {
   const int R = TC_M + (K - 1) * dil;
   const int parts = nsplit == 3 ? 2 : 1;
   const size_t a_buf = (size_t)(Cp / 8) * R * 16 * parts;
   const size_t wb = (size_t)Cp * Cp * 2;
   const size_t nch = (size_t)K * parts;
-  const size_t limit = 227 * 1024 - 1024 - AMP_STRIP_BYTES;
+  const size_t limit = 227 * 1024 - 1024;
   AmpPlan pl;
-  pl.nw = 2;
-  // resident weights + 2 A buffers when they fit, else a 2-slot weight ring with 2 (or 1) A buffers, else
-  // (wide dilated taps: C = 160, k = 11, dilation 5) one A buffer and one weight slot
-  if (2 * a_buf + nch * wb + 128 <= limit) { pl.resident = 1; pl.nabuf = 2; pl.smem = 2 * a_buf + nch * wb; }
-  else {
-    pl.resident = 0;
-    pl.nabuf = (2 * a_buf + 2 * wb + 128 <= limit) ? 2 : 1;
-    if (pl.nabuf == 1 && a_buf + 2 * wb + 128 > limit) pl.nw = 1;
-    pl.smem = pl.nabuf * a_buf + pl.nw * wb;
-  }
-  pl.smem += AMP_STRIP_BYTES + 128;
+  pl.resident = 2 * a_buf + nch * wb <= limit;
+  pl.nabuf = (pl.resident || 2 * a_buf + 2 * wb <= limit) ? 2 : 1;
+  pl.nw = pl.resident ? 0 : (int)std::min<size_t>(AMP_WMAX, (limit - std::min(limit, pl.nabuf * a_buf)) / wb);
+  pl.pingpong = pl.nabuf == 2 && Cp <= AMP_PP_MAX_C;
+  pl.smem = pl.nabuf * a_buf + (pl.resident ? nch : (size_t)pl.nw) * wb + 128;
   return pl;
 }
 
@@ -358,7 +386,10 @@ int launch_amp_conv_tc(const AmpConvParams& p, cudaStream_t s) {
     return SVCB_E_BAD_SHAPE;
   }
   const AmpPlan pl = amp_plan(p.Cp, p.K, p.dil, p.nsplit);
-  if (pl.smem > 227 * 1024 - 512) { set_error("amp_conv_tc: tile does not fit shared memory"); return SVCB_E_UNSUPPORTED; }
+  if ((!pl.resident && pl.nw < 1) || pl.smem > 227 * 1024 - 512) {
+    set_error("amp_conv_tc: tile does not fit shared memory");
+    return SVCB_E_UNSUPPORTED;
+  }
   const int n_sm = device_sm_count();
   if (n_sm <= 0) { set_error("amp_conv_tc: cannot query the SM count"); return SVCB_E_CUDA; }
   const int ntiles = p.B * ((p.L + TC_M - 1) / TC_M);
@@ -368,16 +399,19 @@ int launch_amp_conv_tc(const AmpConvParams& p, cudaStream_t s) {
   snprintf(kname, sizeof(kname), "amp_conv_tc_%s_c%dk%d", p.nsplit == 3 ? "bf16x3" : "bf16", p.C, p.K);
   KernelScope ks(kname, s, 2.0 * macs,
                  (double)p.B * p.C * p.L * ((p.nsplit == 3 ? 4.0 : 2.0) + 4.0 * (p.res ? 2 : 1)));
-  switch (p.Cp / 16) {
-#define SVCB_AMP_NC(nb)                                                                                          \
-  case nb: {                                                                                                     \
+  switch (p.Cp / 16 * 2 + pl.pingpong) {
+#define SVCB_AMP_NC(nb, pp)                                                                                      \
+  case nb * 2 + pp: {                                                                                            \
     static DevSmemCache attr_cache;                                                                              \
-    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_conv_tc_kernel<16 * nb>, pl.smem, attr_cache));                          \
-    amp_conv_tc_kernel<16 * nb><<<grid, AMP_THREADS, pl.smem, s>>>(p, pl.resident, pl.nabuf, pl.nw);             \
+    SVCB_CUDA_CHECK(ensure_dyn_smem(amp_conv_tc_kernel<16 * nb, pp>, pl.smem, attr_cache));                      \
+    amp_conv_tc_kernel<16 * nb, pp><<<grid, AMP_THREADS, pl.smem, s>>>(p, pl.resident, pl.nabuf, pl.nw);         \
     break;                                                                                                       \
   }
-    SVCB_AMP_NC(1) SVCB_AMP_NC(2) SVCB_AMP_NC(3) SVCB_AMP_NC(4) SVCB_AMP_NC(5) SVCB_AMP_NC(6) SVCB_AMP_NC(7) SVCB_AMP_NC(8)
-    SVCB_AMP_NC(9) SVCB_AMP_NC(10) SVCB_AMP_NC(11) SVCB_AMP_NC(12) SVCB_AMP_NC(13) SVCB_AMP_NC(14) SVCB_AMP_NC(15) SVCB_AMP_NC(16)
+    SVCB_AMP_NC(1, 0) SVCB_AMP_NC(2, 0) SVCB_AMP_NC(3, 0) SVCB_AMP_NC(4, 0) SVCB_AMP_NC(5, 0) SVCB_AMP_NC(6, 0)
+    SVCB_AMP_NC(7, 0) SVCB_AMP_NC(8, 0) SVCB_AMP_NC(9, 0) SVCB_AMP_NC(10, 0) SVCB_AMP_NC(11, 0) SVCB_AMP_NC(12, 0)
+    SVCB_AMP_NC(13, 0) SVCB_AMP_NC(14, 0) SVCB_AMP_NC(15, 0) SVCB_AMP_NC(16, 0)
+    SVCB_AMP_NC(1, 1) SVCB_AMP_NC(2, 1) SVCB_AMP_NC(3, 1) SVCB_AMP_NC(4, 1) SVCB_AMP_NC(5, 1) SVCB_AMP_NC(6, 1)
+    SVCB_AMP_NC(7, 1)
 #undef SVCB_AMP_NC
   }
   SVCB_LAUNCH_CHECK("amp_conv_tc");

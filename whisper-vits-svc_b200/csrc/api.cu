@@ -1191,8 +1191,8 @@ size_t svcb_op_amp_conv_tc_scratch_bytes(int32_t B, int32_t C, int32_t L) { retu
 
 int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float* ea, const float* inv_b,
                         const float* fu, const float* fd, const void* w_tc, const float* bias, int32_t B,
-                        int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t nsplit, void* scratch,
-                        size_t scratch_bytes, svcb_stream stream) {
+                        int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t nsplit, int32_t accum,
+                        float out_div, void* scratch, size_t scratch_bytes, svcb_stream stream) {
   g_launches = 0;
   const size_t img = align256(p8_image_bytes(B, C, L));
   SVCB_TRY(check_workspace(scratch, scratch_bytes, 2 * img, "svcb_op_amp_conv_tc"));
@@ -1204,6 +1204,7 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
   q.a_hi = hi; q.a_lo = lo; q.Lp = p8_rows(L); q.y = y; q.res = res;
   q.wpk = static_cast<const uint8_t*>(w_tc); q.bias = bias;
   q.B = B; q.C = C; q.Cp = (C + 15) / 16 * 16; q.L = L; q.K = K; q.dil = dilation; q.nsplit = nsplit;
+  q.accum = accum; q.out_div = out_div;
   return launch_amp_conv_tc(q, s);
 }
 

@@ -68,8 +68,9 @@ def rel_attention(qkv, emb_k, emb_v, lengths, heads=2, window=4, tc=False):
     return out
 
 
-def amp_conv_tc(x, alpha, beta, fu, fd, weight, bias, dilation=1, res=None, nsplit=3):
-    """SnakeAlias -> Conv1d(C->C, K, dilation, 'same') + bias (+res) on the tensor cores."""
+def amp_conv_tc(x, alpha, beta, fu, fd, weight, bias, dilation=1, res=None, nsplit=3, acc=None, out_div=0.0):
+    """SnakeAlias -> Conv1d(C->C, K, dilation, 'same') + bias (+res) on the tensor cores.  acc: a stage sum
+    [B, C, L] that the result is added to (in a copy), then divided by out_div when it is not 0."""
     x = _c(x)
     B, C, L = x.shape
     K = weight.shape[-1]
@@ -79,11 +80,11 @@ def amp_conv_tc(x, alpha, beta, fu, fd, weight, bias, dilation=1, res=None, nspl
     wtc = pack.pack_conv_tc(weight.detach().cpu().float()).to(x.device)
     b = _c(bias)
     r = _c(res) if res is not None else None
-    y = torch.empty_like(x)
+    y = _c(acc).clone() if acc is not None else torch.empty_like(x)
     scratch = torch.empty(int(_lib.load().svcb_op_amp_conv_tc_scratch_bytes(B, C, L)), dtype=torch.uint8, device=x.device)
     _lib.call("op_amp_conv_tc", x.data_ptr(), y.data_ptr(), r.data_ptr() if r is not None else None,
               ea.data_ptr(), ib.data_ptr(), fu.data_ptr(), fd.data_ptr(),
-              wtc.data_ptr(), b.data_ptr(), B, C, L, K, dilation, nsplit,
+              wtc.data_ptr(), b.data_ptr(), B, C, L, K, dilation, nsplit, int(acc is not None), float(out_div),
               scratch.data_ptr(), scratch.numel(), device=x.device)
     return y
 
