@@ -154,7 +154,7 @@ int svcb_infer(const svcb_model* m, const float* ppg, const float* vec, const fl
  * item (B = 1, T = n_b, lengths = {n_b}, same inputs); its later samples are zero.  (svcb_infer with lengths < T keeps
  * the reference's padded-batch semantics instead: the generator there runs unmasked over all T frames.)
  * The lengths are checked on the host before any launch.  SVCB_E_UNSUPPORTED, also before any launch, unless the model
- * is at precision 3 and every generator stage takes a form with per-item ends at T and at every n_b: the tensor-core
+ * is at precision 3 and every generator stage takes the same form with per-item ends at T and at every n_b: the tensor-core
  * upsamplers (comb, fused, or tensor-core phases with the tensor-core noise conv), AMP_TC or space-to-depth AMP
  * blocks, and the fused tail (a 16-byte aligned wave); configs/base.yaml's generator does at any length.
  * ws_bytes >= svcb_workspace_bytes(m, B, T), which includes a region for the lengths.  No taps. */
@@ -514,7 +514,7 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
  * snake_pack_s2d, then the block-Toeplitz wgmma convolution whose epilogue writes y (fp32, may be NULL)
  * and — when y_act != NULL — SnakeAlias_out(result) as the next link's bf16 hi/lo operand image, returned
  * here decoded to fp32 [B,C,L].  w_s2d = pack.py:pack_conv_s2d_slots image (output columns in the kernel's
- * phase-slot order); L % (160/C) == 0. */
+ * phase-slot order); L % (160/C) == 0 and L % 8 == 0 (the scratch size is 0 for other shapes). */
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L);
 int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                          const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,

@@ -65,8 +65,7 @@ static void tc_tiling(ConvW& w) {
 }
 struct SnakeW {
   const float *ea = nullptr, *ib = nullptr, *fu = nullptr, *fd = nullptr;
-  float fu_h[12] = {0}, fd_h[12] = {0};   // host copies of the 12 + 12 alias-filter taps (read back once at model creation)
-  SnakeTapsV tapsv() const { return snake_taps_pack(fu_h, fd_h); }
+  SnakeTapsV taps = {};   // the 12 + 12 alias-filter taps by value (read back once at model creation)
 };
 
 struct EncLayer {
@@ -95,7 +94,10 @@ struct UpStage {
   int sf = 1;                // source samples per output sample: the product of the later stages' rates
   UpsForm form = UPS_POLYPHASE;
   std::vector<bool> phase_tc;   // UPS_POLYPHASE: phase r runs as conv_tc, else conv1d
+  std::vector<int> q0;          // UPS_POLYPHASE: phase r's first output (independent of L)
   NoiseForm noise_form = NOISE_IN_UPS;
+  bool ragged = false;          // stops each ragged item at its end: comb and ups_fused read it, and tensor-core phases over the
+                                // zero tail + NOISE_TC read nothing past it (SRCP is cut there)
 };
 struct ResBlock {
   ConvW c1[3], c2[3];
@@ -107,12 +109,13 @@ struct ResBlock {
   SnakeW act[6];
   int k, dil[3];
   AmpForm form = AMP_FP32;
-  AmpForm fallback = AMP_FP32;   // the form when the stage runs without s2d images (= form unless that is AMP_S2D):
-                                 // AMP_S2D needs L % s2d_r == 0 and L % 8 == 0
+  AmpForm fallback = AMP_FP32;   // the form at a length the S2D links do not fit (= form unless that is AMP_S2D)
 };
 
 // must match pack.py:s2d_factor
 static int s2d_link_factor(int ch) { return ch == 40 ? 4 : ch == 20 ? 8 : ch == 10 ? 16 : 0; }
+// The S2D links of factor r run at length L: whole rows of r samples, whole octets of rows.
+static bool s2d_fits(long long L, int r) { return L > 0 && r > 0 && L % r == 0 && L % 8 == 0; }
 
 }  // namespace svcb
 
@@ -396,61 +399,69 @@ static int run_flow(const svcb_model* m, Ctx& ctx, const float* z_p, const long 
 }
 
 // ----------------------------------------------------------------------------- generator
-// The buffers of one stage's AMP blocks.  Unit d of block j writes RA, RB, then ACC: each block adds its output to
-// the stage mean there (generator.py:188-194), the first block writes it, the others accumulate, the last divides.
-struct AmpStage {
-  const float* X;             // stage input [B, C, L]
+// The operands of one generator stage.  Its upsampler and noise conv write the stage input X from x and the source.
+// Unit d of its AMP block j writes RA, RB, then ACC: each block adds its output to the stage mean there
+// (generator.py:188-194), the first block writes it, the others accumulate, the last divides.
+struct Stage {
+  const float* x;             // the previous stage's output [B, 2C, L / rate]
+  float* X;                   // stage input [B, C, L]
   float* ACC;
-  float *T1, *T2, *RA, *RB;   // fp32 temporaries [B, C, L]
+  float *T1, *T2, *RA, *RB;   // fp32 temporaries [B, C, L]; T1 also holds UPS_POLYPHASE's phases
   void *img_hi, *img_lo;      // snake_pack operand images (AMP_TC)
   void* s2d[4];               // two ping-pong S2D images, hi and lo each (AMP_S2D)
-  int B, C, L, nres, nsplit;
-  const int* lens;            // ragged batch (AMP_TC, AMP_S2D): item b ends at lens[b] * lscale samples, or null
-  int lscale;
+  const float *source, *SRCP; // [B][Ltot]; [B][Lpad] from SRC_PADF samples before the source, zero-padded (tensor-core forms)
+  long long Ltot, Lpad;
+  int B, C, L, nres, nsplit, hop, lscale;
+  const int* lens;            // ragged batch (UPS_FUSED, AMP_TC, AMP_S2D): item b ends at lens[b] * lscale samples, or null
+  const long long* len64;     // ragged batch (UPS_COMB): item b's length at the upsampler's input rate in len64[b], or null
   float* out(int d) const { return d == 0 ? RA : d == 1 ? RB : ACC; }
   bool accum(int d, int j) const { return d == 2 && j > 0; }
   float out_div(int d, int j) const { return d == 2 && j == nres - 1 ? (float)nres : 0.f; }
 };
 
-// Link `half` of unit d: c1[d] from S2D image 0 to image 1, or c2[d] from image 1 to image 0 (a.s2d = hi, lo of each);
-// the output image is the SnakeAlias that follows the conv, none after the block's last one.
-static AmpS2dParams s2d_link(const AmpStage& a, const ResBlock& R, int d, int half) {
-  void* const* in = a.s2d + 2 * half;
-  void* const* out = a.s2d + 2 - 2 * half;
-  const int next = 2 * d + 1 + half;   // the SnakeAlias after this conv
+// An amp_s2d_link over the S2D image in = (hi, lo) of x[B, C, L]; with act, its epilogue also writes act(result) as the
+// image out = (hi, lo).  The caller sets the weights, their tap plan, the bias, res and y.
+static AmpS2dParams s2d_link_params(int B, int C, int L, int K, void* const* in, void* const* out, const SnakeW* act) {
   AmpS2dParams q;
-  q.B = a.B; q.C = a.C; q.L = a.L; q.K = R.k; q.Rp = s2d_rows(a.L, R.s2d_r);
+  q.B = B; q.C = C; q.L = L; q.K = K; q.Rp = s2d_rows(L, s2d_link_factor(C));
   q.a_hi = in[0]; q.a_lo = in[1];
-  q.wpk = half ? R.c2_s2d[d] : R.c1_s2d[d]; q.bias = half ? R.c2[d].b : R.c1[d].b;
-  q.ntaps = half ? R.s2d_nt2[d] : R.s2d_nt1[d]; q.mlo = half ? R.s2d_ml2[d] : R.s2d_ml1[d];
-  q.tap_cols = half ? R.s2d_tc2[d] : R.s2d_tc1[d];
-  q.lens = a.lens; q.lscale = a.lscale;
-  if (next < 6) {
-    const SnakeW& act = R.act[next];
+  if (act) {
     q.o_hi = out[0]; q.o_lo = out[1];
-    q.ea = act.ea; q.ib = act.ib; q.fu = act.fu; q.fd = act.fd; q.taps = act.tapsv();
+    q.ea = act->ea; q.ib = act->ib; q.fu = act->fu; q.fd = act->fd; q.taps = act->taps;
   }
   return q;
 }
 
-// narrow stages: every link = block-Toeplitz wgmma conv with the next SnakeAlias in its epilogue
-static int run_amp_s2d(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+// An amp_conv_tc link over the snake_pack image (hi, lo) of x[B, C, L]; the caller sets the weights and the epilogue.
+static AmpConvParams amp_conv_params(const void* hi, const void* lo, int B, int C, int L, int K, int nsplit) {
+  AmpConvParams q;
+  q.a_hi = hi; q.a_lo = lo; q.Lp = p8_rows(L);
+  q.B = B; q.C = C; q.Cp = (C + 15) / 16 * 16; q.L = L; q.K = K; q.nsplit = nsplit;
+  return q;
+}
+
+// narrow stages: every link = block-Toeplitz wgmma conv with the next SnakeAlias in its epilogue.  Link k = 2d + half
+// is c1[d] from S2D image 0 to image 1 or c2[d] from image 1 to image 0 (a.s2d = hi, lo of each); its output image is
+// SnakeAlias k + 1, none after the block's last conv.
+static int run_amp_s2d(Ctx& ctx, const Stage& a, const ResBlock& R, int j) {
   const SnakeW& s0 = R.act[0];
-  const SnakeTapsV tv0 = s0.tapsv();
-  RUN(launch_snake_pack_s2d(a.X, a.s2d[0], a.s2d[1], s0.ea, s0.ib, s0.fu, s0.fd, a.B, a.C, a.L, ctx.stream, &tv0, a.lens, a.lscale));
+  RUN(launch_snake_pack_s2d(a.X, a.s2d[0], a.s2d[1], s0.ea, s0.ib, s0.fu, s0.fd, a.B, a.C, a.L, ctx.stream, &s0.taps, a.lens, a.lscale));
   const float* cur = a.X;
-  for (int d = 0; d < 3; ++d) {
-    RUN(launch_amp_s2d_link(s2d_link(a, R, d, 0), ctx.stream));
-    AmpS2dParams q = s2d_link(a, R, d, 1);
-    q.res = cur; q.y = a.out(d); q.accum = a.accum(d, j); q.out_div = a.out_div(d, j);
+  for (int k = 0; k < 6; ++k) {
+    const int d = k / 2, half = k % 2;
+    AmpS2dParams q = s2d_link_params(a.B, a.C, a.L, R.k, a.s2d + 2 * half, a.s2d + 2 - 2 * half, k < 5 ? &R.act[k + 1] : nullptr);
+    q.wpk = half ? R.c2_s2d[d] : R.c1_s2d[d]; q.bias = half ? R.c2[d].b : R.c1[d].b;
+    q.ntaps = half ? R.s2d_nt2[d] : R.s2d_nt1[d]; q.mlo = half ? R.s2d_ml2[d] : R.s2d_ml1[d];
+    q.tap_cols = half ? R.s2d_tc2[d] : R.s2d_tc1[d];
+    q.lens = a.lens; q.lscale = a.lscale;
+    if (half) { q.res = cur; q.y = a.out(d); q.accum = a.accum(d, j); q.out_div = a.out_div(d, j); cur = q.y; }
     RUN(launch_amp_s2d_link(q, ctx.stream));
-    cur = q.y;
   }
   return SVCB_OK;
 }
 
 // narrow stages: the whole block (6 convs + 6 SnakeAlias + residuals) in one fp32 kernel
-static int run_amp_block_fused(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+static int run_amp_block_fused(Ctx& ctx, const Stage& a, const ResBlock& R, int j) {
   AmpBlockParams q;
   q.x = a.X; q.y = a.ACC; q.B = a.B; q.C = a.C; q.L = a.L; q.K = R.k;
   for (int d = 0; d < 3; ++d) {
@@ -465,20 +476,17 @@ static int run_amp_block_fused(Ctx& ctx, const AmpStage& a, const ResBlock& R, i
 }
 
 // tensor-core path: snake_pack -> amp_conv_tc, twice per unit
-static int run_amp_tc(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+static int run_amp_tc(Ctx& ctx, const Stage& a, const ResBlock& R, int j) {
   void* lo = a.nsplit == 3 ? a.img_lo : nullptr;
   const float* cur = a.X;
   for (int d = 0; d < 3; ++d) {
     const SnakeW& s1 = R.act[2 * d];
     const SnakeW& s2 = R.act[2 * d + 1];
-    AmpConvParams q;
-    q.B = a.B; q.C = a.C; q.Cp = (a.C + 15) / 16 * 16; q.L = a.L; q.K = R.k; q.nsplit = a.nsplit;
-    q.Lp = p8_rows(a.L); q.a_hi = a.img_hi; q.a_lo = lo;
-    const SnakeTapsV tv1 = s1.tapsv(), tv2 = s2.tapsv();
-    RUN(launch_snake_pack(cur, a.img_hi, lo, s1.ea, s1.ib, s1.fu, s1.fd, a.B, a.C, a.L, ctx.stream, &tv1, a.lens, a.lscale));
+    AmpConvParams q = amp_conv_params(a.img_hi, lo, a.B, a.C, a.L, R.k, a.nsplit);
+    RUN(launch_snake_pack(cur, a.img_hi, lo, s1.ea, s1.ib, s1.fu, s1.fd, a.B, a.C, a.L, ctx.stream, &s1.taps, a.lens, a.lscale));
     q.y = a.T2; q.wpk = R.c1_tc[d]; q.bias = R.c1[d].b; q.dil = R.dil[d];
     RUN(launch_amp_conv_tc(q, ctx.stream));
-    RUN(launch_snake_pack(a.T2, a.img_hi, lo, s2.ea, s2.ib, s2.fu, s2.fd, a.B, a.C, a.L, ctx.stream, &tv2, a.lens, a.lscale));
+    RUN(launch_snake_pack(a.T2, a.img_hi, lo, s2.ea, s2.ib, s2.fu, s2.fd, a.B, a.C, a.L, ctx.stream, &s2.taps, a.lens, a.lscale));
     q.wpk = R.c2_tc[d]; q.bias = R.c2[d].b; q.dil = 1; q.res = cur;
     q.y = a.out(d); q.accum = a.accum(d, j); q.out_div = a.out_div(d, j);
     RUN(launch_amp_conv_tc(q, ctx.stream));
@@ -487,7 +495,7 @@ static int run_amp_tc(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
   return SVCB_OK;
 }
 
-static int run_amp_fp32(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
+static int run_amp_fp32(Ctx& ctx, const Stage& a, const ResBlock& R, int j) {
   const float* cur = a.X;
   for (int d = 0; d < 3; ++d) {
     const SnakeW& s1 = R.act[2 * d];
@@ -503,6 +511,97 @@ static int run_amp_fp32(Ctx& ctx, const AmpStage& a, const ResBlock& R, int j) {
   return SVCB_OK;
 }
 
+// wide stages: every phase AND the stage's noise conv in one tensor-core conv whose epilogue stores the interleaved
+// samples — the stage input is read once, X is written once
+static int run_ups_comb(Ctx& ctx, const UpStage& us, const Stage& a) {
+  const int C = 2 * a.C, L = a.L / us.rate;
+  ConvTcParams q = conv_tc_params(us.comb, a.x, (long long)C * L, L, 1, a.X, a.B, L, L, 1, us.taps - 1, a.nsplit);
+  q.Cin = C; q.ilv = us.rate;
+  q.x2 = a.SRCP + (SRC_PADF - us.sf / 2); q.sx2b = a.Lpad; q.sx2t = (long long)us.sf * us.rate;
+  q.cin1 = us.comb_cin1; q.cin2 = us.comb_cin2;
+  // ragged: rows past an item's end read as zero in both inputs; a lone call's row bound (tau < Tin) also drops
+  // the source window of the row at its end, whose first sf/2 samples precede that end
+  if (a.len64) { q.lengths = a.len64; q.flags = CONV_IN_MASK; }
+  RUN(launch_conv_tc(q, ctx.stream));
+  return SVCB_OK;
+}
+
+// narrow stages: transposed conv + noise conv + biases in one fp32 pass
+static int run_ups_fused(Ctx& ctx, const UpStage& us, const Stage& a) {
+  UpsFusedParams q;
+  q.x = a.x; q.wph[0] = us.phase[0].w; q.wph[1] = us.phase[1].w; q.bias = us.bias;
+  q.src = a.source; q.wn = us.noise.w; q.bn = us.noise.b; q.y = a.X;
+  q.B = a.B; q.Cin = 2 * a.C; q.Cout = a.C; q.L = a.L / us.rate; q.Ln = a.L; q.rate = us.rate; q.M = us.taps; q.pad = us.pad;
+  q.cout_pad = us.phase[0].cout_pad; q.Kn = us.noise.k; q.sf = us.sf; q.padn = us.sf / 2;
+  q.cout_pad_n = us.noise.cout_pad; q.Ltot = a.Ltot;
+  q.lens = a.lens; q.src_scale = a.hop;
+  RUN(launch_ups_fused(q, ctx.stream));
+  return SVCB_OK;
+}
+
+// `rate` polyphase sub-convolutions, each into its own contiguous slab of T1 (coalesced), interleaved + biased
+// + (short) noise conv by ups_finalize
+static int run_ups_polyphase(Ctx& ctx, const UpStage& us, const Stage& a) {
+  const int C = 2 * a.C, L = a.L / us.rate;
+  UpsFinalizeParams fp;
+  fp.bias = us.bias; fp.y = a.X; fp.C = a.C; fp.Ln = a.L; fp.rate = us.rate; fp.pad = us.pad;
+  fp.src = us.noise_form == NOISE_IN_UPS ? a.source : nullptr; fp.wn = us.noise.w; fp.bn = us.noise.b;
+  fp.Kn = us.noise.k; fp.sf = us.sf; fp.padn = us.sf / 2; fp.cout_pad = us.noise.cout_pad; fp.Ltot = a.Ltot;
+  size_t slab = 0;
+  for (int r = 0; r < us.rate; ++r) {
+    ConvParams p = std_conv(us.phase[r], a.x, nullptr, a.B, L, a.L, us.taps - 1);
+    p.q0 = us.q0[r];
+    p.nq = (a.L - 1 + us.pad - r) / us.rate - p.q0 + 1;   // up to the last output q of phase r
+    p.y = a.T1 + slab;
+    p.syb = (long long)a.C * p.nq; p.syc = p.nq; p.syt = 1;
+    fp.tmp[r] = p.y; fp.nq[r] = p.nq; fp.q0[r] = p.q0;
+    slab += (size_t)a.B * a.C * p.nq;
+    if (us.phase_tc[r]) {
+      // phase r is a stride-1 convolution with nq == L outputs: x index = t + j - (taps-1-q0)
+      RUN(launch_conv_tc(conv_tc_params(us.phase[r], a.x, (long long)C * L, L, 1, p.y, a.B, L, L, 1, us.taps - 1 - p.q0, a.nsplit), ctx.stream));
+    } else {
+      RUN(launch_conv1d(p, ctx.stream));
+    }
+  }
+  RUN(launch_ups_finalize(fp, a.B, ctx.stream));
+  return SVCB_OK;
+}
+
+// long noise filter as Conv1d(sf -> C, K=2) over the space-to-depth view of the padded source:
+// x[b, ci, t] = srcp[b][32 - sf/2 + sf*t + ci]
+static int run_noise_tc(Ctx& ctx, const UpStage& us, const Stage& a) {
+  ConvTcParams q = conv_tc_params(us.noise_tc, a.SRCP + (SRC_PADF - us.sf / 2), a.Lpad, 1, us.sf, a.X, a.B, a.L + 1, a.L, 1, 0, a.nsplit);
+  q.flags = CONV_ACCUM;
+  RUN(launch_conv_tc(q, ctx.stream));
+  return SVCB_OK;
+}
+
+// long noise filters (K = 2*prod(later rates)): separate accumulate pass
+static int run_noise_conv1d(Ctx& ctx, const UpStage& us, const Stage& a) {
+  ConvParams p = std_conv(us.noise, a.source, a.X, a.B, (int)a.Ltot, a.L, us.sf / 2, 1, us.sf);
+  p.flags = CONV_ACCUM;
+  RUN(launch_conv1d(p, ctx.stream));
+  return SVCB_OK;
+}
+
+// What the generator launches at T frames where that depends on the length: each AMP block's form (resolve()'s `form`
+// where the S2D links fit the stage's length, else its `fallback`) and whether the tail runs as post_fused.  Everything
+// else resolve() chose at model creation.  wave: where the tail writes (post_fused needs it 16-byte aligned).
+struct GenPlan {
+  AmpForm amp[SVCB_MAX_UPS * SVCB_MAX_RES];   // block j of stage i at i * n_res + j, as svcb_model::res
+  bool post_fused;
+  GenPlan(const svcb_model* m, long long T, const float* wave) {
+    const svcb_config& c = m->cfg;
+    long long L = T;
+    for (int i = 0; i < c.n_ups; ++i) {
+      L *= c.up_rates[i];
+      for (int j = i * c.n_res; j < (i + 1) * c.n_res; ++j) amp[j] = s2d_fits(L, m->res[j].s2d_r) ? m->res[j].form : m->res[j].fallback;
+    }
+    // the stage mean the tail reads is an arena buffer, 256-byte aligned
+    post_fused = !m->conv_post.b && post_fused_supported(m->conv_post.cin, (int)L, m->conv_post.k, wave, wave);
+  }
+};
+
 // A ragged batch (svcb_infer_ragged) passes its lengths as lens (int32 frames, for the generator's own kernels) and
 // len64 ([n_ups + 1][B] int64: item b's length at the input rate of stage i in row i, for zero_tail and conv_tc) and has
 // been checked by ragged_forms(): every stage takes a form that reads them.  Item b then ends at its own length at
@@ -511,6 +610,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
                          const float* source, float* wave, int B, int T, const long long* len64 = nullptr,
                          const int* lens = nullptr, int min_n = 0) {
   const svcb_config& c = m->cfg;
+  const GenPlan plan(m, T, wave);
   cudaStream_t s = ctx.stream;
   const int U = c.gen_input;
   const int nsplit = m->nsplit;
@@ -562,78 +662,28 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
   int L = T;
   for (int i = 0; i < c.n_ups; ++i) {
     const UpStage& us = m->ups[i];
-    const int chn = ch / 2, Ln = L * us.rate, sf = us.sf;
+    const int chn = ch / 2, Ln = L * us.rate;
     float* X = ctx.alloc<float>((size_t)B * chn * Ln);
     float* ACC = ctx.alloc<float>((size_t)B * chn * Ln);
     SVCB_TRY(ctx.check());
-    // ups[i](x) (ConvTranspose1d, generator.py:183) + noise_convs[i](source) (generator.py:185-186)
-    if (us.form == UPS_COMB) {
-      // wide stages: every phase AND the stage's noise conv in one tensor-core conv whose epilogue stores the
-      // interleaved samples — the stage input is read once, X is written once
-      ConvTcParams q = conv_tc_params(us.comb, x, (long long)ch * L, L, 1, X, B, L, L, 1, us.taps - 1, nsplit);
-      q.Cin = ch; q.ilv = us.rate;
-      q.x2 = SRCP + (SRC_PADF - sf / 2); q.sx2b = Lpad; q.sx2t = (long long)sf * us.rate;
-      q.cin1 = us.comb_cin1; q.cin2 = us.comb_cin2;
-      // ragged: rows past an item's end read as zero in both inputs; a lone call's row bound (tau < Tin) also drops
-      // the source window of the row at its end, whose first sf/2 samples precede that end
-      if (len64) { q.lengths = len64 + (size_t)i * B; q.flags = CONV_IN_MASK; }
-      RUN(launch_conv_tc(q, s));
-    } else if (us.form == UPS_FUSED) {  // narrow stages: transposed conv + noise conv + biases in one fp32 pass
-      UpsFusedParams q;
-      q.x = x; q.wph[0] = us.phase[0].w; q.wph[1] = us.phase[1].w; q.bias = us.bias;
-      q.src = source; q.wn = us.noise.w; q.bn = us.noise.b; q.y = X;
-      q.B = B; q.Cin = ch; q.Cout = chn; q.L = L; q.Ln = Ln; q.rate = us.rate; q.M = us.taps; q.pad = us.pad;
-      q.cout_pad = us.phase[0].cout_pad; q.Kn = us.noise.k; q.sf = sf; q.padn = sf / 2;
-      q.cout_pad_n = us.noise.cout_pad; q.Ltot = Ltot;
-      q.lens = lens; q.src_scale = m->hop;
-      RUN(launch_ups_fused(q, s));
-    } else {
-      // `rate` polyphase sub-convolutions, each into its own contiguous slab of T1 (coalesced), interleaved + biased
-      // + (short) noise conv by ups_finalize
-      UpsFinalizeParams fp;
-      fp.bias = us.bias; fp.y = X; fp.C = chn; fp.Ln = Ln; fp.rate = us.rate; fp.pad = us.pad;
-      fp.src = us.noise_form == NOISE_IN_UPS ? source : nullptr; fp.wn = us.noise.w; fp.bn = us.noise.b;
-      fp.Kn = us.noise.k; fp.sf = sf; fp.padn = sf / 2; fp.cout_pad = us.noise.cout_pad; fp.Ltot = Ltot;
-      size_t slab = 0;
-      for (int r = 0; r < us.rate; ++r) {
-        ConvParams p = std_conv(us.phase[r], x, nullptr, B, L, Ln, us.taps - 1);
-        const int pr = us.pad - r;
-        p.q0 = pr > 0 ? (pr + us.rate - 1) / us.rate : 0;
-        const int qmax = (Ln - 1 + us.pad - r) / us.rate;
-        p.nq = qmax - p.q0 + 1;
-        p.y = T1 + slab;
-        p.syb = (long long)chn * p.nq; p.syc = p.nq; p.syt = 1;
-        fp.tmp[r] = p.y; fp.nq[r] = p.nq; fp.q0[r] = p.q0;
-        slab += (size_t)B * chn * p.nq;
-        if (us.phase_tc[r]) {
-          // phase r is a stride-1 convolution with nq == L outputs: x index = t + j - (taps-1-q0)
-          RUN(launch_conv_tc(conv_tc_params(us.phase[r], x, (long long)ch * L, L, 1, p.y, B, L, L, 1, us.taps - 1 - p.q0, nsplit), s));
-        } else {
-          RUN(launch_conv1d(p, s));
-        }
-      }
-      if (!ctx.dry) SVCB_TRY(launch_ups_finalize(fp, B, s));
+    Stage a{x, X, ACC, T1, T2, RA, RB, IMG_HI, IMG_LO, {nullptr, nullptr, nullptr, nullptr}, source, SRCP, Ltot, Lpad,
+            B, chn, Ln, c.n_res, nsplit, m->hop, Ln / T, lens, len64 ? len64 + (size_t)i * B : nullptr};
+    switch (us.form) {
+      case UPS_COMB: SVCB_TRY(run_ups_comb(ctx, us, a)); break;
+      case UPS_FUSED: SVCB_TRY(run_ups_fused(ctx, us, a)); break;
+      case UPS_POLYPHASE: SVCB_TRY(run_ups_polyphase(ctx, us, a)); break;
     }
-    if (us.noise_form == NOISE_TC) {
-      // long noise filter as Conv1d(sf -> C, K=2) over the space-to-depth view of the padded source:
-      // x[b, ci, t] = srcp[b][32 - sf/2 + sf*t + ci]
-      ConvTcParams q = conv_tc_params(us.noise_tc, SRCP + (SRC_PADF - sf / 2), Lpad, 1, sf, X, B, Ln + 1, Ln, 1, 0, nsplit);
-      q.flags = CONV_ACCUM;
-      RUN(launch_conv_tc(q, s));
-    } else if (us.noise_form == NOISE_CONV1D) {  // long noise filters (K = 2*prod(later rates)): separate accumulate pass
-      ConvParams p = std_conv(us.noise, source, X, B, (int)Ltot, Ln, sf / 2, 1, sf);
-      p.flags = CONV_ACCUM;
-      RUN(launch_conv1d(p, s));
+    switch (us.noise_form) {
+      case NOISE_IN_UPS: break;
+      case NOISE_TC: SVCB_TRY(run_noise_tc(ctx, us, a)); break;
+      case NOISE_CONV1D: SVCB_TRY(run_noise_conv1d(ctx, us, a)); break;
     }
     SVCB_TRY(tap(ctx, SVCB_TAP_GEN_UP0 + i, X, (size_t)B * chn * Ln));
 
     const ResBlock* rb = &m->res[(size_t)i * c.n_res];
-    AmpStage a{X, ACC, T1, T2, RA, RB, IMG_HI, IMG_LO, {nullptr, nullptr, nullptr, nullptr}, B, chn, Ln, c.n_res, nsplit,
-               lens, Ln / T};
-    // every block of a stage has the same channel count, so either all or none take the s2d form
-    const bool s2d = rb[0].form == AMP_S2D && Ln % rb[0].s2d_r == 0 && Ln % 8 == 0;
+    const AmpForm* forms = &plan.amp[(size_t)i * c.n_res];
     const size_t mark = ctx.off;
-    if (s2d) {
+    if (forms[0] == AMP_S2D) {   // (every block of a stage has the same channel count: all or none take this form)
       // two ping-pong S2D images (hi, lo each), cleared once per stage: rows outside the sequences are the
       // convolutions' zero padding and are never written by the link kernels
       const size_t ib = s2d_image_bytes(B, Ln, rb[0].s2d_r);
@@ -647,7 +697,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
     }
     for (int j = 0; j < c.n_res; ++j) {
       const ResBlock& R = rb[j];
-      switch (s2d ? R.form : R.fallback) {
+      switch (forms[j]) {
         case AMP_S2D: SVCB_TRY(run_amp_s2d(ctx, a, R, j)); break;
         case AMP_BLOCK_FUSED: SVCB_TRY(run_amp_block_fused(ctx, a, R, j)); break;
         case AMP_TC: SVCB_TRY(run_amp_tc(ctx, a, R, j)); break;
@@ -661,8 +711,8 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
     x = ACC; ch = chn; L = Ln;
   }
   // activation_post + conv_post + tanh (generator.py:196-199)
-  if (!m->conv_post.b && post_fused_supported(ch, L, m->conv_post.k, x, wave)) {
-    RUN(launch_post_fused(x, wave, m->post_act.ea, m->post_act.ib, m->post_act.tapsv(), m->conv_post_h.data(), B, ch, L, s,
+  if (plan.post_fused) {
+    RUN(launch_post_fused(x, wave, m->post_act.ea, m->post_act.ib, m->post_act.taps, m->conv_post_h.data(), B, ch, L, s,
                           lens, L / T));
     return SVCB_OK;
   }
@@ -736,21 +786,20 @@ struct Resolver : BlobTensors {
     w.cin = cin; w.cout = cout; w.k = k; w.cout_pad = (cout + 7) / 8 * 8;
     w.w = get(prefix + ".w", (uint64_t)cin * k * w.cout_pad);
     w.b = bias ? get(prefix + ".b", cout) : nullptr;
-    if (tc) {
-      tc_tiling(w);
-      const uint64_t numel = (uint64_t)k * 2 * w.cin_pad * w.ntiles * w.bn / 2;
-      w.tc = reinterpret_cast<const uint8_t*>(get(prefix + ".tc", numel));
-    }
+    if (tc) tc_image(w, prefix + ".tc", cin, cout, k);
     return w;
+  }
+  // w as a conv of cin -> cout channels and k taps with its tensor-core tile image (pack.py:pack_conv_tc_general)
+  void tc_image(ConvW& w, const std::string& name, int cin, int cout, int k) {
+    w.cin = cin; w.cout = cout; w.k = k; w.cout_pad = (cout + 7) / 8 * 8;
+    tc_tiling(w);
+    w.tc = reinterpret_cast<const uint8_t*>(get(name, (uint64_t)w.k * 2 * w.cin_pad * w.ntiles * w.bn / 2));
   }
   SnakeW snake(const std::string& prefix, int ch) {
     SnakeW s;
     s.ea = get(prefix + ".ea", ch); s.ib = get(prefix + ".ib", ch);
     s.fu = get(prefix + ".fu", 12); s.fd = get(prefix + ".fd", 12);
-    if (s.fu && s.fd && (cudaMemcpy(s.fu_h, s.fu, 12 * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
-                         cudaMemcpy(s.fd_h, s.fd, 12 * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)) {
-      fail(prefix + ".fu/.fd (device read-back failed)");
-    }
+    if (s.fu && s.fd && snake_taps_from_device(s.fu, s.fd, &s.taps) != SVCB_OK) fail(prefix + ".fu/.fd (device read-back failed)");
     return s;
   }
 };
@@ -814,29 +863,17 @@ static int resolve(svcb_model* m, Resolver& R) {
       us.phase.push_back(R.conv(p + ".ph" + std::to_string(r), ch, ch / 2, us.taps, false, true));
     us.bias = R.get(p + ".b", ch / 2);
     if (us.rate == 4 && us.taps == 2 && i + 1 < c.n_ups) {   // must match pack.py:pack_svc_state_dict (+ the stage's noise conv)
-      ConvW& w = us.comb;
       us.comb_cin1 = (ch + 31) / 32 * 32;
       us.comb_cin2 = us.rate * us.sf + us.sf;         // source samples a frame's rate outputs reach (filter 2 sf, stride sf)
-      w.cin = us.comb_cin1 + us.comb_cin2; w.cout = us.rate * (ch / 2); w.k = us.taps + 1; w.cout_pad = (w.cout + 7) / 8 * 8;
-      tc_tiling(w);
-      w.tc = reinterpret_cast<const uint8_t*>(R.get(p + ".comb.tc", (uint64_t)w.k * 2 * w.cin_pad * w.ntiles * w.bn / 2));
-      w.b = R.get(p + ".comb.b", w.cout);
+      R.tc_image(us.comb, p + ".comb.tc", us.comb_cin1 + us.comb_cin2, us.rate * (ch / 2), us.taps + 1);
+      us.comb.b = R.get(p + ".comb.b", us.comb.cout);
     }
-    ch /= 2;
-  }
-  ch = c.gen_initial_channel;
-  for (int i = 0; i < c.n_ups; ++i) {
-    UpStage& us = m->ups[i];
     const int sf = us.sf;
     const int nk = (i + 1 == c.n_ups) ? 1 : 2 * sf;
     us.noise = R.conv("dec.noise." + std::to_string(i), 1, ch / 2, nk);
     if (nk > 8) {
-      ConvW& w = us.noise_tc;
-      w.cin = sf; w.cout = ch / 2; w.k = 2; w.cout_pad = (w.cout + 7) / 8 * 8;
-      tc_tiling(w);
-      w.tc = reinterpret_cast<const uint8_t*>(
-          R.get("dec.noise." + std::to_string(i) + ".tc", (uint64_t)2 * 2 * w.cin_pad * w.ntiles * w.bn / 2));
-      w.b = us.noise.b;
+      R.tc_image(us.noise_tc, "dec.noise." + std::to_string(i) + ".tc", sf, ch / 2, 2);
+      us.noise_tc.b = us.noise.b;
     }
     // the stage's kernels (comb and noise_tc exist only for stages before the last)
     if (tc && nk <= 8 && ups_fused_supported(ch, ch / 2, us.rate, us.taps, nk)) us.form = UPS_FUSED;
@@ -844,12 +881,13 @@ static int resolve(svcb_model* m, Resolver& R) {
     else us.form = UPS_POLYPHASE;
     // phase r's outputs start at q0 (independent of L); with pad >= 0 it has exactly L of them, a stride-1 conv
     for (int r = 0; r < us.rate; ++r) {
-      const int q0 = us.pad - r > 0 ? (us.pad - r + us.rate - 1) / us.rate : 0;
-      us.phase_tc.push_back(tc && us.phase[r].tc && us.pad >= 0 && us.taps - 1 - q0 >= 0);
+      us.q0.push_back(us.pad - r > 0 ? (us.pad - r + us.rate - 1) / us.rate : 0);
+      us.phase_tc.push_back(tc && us.phase[r].tc && us.pad >= 0 && us.taps - 1 - us.q0[r] >= 0);
     }
     if (us.form != UPS_POLYPHASE || nk <= 8) us.noise_form = NOISE_IN_UPS;
     else if (tc && us.noise_tc.tc && sf <= 2 * SRC_PADF) us.noise_form = NOISE_TC;
     else us.noise_form = NOISE_CONV1D;
+    us.ragged = us.form != UPS_POLYPHASE || (us.noise_form == NOISE_TC && !std::count(us.phase_tc.begin(), us.phase_tc.end(), false));
     ch /= 2;
   }
   m->res.resize((size_t)c.n_ups * c.n_res);
@@ -898,48 +936,26 @@ static int resolve(svcb_model* m, Resolver& R) {
   return SVCB_OK;
 }
 
-// svcb_infer_ragged: SVCB_E_UNSUPPORTED unless every generator stage takes, at T frames and at each item's own n[b], a
-// form that reads per-item ends (precision 3: the tensor-core upsamplers, AMP_TC or AMP_S2D, post_fused).
+// svcb_infer_ragged: SVCB_E_UNSUPPORTED unless the model is at precision 3, every upsampler stops items at their own ends,
+// and the generator's plan at T frames takes only forms that do (AMP_TC, AMP_S2D, post_fused) and is its plan at every n[b].
 static int ragged_forms(const svcb_model* m, const int32_t* n, int B, int T, const float* wave) {
-  const std::string who = "svcb_infer_ragged: ";
   const svcb_config& c = m->cfg;
-  if (m->nsplit != 3) {
-    set_error(who + "needs a model at precision 3; this one has precision " + std::to_string(c.precision));
-    return SVCB_E_UNSUPPORTED;
-  }
-  int ch = c.gen_initial_channel;
-  long long f = 1;   // samples per frame after stage i
+  const auto reject = [](const std::string& why) { set_error("svcb_infer_ragged: " + why); return SVCB_E_UNSUPPORTED; };
+  const auto stage = [](int k) { return "generator stage " + std::to_string(k); };
+  if (m->nsplit != 3) return reject("needs a model at precision 3; this one has precision " + std::to_string(c.precision));
+  const std::string tail = "the generator's tail needs post_fused (a 16-byte aligned wave and 8 | samples)";
+  const GenPlan plan(m, T, wave);
   for (int i = 0; i < c.n_ups; ++i) {
-    const UpStage& us = m->ups[i];
-    ch /= 2; f *= us.rate;
-    bool ups = us.form == UPS_COMB || us.form == UPS_FUSED;
-    if (us.form == UPS_POLYPHASE && us.noise_form == NOISE_TC) {   // phases on conv_tc, source only through SRCP
-      ups = true;
-      for (bool tcp : us.phase_tc) ups = ups && tcp;
-    }
-    if (!ups) {
-      set_error(who + "generator stage " + std::to_string(i) + "'s upsampler has no ragged form");
-      return SVCB_E_UNSUPPORTED;
-    }
-    const ResBlock& R = m->res[(size_t)i * c.n_res];
-    if (R.form == AMP_S2D) {   // every block of a stage has the same form; the s2d test of run_generator per length
-      auto s2d = [&](long long L) { return L % R.s2d_r == 0 && L % 8 == 0; };
-      bool ok = s2d(T * f);
-      for (int b = 0; b < B && ok; ++b) ok = s2d(n[b] * f);
-      if (!ok) {
-        set_error(who + "generator stage " + std::to_string(i) + " would leave the space-to-depth form at some length");
-        return SVCB_E_UNSUPPORTED;
-      }
-    } else if (R.form != AMP_TC) {
-      set_error(who + "generator stage " + std::to_string(i) + "'s AMP blocks have no ragged form");
-      return SVCB_E_UNSUPPORTED;
-    }
+    if (!m->ups[i].ragged) return reject(stage(i) + "'s upsampler has no ragged form");
+    for (int j = i * c.n_res; j < (i + 1) * c.n_res; ++j)
+      if (plan.amp[j] != AMP_TC && plan.amp[j] != AMP_S2D) return reject(stage(i) + "'s AMP blocks have no ragged form");
   }
-  bool post = !m->conv_post.b && post_fused_supported(ch, (int)(T * f), m->conv_post.k, wave, wave);
-  for (int b = 0; b < B && post; ++b) post = post_fused_supported(ch, (int)(n[b] * f), m->conv_post.k, wave, wave);
-  if (!post) {
-    set_error(who + "the generator's tail needs post_fused (a 16-byte aligned wave and 8 | samples)");
-    return SVCB_E_UNSUPPORTED;
+  if (!plan.post_fused) return reject(tail);
+  for (int b = 0; b < B; ++b) {
+    const GenPlan pb(m, n[b], wave);
+    for (int j = 0; j < c.n_ups * c.n_res; ++j)
+      if (pb.amp[j] != plan.amp[j]) return reject(stage(j / c.n_res) + " would leave the space-to-depth form at some length");
+    if (!pb.post_fused) return reject(tail);
   }
   return SVCB_OK;
 }
@@ -949,6 +965,33 @@ struct StageRates { long long v[SVCB_MAX_UPS + 1]; };
 __global__ void stage_lens_kernel(const int* __restrict__ n, long long* __restrict__ n64, StageRates f, int B, int rows) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k < B * rows) n64[k] = n[k % B] * f.v[k / B];
+}
+
+// prior -> flow -> generator in the workspace (svcb_infer; svcb_workspace_bytes as a dry run).  ragged: first the region
+// svcb_infer_ragged stages its lengths in (rl: those lengths, null in the dry run); the pipeline then reads them.
+static int run_infer(const svcb_model* m, Ctx& ctx, const float* ppg, const float* vec, const float* pit, const float* spk,
+                     const long long* lengths, const float* source, const float* eps, float* wave, int B, int T,
+                     bool ragged = false, RaggedLens* rl = nullptr) {
+  const int rows = m->cfg.n_ups + 1;
+  int* lens = ragged ? ctx.alloc<int>(ragged_lens_bytes(B) / sizeof(int)) : nullptr;
+  long long* len64 = ragged ? ctx.alloc<long long>((size_t)rows * B) : nullptr;
+  float* zp = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
+  float* z = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
+  SVCB_TRY(ctx.check());
+  if (rl) {
+    SVCB_TRY(rl->stage(lens, ctx.stream));
+    StageRates f = {{1}};
+    for (int i = 0; i < m->cfg.n_ups; ++i) f.v[i + 1] = f.v[i] * m->cfg.up_rates[i];
+    stage_lens_kernel<<<(B * rows + 255) / 256, 256, 0, ctx.stream>>>(lens, len64, f, B, rows);
+    SVCB_LAUNCH_CHECK("stage_lens");
+    lengths = len64;
+  }
+  const size_t mark = ctx.off;
+  SVCB_TRY(run_prior(m, ctx, ppg, vec, pit, lengths, eps, zp, B, T, rl != nullptr));
+  ctx.off = mark;
+  SVCB_TRY(run_flow(m, ctx, zp, lengths, spk, z, B, T));
+  ctx.off = mark;
+  return run_generator(m, ctx, spk, z, source, wave, B, T, rl ? len64 : nullptr, rl ? lens : nullptr, rl ? rl->min_out : 0);
 }
 
 static int validate_cfg(const svcb_config& c) {
@@ -1035,23 +1078,10 @@ void svcb_model_destroy(svcb_model* m) { delete m; }
 
 size_t svcb_workspace_bytes(const svcb_model* m, int32_t B, int32_t T) {
   if (!m || B <= 0 || T <= 0) return 0;
-  size_t peak = 0;
-  {
-    Ctx ctx; ctx.dry = true;
-    ctx.alloc<int>(ragged_lens_bytes(B) / sizeof(int));   // svcb_infer_ragged's lengths, int32 then int64 per rate
-    ctx.alloc<long long>((size_t)(m->cfg.n_ups + 1) * B);
-    float* zp = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
-    float* z = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
-    const size_t mark = ctx.off;
-    run_prior(m, ctx, nullptr, nullptr, nullptr, nullptr, nullptr, zp, B, T);
-    ctx.off = mark;
-    run_flow(m, ctx, zp, nullptr, nullptr, z, B, T);
-    ctx.off = mark;
-    run_generator(m, ctx, nullptr, z, nullptr, nullptr, B, T);
-    peak = ctx.peak;
-  }
-  peak = std::max(peak, source_scan_ws_bytes(B, T, m->cfg.n_harmonics) + 256);
-  return peak + 4096;
+  Ctx ctx;
+  ctx.dry = true;
+  run_infer(m, ctx, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, T, true);
+  return std::max(ctx.peak, source_scan_ws_bytes(B, T, m->cfg.n_harmonics) + 256) + 4096;
 }
 
 size_t svcb_source_workspace_bytes(const svcb_model* m, int32_t B, int32_t T) {
@@ -1121,16 +1151,7 @@ int svcb_infer(const svcb_model* m, const float* ppg, const float* vec, const fl
   if (!m || B <= 0 || T <= 0 || !lengths) { set_error("svcb_infer: bad shape or null lengths"); return SVCB_E_BAD_SHAPE; }
   Ctx ctx;
   SVCB_TRY(make_ctx(ctx, ws, ws_bytes, taps, stream));
-  const long long* len = reinterpret_cast<const long long*>(lengths);
-  float* zp = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
-  float* z = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
-  SVCB_TRY(ctx.check());
-  const size_t mark = ctx.off;
-  SVCB_TRY(run_prior(m, ctx, ppg, vec, pit, len, eps, zp, B, T));
-  ctx.off = mark;
-  SVCB_TRY(run_flow(m, ctx, zp, len, spk, z, B, T));
-  ctx.off = mark;
-  return run_generator(m, ctx, spk, z, source, wave, B, T);
+  return run_infer(m, ctx, ppg, vec, pit, spk, reinterpret_cast<const long long*>(lengths), source, eps, wave, B, T);
 }
 
 int svcb_infer_ragged(const svcb_model* m, const float* ppg, const float* vec, const float* pit, const float* spk,
@@ -1143,24 +1164,7 @@ int svcb_infer_ragged(const svcb_model* m, const float* ppg, const float* vec, c
   SVCB_TRY(ragged_forms(m, n_frames_host, B, T, wave));
   Ctx ctx;
   SVCB_TRY(make_ctx(ctx, ws, ws_bytes, nullptr, stream));
-  const int rows = m->cfg.n_ups + 1;
-  int* lens = ctx.alloc<int>(ragged_lens_bytes(B) / sizeof(int));
-  long long* len64 = ctx.alloc<long long>((size_t)rows * B);
-  float* zp = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
-  float* z = ctx.alloc<float>((size_t)B * m->cfg.inter_channels * T);
-  SVCB_TRY(ctx.check());
-  SVCB_TRY(rl.stage(lens, ctx.stream));
-  StageRates f;
-  f.v[0] = 1;
-  for (int i = 0; i < m->cfg.n_ups; ++i) f.v[i + 1] = f.v[i] * m->cfg.up_rates[i];
-  stage_lens_kernel<<<(B * rows + 255) / 256, 256, 0, ctx.stream>>>(lens, len64, f, B, rows);
-  SVCB_LAUNCH_CHECK("stage_lens");
-  const size_t mark = ctx.off;
-  SVCB_TRY(run_prior(m, ctx, ppg, vec, pit, len64, eps, zp, B, T, true));
-  ctx.off = mark;
-  SVCB_TRY(run_flow(m, ctx, zp, len64, spk, z, B, T));
-  ctx.off = mark;
-  return run_generator(m, ctx, spk, z, source, wave, B, T, len64, lens, rl.min_out);
+  return run_infer(m, ctx, ppg, vec, pit, spk, nullptr, source, eps, wave, B, T, true, &rl);
 }
 
 // ---- single-operator entry points
@@ -1200,17 +1204,15 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
   void* hi = scratch;
   void* lo = nsplit == 3 ? static_cast<char*>(scratch) + img : nullptr;
   SVCB_TRY(launch_snake_pack(x, hi, lo, ea, inv_b, fu, fd, B, C, L, s));
-  AmpConvParams q;
-  q.a_hi = hi; q.a_lo = lo; q.Lp = p8_rows(L); q.y = y; q.res = res;
-  q.wpk = static_cast<const uint8_t*>(w_tc); q.bias = bias;
-  q.B = B; q.C = C; q.Cp = (C + 15) / 16 * 16; q.L = L; q.K = K; q.dil = dilation; q.nsplit = nsplit;
-  q.accum = accum; q.out_div = out_div;
+  AmpConvParams q = amp_conv_params(hi, lo, B, C, L, K, nsplit);
+  q.wpk = static_cast<const uint8_t*>(w_tc); q.bias = bias; q.dil = dilation;
+  q.y = y; q.res = res; q.accum = accum; q.out_div = out_div;
   return launch_amp_conv_tc(q, s);
 }
 
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L) {
-  const int r = C > 0 ? 160 / C : 0;
-  if (B <= 0 || L <= 0 || !s2d_link_factor(C) || L % r) return 0;
+  const int r = s2d_link_factor(C);
+  if (B <= 0 || !s2d_fits(L, r)) return 0;
   return 4 * align256(s2d_image_bytes(B, L, r)) + 512;
 }
 
@@ -1220,20 +1222,17 @@ int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_ac
                          int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes, svcb_stream stream) {
   g_launches = 0;
   const int r = s2d_link_factor(C);
-  if (!r || B <= 0 || L <= 0 || L % r || L % 8) { set_error("svcb_op_amp_s2d_link: need C in {40, 20, 10}, L % (160/C) == 0 and L % 8 == 0"); return SVCB_E_BAD_SHAPE; }
+  if (B <= 0 || !s2d_fits(L, r)) { set_error("svcb_op_amp_s2d_link: need C in {40, 20, 10}, L % (160/C) == 0 and L % 8 == 0"); return SVCB_E_BAD_SHAPE; }
   const size_t img = align256(s2d_image_bytes(B, L, r));
   SVCB_TRY(check_workspace(scratch, scratch_bytes, 4 * img, "svcb_op_amp_s2d_link"));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   char* b0 = static_cast<char*>(scratch);
+  void* img4[4] = {b0, b0 + img, b0 + 2 * img, b0 + 3 * img};   // the input image (hi, lo), then the output image
   SVCB_CUDA_CHECK(cudaMemsetAsync(b0, 0, 4 * img, s));
-  SVCB_TRY(launch_snake_pack_s2d(x, b0, b0 + img, ea_in, ib_in, fu, fd, B, C, L, s));
-  AmpS2dParams q;
-  q.B = B; q.C = C; q.L = L; q.K = K; q.Rp = s2d_rows(L, r);
-  q.a_hi = b0; q.a_lo = b0 + img;
-  if (y_act) {
-    q.o_hi = b0 + 2 * img; q.o_lo = b0 + 3 * img; q.ea = ea_out; q.ib = ib_out; q.fu = fu; q.fd = fd;
-    SVCB_TRY(snake_taps_from_device(fu, fd, &q.taps));
-  }
+  SVCB_TRY(launch_snake_pack_s2d(x, img4[0], img4[1], ea_in, ib_in, fu, fd, B, C, L, s));
+  SnakeW act{ea_out, ib_out, fu, fd};
+  if (y_act) SVCB_TRY(snake_taps_from_device(fu, fd, &act.taps));
+  AmpS2dParams q = s2d_link_params(B, C, L, K, img4, img4 + 2, y_act ? &act : nullptr);
   q.wpk = static_cast<const uint8_t*>(w_s2d); q.bias = bias; q.res = res; q.y = y;
   if (!s2d_tap_plan(K, dilation, r, q.mlo, q.ntaps, q.tap_cols)) { set_error("svcb_op_amp_s2d_link: too many taps"); return SVCB_E_BAD_SHAPE; }
   SVCB_TRY(launch_amp_s2d_link(q, s));
