@@ -57,7 +57,7 @@ def resample_files(jobs, sr, threads, batch, max_padded=MAX_PADDED, device="cuda
                                max_padded=max_padded)
 
 
-if __name__ == "__main__":
+def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
     parser.add_argument("-o", "--out", help="out", dest="out", required=True)
@@ -65,15 +65,26 @@ if __name__ == "__main__":
     parser.add_argument("-t", "--thread_count", help="thread count to process, set 0 to use all cpu cores",
                         dest="thread_count", type=int, default=1)
     parser.add_argument("--batch", type=int, default=64, help="maximum files per device batch")
-    args = parser.parse_args()
+    args = parser.parse_args(argv)
     print(args.wav)
     print(args.out)
     print(args.sr)
     os.makedirs(args.out, exist_ok=True)
     if args.sr not in (16000, 32000):
-        sys.exit(f"-s must be 16000 or 32000, not {args.sr}")
+        print(f"-s must be 16000 or 32000, not {args.sr}", file=sys.stderr)
+        return 1
+    from whisper_vits_svc_b200 import resample
+
     jobs = resample_jobs(args.wav, args.out)
     threads = os.cpu_count() // 2 + 1 if args.thread_count == 0 else args.thread_count
-    st = resample_files(jobs, args.sr, threads, args.batch)
+    try:
+        st = resample_files(jobs, args.sr, threads, args.batch)
+    finally:
+        resample.release_filters()
     if st["failed"]:
         print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

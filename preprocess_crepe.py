@@ -44,13 +44,13 @@ def extract_pitch(jobs, model, threads, batch, max_padded=MAX_PADDED):
                                size=lambda a: a.shape[0], max_padded=max_padded)
 
 
-if __name__ == "__main__":
+def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
     parser.add_argument("-p", "--pit", help="pit", dest="pit", required=True)
     parser.add_argument("-t", "--threads", type=int, default=2, help="host threads reading the wavs (0: all cores)")
     parser.add_argument("--batch", type=int, default=32, help="maximum files per device batch")
-    args = parser.parse_args()
+    args = parser.parse_args(argv)
     print(args.wav)
     print(args.pit)
     require_cuda()
@@ -61,3 +61,8 @@ if __name__ == "__main__":
     st = extract_pitch(jobs, model, os.cpu_count() if args.threads == 0 else args.threads, args.batch)
     if st["failed"]:
         print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

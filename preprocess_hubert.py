@@ -42,13 +42,13 @@ def extract_vecs(jobs, hubert, threads, batch, max_padded=MAX_PADDED):
                                size=lambda a: a.shape[0], max_padded=max_padded)
 
 
-if __name__ == "__main__":
+def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
     parser.add_argument("-v", "--vec", help="vec", dest="vec", required=True)
     parser.add_argument("-t", "--threads", type=int, default=2, help="host threads reading the wavs (0: all cores)")
     parser.add_argument("--batch", type=int, default=32, help="maximum files per device batch")
-    args = parser.parse_args()
+    args = parser.parse_args(argv)
     print(args.wav)
     print(args.vec)
     from whisper_vits_svc_b200 import hubert_infer
@@ -59,3 +59,8 @@ if __name__ == "__main__":
     print(f"padding overhead: {st['padded'] / max(st['samples'], 1):.3f} (padded samples / samples)")
     if st["failed"]:
         print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

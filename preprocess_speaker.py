@@ -47,7 +47,7 @@ def extract_speaker_embeddings(wav_files, dataset_path, output_path, model, conc
                                save, concurrency, batch)["failed"]
 
 
-if __name__ == "__main__":
+def main(argv=None):
     parser = argparse.ArgumentParser(description="""Compute embedding vectors for each wav file in a dataset.""",
                                      formatter_class=RawTextHelpFormatter)
     parser.add_argument("dataset_path", type=str, help="Path to dataset waves.")
@@ -56,7 +56,7 @@ if __name__ == "__main__":
     parser.add_argument("-t", "--thread_count", help="thread count to process, set 0 to use all cpu cores",
                         dest="thread_count", type=int, default=1)
     parser.add_argument("--batch", type=int, default=32, help="utterances per device batch")
-    args = parser.parse_args()
+    args = parser.parse_args(argv)
     from whisper_vits_svc_b200 import speaker_infer
 
     model = speaker_infer.load_model(os.path.join("speaker_pretrain", "best_model.pth.tar"),
@@ -66,3 +66,8 @@ if __name__ == "__main__":
     n_failed = extract_speaker_embeddings(wav_files, args.dataset_path, args.output_path, model, process_num, args.batch)
     if n_failed:
         print(f"{n_failed} of {len(wav_files)} files failed", file=sys.stderr)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -37,14 +37,14 @@ def compute_specs(jobs, hp, threads, batch, max_padded=MAX_PADDED, device="cuda"
                                size=len, max_padded=max_padded)
 
 
-if __name__ == "__main__":
+def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
     parser.add_argument("-s", "--spe", help="spe", dest="spe", required=True)
     parser.add_argument("-t", "--thread_count", help="thread count to process, set 0 to use all cpu cores",
                         dest="thread_count", type=int, default=1)
     parser.add_argument("--batch", type=int, default=64, help="maximum files per device batch")
-    args = parser.parse_args()
+    args = parser.parse_args(argv)
     print(args.wav)
     print(args.spe)
     from whisper_vits_svc_b200 import hparams, spectrogram
@@ -53,9 +53,15 @@ if __name__ == "__main__":
     try:
         spectrogram.check_hparams(hp)
     except ValueError as e:
-        sys.exit(str(e))
+        print(e, file=sys.stderr)
+        return 1
     jobs = spec_jobs(args.wav, args.spe)
     threads = os.cpu_count() // 2 + 1 if args.thread_count == 0 else args.thread_count
     st = compute_specs(jobs, hp, threads, args.batch)
     if st["failed"]:
         print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

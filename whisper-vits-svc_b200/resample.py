@@ -82,6 +82,12 @@ def _device_taps(up: int, down: int, dev: torch.device):
     return _TAPS[key]
 
 
+def release_filters() -> None:
+    """Free the device filters cached by earlier calls, so that a process running other device work afterwards gets
+    their memory back.  The next call designs and uploads its filter again."""
+    _TAPS.clear()
+
+
 def _resample_device(audios: Sequence, sr_in: int, sr_out: int, dev: torch.device):
     """The batch resampled on the device: (flat float32 device tensor, output offsets).  Equal rates copy the input."""
     up, down = ratio(sr_in, sr_out)
