@@ -9,8 +9,9 @@ ops.amp_conv_tc also runs snake_pack; only the `amp_conv_tc_*` launches are coun
 svcb_timing_report: CUDA events around each launch).
 
 Prints one JSON line: the card, its power limit and max SM clock (read in the same run) and, per shape, ms per
-launch, the launches per step, and the tensor work's share of the 989 TFLOP/s dense bf16 data-sheet peak (3 bf16
-products per tap and output row).
+launch, the launches per step, the tensor work's share of the 989 TFLOP/s dense bf16 data-sheet peak (3 bf16
+products per tap and output row), and the HBM bytes a launch must move with their share of the 3.35 TB/s data-sheet
+bandwidth: per element 4 B of bf16 hi/lo image read and 4 B of y written, plus 4 B each of residual and stage sum read.
 
     python scripts/bench_amp_conv_tc.py [--batch 32] [--frames 1000] [--iters 20]"""
 import argparse
@@ -24,6 +25,7 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 PEAK_BF16 = 989e12
+PEAK_HBM = 3.35e12
 STAGES = [(160, 5), (80, 20)]   # (C, samples per frame) of generator stages 0-1
 KERNELS = (3, 7, 11)
 DILATIONS = (1, 3, 5)
@@ -99,9 +101,11 @@ def main():
                     call()
                 ms = conv_ms(lib, call, args.iters)
                 tensor_flop = 3 * 2.0 * C * C * k * B * L
+                hbm_bytes = (8 + 4 * with_res + 4 * accum) * B * C * L
                 rows.append({"C": C, "k": k, "dilation": d, "res": with_res, "accum": accum, "div": div,
                              "launches_per_step": per_step, "ms": round(ms, 4),
-                             "tensor_share_of_peak": round(tensor_flop / (ms * 1e-3) / PEAK_BF16, 3)})
+                             "tensor_share_of_peak": round(tensor_flop / (ms * 1e-3) / PEAK_BF16, 3),
+                             "hbm_bytes": hbm_bytes, "hbm_share_of_peak": round(hbm_bytes / (ms * 1e-3) / PEAK_HBM, 3)})
         del x, res, acc
         torch.cuda.empty_cache()
     per_stage = {C: round(sum(r["ms"] * r["launches_per_step"] for r in rows if r["C"] == C), 3) for C, _ in STAGES}

@@ -171,8 +171,14 @@ int launch_snake_pack(const float* x, void* hi, void* lo, const float* ea, const
 // Persistent and warp-specialised: each CTA walks tiles (item, 128 samples) with a static stride.
 //   warp 0 (one lane)  the A image rows of each tile (bulk copies, one buffer per tile in flight)
 //   warp 1 (one lane)  the weight matrices: all resident in shared memory when they fit, else a ring of 2-8 slots
+//   warps 2-3 (a lane each)  the residual (and the stage sum y_old) of the tiles of A buffer 0 / 1, one channel octet
+//                      per slot of a ring per buffer: one bulk copy of the tile's samples per channel (a contiguous
+//                      run of [B][C][L])
 //   warpgroups 1-2     all taps x split parts as wgmma m64nCpk16 into register accumulators, then
 //                      + bias (+res, +stage accumulation, /3) stored straight from the accumulator fragments
+// The residual copies of a tile start as soon as its buffer's previous epilogue has released their slots, so their HBM
+// time runs under the MMAs.  They need 16-byte aligned channel rows (L % 4 == 0); other lengths load the residual with
+// generic loads after the MMAs (AmpPlan::nr == 0).
 // Two schedules (amp_plan):
 //   ping-pong    (PP) each consumer warpgroup owns whole 128-row tiles, as two m64 accumulators: warpgroup 0 the even
 //                tiles of the CTA's walk, warpgroup 1 the odd ones, each with its own A buffer.  One warpgroup's
@@ -180,17 +186,21 @@ int launch_snake_pack(const float* x, void* hi, void* lo, const float* ea, const
 //   cooperative  both warpgroups on one tile, 64 rows each, when two A buffers and two weight slots do not fit
 //                (C = 160) or two 128-row accumulators would not fit the registers.
 // Either way every output row sees the same wgmma sequence (tap, weight part, A part, K step) into one accumulator.
-struct AmpPlan { int pingpong, resident, nabuf, nw; size_t smem; };
+struct AmpPlan { int pingpong, resident, nabuf, nw, nr; size_t smem; };
 constexpr int AMP_WMAX = 8;       // weight ring depth (max) when the taps do not stay resident
+constexpr int AMP_WKEEP = 4;      // ring slots a streamed shape keeps when the residual wants the room
+constexpr int AMP_RMAX = 16;      // residual slots per A buffer (max)
+constexpr int AMP_RSTRIDE = TC_M + 4;   // floats per staged channel row: the epilogue's 4 channels x 8 rows hit 32 banks
 constexpr int AMP_THREADS = 384;
 constexpr int AMP_PRODUCER_REGS = 40, AMP_CONSUMER_REGS = 232;   // 128 * 40 + 256 * 232 <= 64 K registers
 constexpr int AMP_PP_MAX_C = 112;  // ping-pong: two 64 x C accumulators per warpgroup (at C = 128 they spill)
 
 template <int NC, bool PP>
 __global__ void __launch_bounds__(AMP_THREADS, 1)
-amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, const int nw) {
+amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, const int nw, const int nr) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t a_full[2], a_empty[2], w_full[AMP_WMAX], w_empty[AMP_WMAX], w_res, order[2];
+  __shared__ __align__(8) uint64_t r_full[2 * AMP_RMAX], r_empty[2 * AMP_RMAX];
   constexpr int MB = PP ? 2 : 1;    // 64-row accumulators per consumer warpgroup
 
   const int tid = threadIdx.x, warp = tc::warp_uniform_idx();
@@ -206,12 +216,19 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
   uint8_t* Wbase = smem + (size_t)nabuf * a_buf;
   const int tpi = (p.L + TC_M - 1) / TC_M;
   const int ntiles = p.B * tpi;
+  // staged residual: per A buffer nr slots of one channel octet each, [array (res, y_old)][8 channels][AMP_RSTRIDE]
+  const int nres = (p.res ? 1 : 0) + (p.accum ? 1 : 0);
+  const int nu = (p.C + 7) / 8;   // octets per tile
+  const uint32_t r_slot = (uint32_t)nres * 8u * AMP_RSTRIDE * 4u;
+  float* Rbase = reinterpret_cast<float*>(Wbase + (size_t)(resident ? nch : nw) * wb);
 
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) { tc::mbar_init(&a_full[i], 1); tc::mbar_init(&a_empty[i], PP ? 1 : 2); }
     for (int i = 0; i < AMP_WMAX; ++i) { tc::mbar_init(&w_full[i], 1); tc::mbar_init(&w_empty[i], PP ? 1 : 2); }
     tc::mbar_init(&w_res, 1);
     for (int i = 0; i < 2; ++i) tc::mbar_init(&order[i], 1);
+    for (int b = 0; b < nabuf; ++b)
+      for (int i = b * AMP_RMAX; i < b * AMP_RMAX + nr; ++i) { tc::mbar_init(&r_full[i], 1); tc::mbar_init(&r_empty[i], PP ? 4 : 8); }
     tc::fence_barrier_init();
   }
   __syncthreads();
@@ -249,6 +266,27 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
             if (wi >= nw) tc::mbar_wait(&w_empty[st], (uint32_t)(((wi / nw) - 1) & 1));
             tc::mbar_arrive_expect_tx(&w_full[st], wb);
             tc::bulk_g2s(Wbase + (size_t)st * wb, p.wpk + ((size_t)(i / parts) * 2 + (i % parts)) * wb, wb, &w_full[st]);
+          }
+        }
+      }
+    } else if (warp >= 2 && warp - 2 < nabuf && nr > 0 && tc::elect_one()) {
+      // warp 2 + buf stages the tiles of A buffer buf: a lane that waits for its buffer's epilogue to free a slot then
+      // does not hold back the copies of the other buffer's next tile
+      const int buf = warp - 2;
+      int g = 0;   // position in the buffer's residual stream
+      for (int tile = blockIdx.x + buf * gridDim.x; tile < ntiles; tile += nabuf * gridDim.x, g += nu) {
+        const int b = tile / tpi, t0 = (tile - b * tpi) * TC_M;
+        const uint32_t run = (uint32_t)min(TC_M, p.L - t0) * 4u;
+        for (int u = 0; u < nu; ++u) {
+          const int q = g + u, s = buf * AMP_RMAX + q % nr;
+          if (q >= nr) tc::mbar_wait(&r_empty[s], (uint32_t)(((q / nr) - 1) & 1));
+          const int nc = min(8, p.C - 8 * u);
+          tc::mbar_arrive_expect_tx(&r_full[s], run * (uint32_t)(nres * nc));
+          float* slot = Rbase + (size_t)(buf * nr + q % nr) * (r_slot / 4u);
+          for (int a = 0; a < nres; ++a) {
+            const float* src = ((a == 0 && p.res) ? p.res : p.y) + ((long long)b * p.C + 8 * u) * p.L + t0;
+            float* dst = slot + a * 8 * AMP_RSTRIDE;   // an octet's arrays are 8 rows apart even when it has fewer channels
+            for (int c = 0; c < nc; ++c, src += p.L, dst += AMP_RSTRIDE) tc::bulk_g2s(dst, src, run, &r_full[s]);
           }
         }
       }
@@ -319,10 +357,40 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
     if (t == 0) tc::mbar_arrive(&a_empty[buf]);
 
     // epilogue from the fragments: d[4 j + e] is row 16 w + l/4 + 8 (e/2), column 8 j + 2 (l%4) + e%2, so the 8 lanes
-    // of a column cover 8 consecutive samples, one 32-byte sector of [B][C][L].  All residual / stage loads are
-    // issued before the first store.
+    // of a column cover 8 consecutive samples, one 32-byte sector of [B][C][L].
     const int w = t >> 5, l = t & 31;
     const long long yb = (long long)b * p.C * p.L;
+    if (nr > 0) {
+      // residual staged in shared memory: one octet (slot) at a time, released once all its rows are read
+      const int g0 = (it / nabuf) * nu;
+#pragma unroll
+      for (int j = 0; j < NC / 8; ++j) {
+        if (j >= nu) break;
+        const int g = g0 + j, s = g % nr;
+        tc::mbar_wait(&r_full[buf * AMP_RMAX + s], (uint32_t)((g / nr) & 1));
+        const float* sr = Rbase + (size_t)(buf * nr + s) * (r_slot / 4u);
+#pragma unroll
+        for (int m = 0; m < MB; ++m) {
+          const int r0 = (PP ? 64 * m : 64 * wg) + 16 * w + (l >> 2);   // row in the tile
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int c = 2 * (l & 3) + (e & 1), co = 8 * j + c, tr = r0 + 8 * (e >> 1), tt = t0 + tr;
+            if (co < p.C && tt < p.L) {
+              float a = p.res ? sr[c * AMP_RSTRIDE + tr] : 0.f;
+              if (p.accum) a += sr[((nres - 1) * 8 + c) * AMP_RSTRIDE + tr];
+              float o = acc[m][4 * j + e] + __ldg(p.bias + co) + a;
+              // a real (uniform) branch: if-converted, the division would run its x/0 slow path per element
+              if (do_div) { asm volatile(""); o = o / p.out_div; }
+              p.y[yb + (long long)co * p.L + tt] = o;
+            }
+          }
+        }
+        __syncwarp();
+        if (l == 0) tc::mbar_arrive(&r_empty[buf * AMP_RMAX + s]);
+      }
+      continue;
+    }
+    // generic loads: all residual / stage loads are issued before the first store
 #pragma unroll
     for (int m = 0; m < MB; ++m) {
       const int r0 = t0 + (PP ? 64 * m : 64 * wg) + 16 * w + (l >> 2);
@@ -358,23 +426,30 @@ amp_conv_tc_kernel(const AmpConvParams p, const int resident, const int nabuf, c
 
 // Resident weights when all nch matrices fit beside two A buffers; else a weight ring of as many slots as fit
 // (2-8) beside two A buffers, or beside one (C = 160).  Ping-pong needs the two A buffers.
-static AmpPlan amp_plan(int Cp, int K, int dil, int nsplit) {
+// nres (0-2) arrays are staged (residual, stage sum): each A buffer gets up to one slot per channel octet of a tile in
+// the room left beside the resident weights or AMP_WKEEP ring slots; the ring takes what the residual leaves.
+static AmpPlan amp_plan(int Cp, int K, int dil, int nsplit, int nres) {
   const int R = TC_M + (K - 1) * dil;
   const int parts = nsplit == 3 ? 2 : 1;
   const size_t a_buf = (size_t)(Cp / 8) * R * 16 * parts;
   const size_t wb = (size_t)Cp * Cp * 2;
   const size_t nch = (size_t)K * parts;
+  const size_t r_slot = (size_t)nres * 8 * AMP_RSTRIDE * 4;
   const size_t limit = 227 * 1024 - 1024;
   AmpPlan pl;
   pl.resident = 2 * a_buf + nch * wb <= limit;
   pl.nabuf = (pl.resident || 2 * a_buf + 2 * wb <= limit) ? 2 : 1;
-  pl.nw = pl.resident ? 0 : (int)std::min<size_t>(AMP_WMAX, (limit - std::min(limit, pl.nabuf * a_buf)) / wb);
+  const size_t left = limit - std::min(limit, pl.nabuf * a_buf);
+  const size_t keep = pl.resident ? nch * wb : std::min<size_t>(AMP_WKEEP, left / wb) * wb;
+  pl.nr = nres ? (int)std::min<size_t>(std::min(Cp / 8, AMP_RMAX), (left - std::min(left, keep)) / (pl.nabuf * r_slot)) : 0;
+  const size_t r_bytes = pl.nabuf * pl.nr * r_slot;
+  pl.nw = pl.resident ? 0 : (int)std::min<size_t>(AMP_WMAX, (left - std::min(left, r_bytes)) / wb);
   pl.pingpong = pl.nabuf == 2 && Cp <= AMP_PP_MAX_C;
-  pl.smem = pl.nabuf * a_buf + (pl.resident ? nch : (size_t)pl.nw) * wb + 128;
+  pl.smem = pl.nabuf * a_buf + (pl.resident ? nch : (size_t)pl.nw) * wb + r_bytes + 128;
   return pl;
 }
 
-size_t amp_conv_tc_smem_bytes(int Cp, int K, int dil, int nsplit) { return amp_plan(Cp, K, dil, nsplit).smem; }
+size_t amp_conv_tc_smem_bytes(int Cp, int K, int dil, int nsplit) { return amp_plan(Cp, K, dil, nsplit, 0).smem; }
 
 int launch_amp_conv_tc(const AmpConvParams& p, cudaStream_t s) {
   if (p.Cp % 16 || p.Cp < 16 || p.Cp > 256 || p.Cp < p.C || (p.nsplit != 1 && p.nsplit != 3)) {
@@ -385,7 +460,10 @@ int launch_amp_conv_tc(const AmpConvParams& p, cudaStream_t s) {
     set_error("amp_conv_tc: operand image does not match (halo > 32 rows or wrong Lp)");
     return SVCB_E_BAD_SHAPE;
   }
-  const AmpPlan pl = amp_plan(p.Cp, p.K, p.dil, p.nsplit);
+  // the staged residual is bulk-copied by channel row: rows must start and end on 16 bytes
+  const bool stage = (p.L % 4 == 0) && (reinterpret_cast<uintptr_t>(p.res) & 15) == 0 &&
+                     (!p.accum || (reinterpret_cast<uintptr_t>(p.y) & 15) == 0);
+  const AmpPlan pl = amp_plan(p.Cp, p.K, p.dil, p.nsplit, stage ? (p.res ? 1 : 0) + (p.accum ? 1 : 0) : 0);
   if ((!pl.resident && pl.nw < 1) || pl.smem > 227 * 1024 - 512) {
     set_error("amp_conv_tc: tile does not fit shared memory");
     return SVCB_E_UNSUPPORTED;
@@ -404,7 +482,7 @@ int launch_amp_conv_tc(const AmpConvParams& p, cudaStream_t s) {
   case nb * 2 + pp: {                                                                                            \
     static DevSmemCache attr_cache;                                                                              \
     SVCB_CUDA_CHECK(ensure_dyn_smem(amp_conv_tc_kernel<16 * nb, pp>, pl.smem, attr_cache));                      \
-    amp_conv_tc_kernel<16 * nb, pp><<<grid, AMP_THREADS, pl.smem, s>>>(p, pl.resident, pl.nabuf, pl.nw);         \
+    amp_conv_tc_kernel<16 * nb, pp><<<grid, AMP_THREADS, pl.smem, s>>>(p, pl.resident, pl.nabuf, pl.nw, pl.nr); \
     break;                                                                                                       \
   }
     SVCB_AMP_NC(1, 0) SVCB_AMP_NC(2, 0) SVCB_AMP_NC(3, 0) SVCB_AMP_NC(4, 0) SVCB_AMP_NC(5, 0) SVCB_AMP_NC(6, 0)
