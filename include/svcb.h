@@ -267,6 +267,18 @@ int svcb_pcm16_normalise_ragged(const float* y, const int64_t* offsets_host, int
  * out[0].  Each item is bitwise that of a lone call. */
 int svcb_cdc_ragged(const float* x, const int64_t* offsets_host, int32_t B, int16_t* out, svcb_stream stream);
 
+/* ------------------------------------------------------------------ trimming silence (training data) */
+/* Replaces the silence decision of pydub's detect_silence in prepare/preprocess_trim.py:15-20 (split_on_silence with
+ * min_silence_len = 200, silence_thresh = -45, seek_step = 1) for a ragged batch of 16-bit mono clips: item b is
+ * x[offsets_host[b] .. offsets_host[b+1]) (n_b >= 0 frames) at rates_host[b] Hz (1..192000); B >= 1.  With
+ * L_b = round(1000 n_b / rate) ms (ties to even) and ms m at frame fs(m) = (int)(m * (rate / 1000.0)), window i of
+ * frames [fs(i), fs(i + 200)), zero past n_b, is silent iff (unsigned) sqrt(S / N) <= 10^(-45/20) * 32768, S its sum of
+ * squares and N = fs(i + 200) - fs(i): audioop.rms's decision, exactly.  flags: one byte per window i = 0 .. L_b - 200
+ * (1 = silent; none when L_b < 200), item b's following item b-1's from flags[0].  Each item is bitwise that of a lone
+ * call. */
+int svcb_trim_silence_ragged(const int16_t* x, const int64_t* offsets_host, const int32_t* rates_host, int32_t B,
+                             uint8_t* flags, svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */
