@@ -279,6 +279,18 @@ int svcb_cdc_ragged(const float* x, const int64_t* offsets_host, int32_t B, int1
 int svcb_trim_silence_ragged(const int16_t* x, const int64_t* offsets_host, const int32_t* rates_host, int32_t B,
                              uint8_t* flags, svcb_stream stream);
 
+/* ------------------------------------------------------------------ WORLD DIO + StoneMask F0 (training data) */
+/* Replaces prepare/preprocess_f0.py:28-30: f0, t = pyworld.dio(x, fs=16000, f0_ceil=900, frame_period=10) (f0_floor 71,
+ * two channels per octave, speed 1, allowed_range 0.1) and pyworld.stonemask(x, f0, t, fs=16000), in fp64, for a
+ * ragged batch: item b is x[offsets_host[b] .. offsets_host[b+1]) (n_b >= 1 samples at 16 kHz); B >= 1.  out: float64,
+ * item b's n_b / 160 + 1 frames following item b-1's from out[0], before the reference's round(value, 1).  Items of at
+ * most 3 frames get zeros: WORLD's contour fix returns without writing for them.  The filter bank is a direct FIR
+ * (equal to WORLD's FFT filtering in exact arithmetic, DESIGN.md §5); each item is bitwise that of a lone call.  ws:
+ * svcb_world_f0_workspace_bytes(sum of n_b, B) bytes, 256-byte aligned (about 340 bytes per sample). */
+size_t svcb_world_f0_workspace_bytes(int64_t total_samples, int32_t B);
+int svcb_world_f0_ragged(const double* x, const int64_t* offsets_host, int32_t B, double* out, void* ws, size_t ws_bytes,
+                         svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */
