@@ -544,6 +544,15 @@ int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_ac
                          const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                          const float* fd, const void* w_s2d, const float* bias, int32_t B, int32_t C, int32_t L,
                          int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes, svcb_stream stream);
+/* The same link over a ragged batch: item b ends at lens_host[b] samples (host, each a multiple of 8 and of 160/C in
+ * [8, L]); y and y_act are written over each item's samples only.  The scratch (svcb_op_amp_s2d_link_scratch_bytes,
+ * enough for B <= 128) holds the input image (hi, lo) and then the output image (hi, lo), each
+ * (svcb_op_amp_s2d_link_scratch_bytes(B, C, L) - 512) / 4 bytes, followed by the lengths. */
+int svcb_op_amp_s2d_link_ragged(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
+                                const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
+                                const float* fd, const void* w_s2d, const float* bias, const int32_t* lens_host,
+                                int32_t B, int32_t C, int32_t L, int32_t K, int32_t dilation, void* scratch,
+                                size_t scratch_bytes, svcb_stream stream);
 
 /* Self-test of the wgmma plumbing: D[128,N] = A[shift:shift+128, :K] . B[N,K]^T with
  * bf16 operands (row-major, device) and fp32 accumulation in registers. */

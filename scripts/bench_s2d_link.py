@@ -10,8 +10,10 @@ ops.amp_s2d_link also clears the images, runs snake_pack_s2d and unpacks the out
 ops.amp_s2d_link always writes the fp32 result, which the step's c1 links do not.
 
 Prints one JSON line: the card, its power limit and max SM clock (read in the same run) and, per shape, ms per
-launch, the launches per step, and the tensor work's share of the 989 TFLOP/s dense bf16 data-sheet peak (3 bf16
-products per tap and tile row, halo rows included).
+launch, the launches per step, the tensor work's share of the 989 TFLOP/s dense bf16 data-sheet peak (3 bf16
+products per tap and tile row, halo rows included), and the HBM bytes a launch must move with their share of the
+3.35 TB/s data-sheet bandwidth: per element 4 B of bf16 hi/lo input image read and 4 B of y written, plus 4 B of
+residual read and 4 B of bf16 hi/lo output image written when the shape has them.  The weights are read from L2.
 
     python scripts/bench_s2d_link.py [--batch 32] [--frames 1000] [--iters 20]"""
 import argparse
@@ -25,6 +27,7 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 PEAK_BF16 = 989e12
+PEAK_HBM = 3.35e12
 STAGES = [(40, 80), (20, 160), (10, 320)]   # (C, samples per frame) of generator stages 2-4
 KERNELS = (3, 7, 11)
 DILATIONS = (1, 3, 5)
@@ -96,9 +99,11 @@ def main():
                         call()
                     ms = link_ms(lib, call, args.iters)
                     tensor_flop = 3 * 2.0 * 160 * 160 * (mlo + mhi + 1) * ntiles * 128
+                    hbm_bytes = (8 + 4 * with_res + 4 * snake) * B * C * L
                     rows.append({"C": C, "r": r, "k": k, "dilation": d, "ntaps": mlo + mhi + 1, "snake": snake,
                                  "res": with_res, "launches_per_step": per_step, "ms": round(ms, 4),
-                                 "tensor_share_of_peak": round(tensor_flop / (ms * 1e-3) / PEAK_BF16, 3)})
+                                 "tensor_share_of_peak": round(tensor_flop / (ms * 1e-3) / PEAK_BF16, 3),
+                                 "hbm_bytes": hbm_bytes, "hbm_share_of_peak": round(hbm_bytes / (ms * 1e-3) / PEAK_HBM, 3)})
         del x, res
         torch.cuda.empty_cache()
     print(json.dumps({"gpu": name, "power_limit_w": power, "max_sm_clock_mhz": clk, "batch": B, "frames": args.frames,

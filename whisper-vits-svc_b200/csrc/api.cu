@@ -1216,28 +1216,60 @@ size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L) {
   return 4 * align256(s2d_image_bytes(B, L, r)) + 512;
 }
 
+// lens_host (may be null): a ragged batch, item b ending at lens_host[b] samples; they go to the device through the
+// scratch after the four images
+static int op_amp_s2d_link(const char* who, const float* x, float* y, const float* res, float* y_act, const float* ea_in,
+                           const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
+                           const float* fd, const void* w_s2d, const float* bias, const int32_t* lens_host, int32_t B,
+                           int32_t C, int32_t L, int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes,
+                           svcb_stream stream) {
+  g_launches = 0;
+  const int r = s2d_link_factor(C);
+  if (B <= 0 || !s2d_fits(L, r)) { set_error(std::string(who) + ": need C in {40, 20, 10}, L % (160/C) == 0 and L % 8 == 0"); return SVCB_E_BAD_SHAPE; }
+  const size_t img = align256(s2d_image_bytes(B, L, r));
+  SVCB_TRY(check_workspace(scratch, scratch_bytes, 4 * img + (lens_host ? (size_t)B * sizeof(int32_t) : 0), who));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  char* b0 = static_cast<char*>(scratch);
+  void* img4[4] = {b0, b0 + img, b0 + 2 * img, b0 + 3 * img};   // the input image (hi, lo), then the output image
+  int* lens = nullptr;
+  if (lens_host) {
+    for (int b = 0; b < B; ++b)
+      if (lens_host[b] < 8 || lens_host[b] > L || lens_host[b] % 8 || lens_host[b] % r) {
+        set_error(std::string(who) + ": item " + std::to_string(b) + " has " + std::to_string(lens_host[b]) +
+                  " samples; need a multiple of 8 and of 160/C in [8, L]");
+        return SVCB_E_BAD_SHAPE;
+      }
+    lens = reinterpret_cast<int*>(b0 + 4 * img);
+    SVCB_CUDA_CHECK(cudaMemcpyAsync(lens, lens_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  }
+  SVCB_CUDA_CHECK(cudaMemsetAsync(b0, 0, 4 * img, s));
+  SVCB_TRY(launch_snake_pack_s2d(x, img4[0], img4[1], ea_in, ib_in, fu, fd, B, C, L, s, nullptr, lens, 1));
+  SnakeW act{ea_out, ib_out, fu, fd};
+  if (y_act) SVCB_TRY(snake_taps_from_device(fu, fd, &act.taps));
+  AmpS2dParams q = s2d_link_params(B, C, L, K, img4, img4 + 2, y_act ? &act : nullptr);
+  q.wpk = static_cast<const uint8_t*>(w_s2d); q.bias = bias; q.res = res; q.y = y; q.lens = lens;
+  if (!s2d_tap_plan(K, dilation, r, q.mlo, q.ntaps, q.tap_cols)) { set_error(std::string(who) + ": too many taps"); return SVCB_E_BAD_SHAPE; }
+  SVCB_TRY(launch_amp_s2d_link(q, s));
+  if (y_act) SVCB_TRY(launch_s2d_unpack(q.o_hi, q.o_lo, y_act, B, C, L, s));
+  return SVCB_OK;
+}
+
 int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                          const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                          const float* fd, const void* w_s2d, const float* bias, int32_t B, int32_t C, int32_t L,
                          int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes, svcb_stream stream) {
-  g_launches = 0;
-  const int r = s2d_link_factor(C);
-  if (B <= 0 || !s2d_fits(L, r)) { set_error("svcb_op_amp_s2d_link: need C in {40, 20, 10}, L % (160/C) == 0 and L % 8 == 0"); return SVCB_E_BAD_SHAPE; }
-  const size_t img = align256(s2d_image_bytes(B, L, r));
-  SVCB_TRY(check_workspace(scratch, scratch_bytes, 4 * img, "svcb_op_amp_s2d_link"));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  char* b0 = static_cast<char*>(scratch);
-  void* img4[4] = {b0, b0 + img, b0 + 2 * img, b0 + 3 * img};   // the input image (hi, lo), then the output image
-  SVCB_CUDA_CHECK(cudaMemsetAsync(b0, 0, 4 * img, s));
-  SVCB_TRY(launch_snake_pack_s2d(x, img4[0], img4[1], ea_in, ib_in, fu, fd, B, C, L, s));
-  SnakeW act{ea_out, ib_out, fu, fd};
-  if (y_act) SVCB_TRY(snake_taps_from_device(fu, fd, &act.taps));
-  AmpS2dParams q = s2d_link_params(B, C, L, K, img4, img4 + 2, y_act ? &act : nullptr);
-  q.wpk = static_cast<const uint8_t*>(w_s2d); q.bias = bias; q.res = res; q.y = y;
-  if (!s2d_tap_plan(K, dilation, r, q.mlo, q.ntaps, q.tap_cols)) { set_error("svcb_op_amp_s2d_link: too many taps"); return SVCB_E_BAD_SHAPE; }
-  SVCB_TRY(launch_amp_s2d_link(q, s));
-  if (y_act) SVCB_TRY(launch_s2d_unpack(q.o_hi, q.o_lo, y_act, B, C, L, s));
-  return SVCB_OK;
+  return op_amp_s2d_link("svcb_op_amp_s2d_link", x, y, res, y_act, ea_in, ib_in, ea_out, ib_out, fu, fd, w_s2d, bias,
+                         nullptr, B, C, L, K, dilation, scratch, scratch_bytes, stream);
+}
+
+int svcb_op_amp_s2d_link_ragged(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
+                                const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
+                                const float* fd, const void* w_s2d, const float* bias, const int32_t* lens_host,
+                                int32_t B, int32_t C, int32_t L, int32_t K, int32_t dilation, void* scratch,
+                                size_t scratch_bytes, svcb_stream stream) {
+  if (!lens_host) { set_error("svcb_op_amp_s2d_link_ragged: lens_host is null"); return SVCB_E_BAD_SHAPE; }
+  return op_amp_s2d_link("svcb_op_amp_s2d_link_ragged", x, y, res, y_act, ea_in, ib_in, ea_out, ib_out, fu, fd, w_s2d,
+                         bias, lens_host, B, C, L, K, dilation, scratch, scratch_bytes, stream);
 }
 
 int svcb_op_snake_alias(const float* x, float* y, const float* ea, const float* inv_b,

@@ -118,6 +118,47 @@ def amp_s2d_link(x, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=Non
     return y, y_act
 
 
+def amp_s2d_link_ragged(x, lens, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=None, alpha_out=None,
+                        beta_out=None):
+    """amp_s2d_link over a ragged batch: item b is x[b, :, :lens[b]] (each a multiple of 8 and of 160 / C).
+    Returns (y, y_act, out_hi, out_lo): y and y_act as amp_s2d_link's, zero past each item's end, and the
+    output S2D image as written, bf16 [B, 20, Rp, 8] hi and lo (None without alpha_out)."""
+    x = _c(x)
+    B, C, L = x.shape
+    K = weight.shape[-1]
+    r = pack.s2d_factor(C)
+
+    def snake_params(a, b):
+        return (_c(torch.exp(a.float().cpu()).to(x.device)), _c((1.0 / (torch.exp(b.float().cpu()) + 1e-9)).to(x.device)))
+
+    ea_i, ib_i = snake_params(alpha_in, beta_in)
+    ea_o, ib_o = snake_params(alpha_out, beta_out) if alpha_out is not None else (None, None)
+    fu, fd = _c(fu.reshape(-1).to(x.device)), _c(fd.reshape(-1).to(x.device))
+    w = pack.pack_conv_s2d_slots(weight.detach().cpu().float(), dilation, r).to(x.device)
+    b = _c(bias)
+    rs = _c(res) if res is not None else None
+    ln = torch.as_tensor(lens, dtype=torch.int32).cpu().contiguous()
+    y = torch.zeros_like(x)
+    y_act = torch.zeros_like(x) if alpha_out is not None else None
+    nbytes = int(_lib.load().svcb_op_amp_s2d_link_scratch_bytes(B, C, L))
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    _lib.call("op_amp_s2d_link_ragged", x.data_ptr(), y.data_ptr(), rs.data_ptr() if rs is not None else None,
+              y_act.data_ptr() if y_act is not None else None, ea_i.data_ptr(), ib_i.data_ptr(),
+              ea_o.data_ptr() if ea_o is not None else None, ib_o.data_ptr() if ib_o is not None else None,
+              fu.data_ptr(), fd.data_ptr(), w.data_ptr(), b.data_ptr(), ln.data_ptr(), B, C, L, K, dilation,
+              scratch.data_ptr(), scratch.numel(), device=x.device)
+    if alpha_out is None:
+        return y, y_act, None, None
+    img = (nbytes - 512) // 4
+    S = 128 - 2 * (1 if r >= 8 else 2)                   # useful rows per tile (amp_s2d.cu: s2d_rows)
+    rows = -(-(L // r) // S) * S + 160
+
+    def image(i):
+        return scratch[i * img:i * img + B * 20 * rows * 16].view(torch.bfloat16).view(B, 20, rows, 8)
+
+    return y, y_act, image(2), image(3)
+
+
 def conv_tc(x, weight, bias=None, dilation=1, res=None, lengths=None, nsplit=3, flags=0, act=0):
     """Stride-1 'same' Conv1d on the tensor cores; weight in torch layout [Cout,Cin,K]."""
     x = _c(x)
