@@ -291,6 +291,20 @@ size_t svcb_world_f0_workspace_bytes(int64_t total_samples, int32_t B);
 int svcb_world_f0_ragged(const double* x, const int64_t* offsets_host, int32_t B, double* out, void* ws, size_t ws_bytes,
                          svcb_stream stream);
 
+/* ------------------------------------------------------------------ Praat autocorrelation F0 (training data) */
+/* Replaces prepare/preprocess_f0_mouth.py:11-22: parselmouth.Sound(x, 16000).to_pitch_ac(time_step=0.01,
+ * voicing_threshold=0.5, pitch_floor=30, pitch_ceiling=1000).selected_array['frequency'] (15 candidates, a Hanning
+ * window of 3 periods, silence threshold 0.03, octave cost 0.01, octave-jump cost 0.35, voiced/unvoiced cost 0.14), in
+ * fp64, for a ragged batch: item b is x[offsets_host[b] .. offsets_host[b+1]) (n_b >= 1600 samples at 16 kHz: at
+ * least the 0.1 s window); B >= 1.  out: float64, item b's floor((n_b / 16000 - 0.1) / 0.01) + 1 frames (evaluated in
+ * double precision, about n_b / 160 - 9) following item b-1's from out[0], unpadded (the reference pads 6 zeros on
+ * each side); 0 marks an unvoiced frame.  The autocorrelation is a direct sum (equal to Praat's FFT form in exact
+ * arithmetic, DESIGN.md §5); each item is bitwise that of a lone call.  ws: svcb_praat_f0_workspace_bytes(sum of n_b,
+ * B) bytes, 256-byte aligned (about 1.6 bytes per sample). */
+size_t svcb_praat_f0_workspace_bytes(int64_t total_samples, int32_t B);
+int svcb_praat_f0_ragged(const double* x, const int64_t* offsets_host, int32_t B, double* out, void* ws, size_t ws_bytes,
+                         svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */
