@@ -240,6 +240,16 @@ int svcb_whisper_log_mel_ragged(const float* audio, const int32_t* n_samples_hos
 int svcb_linear_spec_ragged(const float* audio, const int64_t* sample_offsets_host, int32_t B, float* out, void* scratch,
                             size_t scratch_bytes, svcb_stream stream);
 
+/* ------------------------------------------------------------------ log-mel of the validation pass (32 kHz) */
+/* Replaces vits_extend/stft.py:TacotronSTFT.mel_spectrogram (n_fft 1024, hop 320, win 1024, center=False) as
+ * vits_extend/validation.py calls it on a padded batch: audio [B, L] fp32 (1 <= B <= 65535, L > 352, the reflect
+ * padding) -> mel [B, n_mels, L / 320] fp32.  Reflect pad 352 at both ends of every row, periodic-Hann frames of 1024 at
+ * hop 320, magnitude sqrt(re^2 + im^2 + 1e-9) by a direct DFT, mel_basis [n_mels, 513] fp32 (1 <= n_mels <= 128)
+ * accumulated in ascending bin order over each filter's non-zero span, ln(max(x, 1e-5)), all in fp32.  Each row's
+ * result is bitwise that of a lone call.  Bad arguments fail before any launch. */
+int svcb_tacotron_mel(const float* audio, int32_t B, int64_t L, const float* mel_basis, int32_t n_mels, float* mel,
+                      svcb_stream stream);
+
 /* ------------------------------------------------------------------ resampling of raw recordings (training data) */
 /* Replaces librosa.load(path, sr=sample_rate)'s resampling in prepare/preprocess_a.py:11 (resample_wave), as
  * scipy.signal.resample_poly's polyphase FIR, for a ragged batch at one ratio up/down (sr_out / sr_in, reduced):

@@ -96,6 +96,7 @@ SIGNATURES = {
     "svcb_whisper_log_mel": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
     "svcb_whisper_log_mel_ragged": (c_int, [c_void_p, POINTER(c_int32), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
     "svcb_linear_spec_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "svcb_tacotron_mel": (c_int, [c_void_p, c_int32, c_int64, c_void_p, c_int32, c_void_p, c_void_p]),
     "svcb_resample_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32, c_int32, c_int32, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
     "svcb_pcm16_normalise_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p]),
     "svcb_cdc_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p]),

@@ -91,6 +91,10 @@ class SynthesizerInfer(torch.nn.Module):
         self._handle = None
         self._handle = _lib.Handle("model", table, blob_dev, _lib.Config.from_dict(self._cfg))
 
+    def release(self):
+        """Free the device handle, its packed blob and its workspace now; the next compute call packs again."""
+        self._handle = None
+
     def packed_blob(self):
         self._ensure()
         return self._handle.blob, self._handle.table

@@ -215,11 +215,14 @@ def _mel_to_hz_slaney(m):
     return np.where(m >= min_log_mel, min_log_hz * np.exp(logstep * (m - min_log_mel)), f_sp * m)
 
 
-def mel_filters(n_mels: int = N_MELS, sr: int = SAMPLE_RATE, n_fft: int = N_FFT) -> torch.Tensor:
-    """librosa.filters.mel(sr, n_fft, n_mels) defaults (Slaney scale, slaney area norm), which is
-    what whisper/audio.py:54-65 asks librosa for."""
+def mel_filters(n_mels: int = N_MELS, sr: int = SAMPLE_RATE, n_fft: int = N_FFT, fmin: float = 0.0,
+                fmax: float | None = None) -> torch.Tensor:
+    """librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax) (Slaney scale, slaney area norm; fmax None is sr / 2).  The
+    defaults are what whisper/audio.py:54-65 asks librosa for; vits_extend/stft.py:46-47 asks for fmin 50, fmax 16000."""
+    if fmax is None:
+        fmax = sr / 2
     fftfreqs = np.linspace(0, sr / 2, n_fft // 2 + 1)
-    mel_pts = _mel_to_hz_slaney(np.linspace(_hz_to_mel_slaney(0.0), _hz_to_mel_slaney(sr / 2), n_mels + 2))
+    mel_pts = _mel_to_hz_slaney(np.linspace(_hz_to_mel_slaney(fmin), _hz_to_mel_slaney(fmax), n_mels + 2))
     fdiff = np.diff(mel_pts)
     ramps = mel_pts[:, None] - fftfreqs[None, :]
     w = np.zeros((n_mels, n_fft // 2 + 1))
