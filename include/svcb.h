@@ -561,13 +561,17 @@ int svcb_op_amp_conv_tc(const float* x, float* y, const float* res, const float*
  * generator stages (C = 20 or 10; vits_decoder/bigv.py:50-58) in space-to-depth form (csrc/amp_s2d.cu):
  * snake_pack_s2d, then the block-Toeplitz wgmma convolution whose epilogue writes y (fp32, may be NULL)
  * and — when y_act != NULL — SnakeAlias_out(result) as the next link's bf16 hi/lo operand image, returned
- * here decoded to fp32 [B,C,L].  w_s2d = pack.py:pack_conv_s2d_slots image (output columns in the kernel's
- * phase-slot order); L % (160/C) == 0 and L % 8 == 0 (the scratch size is 0 for other shapes). */
+ * here decoded to fp32 [B,C,L].  w_s2d = pack.py:pack_conv_s2d_link image (output columns in the kernel's
+ * phase-slot order; the undilated conv's matrices when the link runs on a folded input, pack.py:s2d_fold);
+ * L % (160/C) == 0 and L % 8 == 0 (the scratch size is 0 for other shapes).  out_dilation (1 .. 5, > 1 only with
+ * y_act and a link whose input is not folded): the output image is written folded for a next link of that
+ * dilation (1 = the standard image). */
 size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L);
 int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                          const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                          const float* fd, const void* w_s2d, const float* bias, int32_t B, int32_t C, int32_t L,
-                         int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes, svcb_stream stream);
+                         int32_t K, int32_t dilation, int32_t out_dilation, void* scratch, size_t scratch_bytes,
+                         svcb_stream stream);
 /* The same link over a ragged batch: item b ends at lens_host[b] samples (host, each a multiple of 8 and of 160/C in
  * [8, L]); y and y_act are written over each item's samples only.  The scratch (svcb_op_amp_s2d_link_scratch_bytes,
  * enough for B <= 128) holds the input image (hi, lo) and then the output image (hi, lo), each
@@ -575,8 +579,8 @@ int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_ac
 int svcb_op_amp_s2d_link_ragged(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                                 const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                                 const float* fd, const void* w_s2d, const float* bias, const int32_t* lens_host,
-                                int32_t B, int32_t C, int32_t L, int32_t K, int32_t dilation, void* scratch,
-                                size_t scratch_bytes, svcb_stream stream);
+                                int32_t B, int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t out_dilation,
+                                void* scratch, size_t scratch_bytes, svcb_stream stream);
 
 /* Self-test of the wgmma plumbing: D[128,N] = A[shift:shift+128, :K] . B[N,K]^T with
  * bf16 operands (row-major, device) and fp32 accumulation in registers. */

@@ -2,8 +2,11 @@
 """The space-to-depth AMP links of generator stages 2-4 (csrc/amp_s2d.cu) at B = 32, T = 1000, one shape at a time
 through ops.amp_s2d_link.  A shape is (C, k, dilation, Snake output or not, residual or not); the step runs 54
 links over 15 distinct shapes per stage, each c1 link without a residual, each c2 link with one, every link but a
-block's last with the next SnakeAlias in its epilogue.  Every shape is also timed without the Snake output: that
-link is the MMA side plus a plain fp32 store, so the difference is what the Snake epilogue costs.
+block's last with the next SnakeAlias in its epilogue.  A c1 link of dilation d runs on the fold pack.s2d_fold
+picks (its input image permuted inside blocks of r*d samples, the undilated conv's taps), and a c2 link writes the
+image in the fold of the c1 link after it; each row reports the folds, taps and tile rows.  The c2 shapes are timed
+writing the standard image and both folded images, and without the Snake output: that link is the MMA side plus a
+plain fp32 store, so the differences are what the Snake epilogue and the folded store cost.
 
 ops.amp_s2d_link also clears the images, runs snake_pack_s2d and unpacks the output image; only the
 `amp_s2d_link_*` launches are counted (svcb_timing_enable / svcb_timing_report: CUDA events around each launch).
@@ -11,7 +14,7 @@ ops.amp_s2d_link always writes the fp32 result, which the step's c1 links do not
 
 Prints one JSON line: the card, its power limit and max SM clock (read in the same run) and, per shape, ms per
 launch, the launches per step, the tensor work's share of the 989 TFLOP/s dense bf16 data-sheet peak (3 bf16
-products per tap and tile row, halo rows included), and the HBM bytes a launch must move with their share of the
+products per tap column and tile row, halo rows included, edge taps counted over their reached columns), and the HBM bytes a launch must move with their share of the
 3.35 TB/s data-sheet bandwidth: per element 4 B of bf16 hi/lo input image read and 4 B of y written, plus 4 B of
 residual read and 4 B of bf16 hi/lo output image written when the shape has them.  The weights are read from L2.
 
@@ -78,29 +81,41 @@ def main():
     for C, up in STAGES:
         L = args.frames * up
         r = pack.s2d_factor(C)
-        S = 128 - 2 * (1 if r >= 8 else 2)
-        ntiles = B * ((L // r + S - 1) // S)
         x = torch.randn(B, C, L, device="cuda", generator=gd)
         res = torch.randn(B, C, L, device="cuda", generator=gd)
         a_in, b_in, a_out, b_out = (torch.randn(C, generator=g) * 0.3 for _ in range(4))
         bias = (torch.randn(C, generator=g) * 0.1).cuda()
         for k in KERNELS:
-            # (dilation, residual, launches per step with Snake output, without)
-            shapes = [(d, False, 1, 0) for d in DILATIONS] + [(1, True, 2, 1)]
-            for d, with_res, n_snake, n_plain in shapes:
+            # (dilation, residual, output fold, launches per step with Snake output, without): c1 links read the fold
+            # pack.s2d_fold picks; c2 links write the next c1 link's fold (c2[0] for d = 3, c2[1] for d = 5), and
+            # each c2 shape is also timed writing the standard image and both folds, so that the folded store's cost
+            # shows on its own
+            nxt = [pack.s2d_fold(k, d, r) for d in DILATIONS[1:]]
+            shapes = [(d, False, 1, 1, 0) for d in DILATIONS]
+            shapes += [(1, True, f, sum(n == f for n in nxt), 1 if f == 1 else 0) for f in (1, 3, 5)]
+            for d, with_res, fout, n_snake, n_plain in shapes:
                 w = torch.randn(C, C, k, generator=g) / (C * k) ** 0.5
-                mlo, mhi = pack.s2d_taps(k, d, r)
+                fin = pack.s2d_fold(k, d, r)
+                mlo, mhi = pack.s2d_taps(k, 1 if fin > 1 else d, r)
                 for snake, per_step in ((True, n_snake), (False, n_plain)):
+                    if not snake and fout > 1:
+                        continue
+                    halo, S, _ = pack.s2d_tile(r, fin, fout if snake else 1, mlo, mhi)
+                    ntiles = B * ((L // r + 4 + S - 1) // S)
+
                     def call():
                         ops.amp_s2d_link(x, a_in, b_in, fu, fd, w, bias, dilation=d, res=res if with_res else None,
-                                         alpha_out=a_out if snake else None, beta_out=b_out if snake else None)
+                                         alpha_out=a_out if snake else None, beta_out=b_out if snake else None,
+                                         out_dilation=fout if snake else 1)
 
                     for _ in range(args.warmup):
                         call()
                     ms = link_ms(lib, call, args.iters)
-                    tensor_flop = 3 * 2.0 * 160 * 160 * (mlo + mhi + 1) * ntiles * 128
+                    cols = sum(n1 - n0 for n0, n1 in pack.s2d_tap_cols(k, 1 if fin > 1 else d, r))
+                    tensor_flop = 3 * 2.0 * 160 * cols * ntiles * 128
                     hbm_bytes = (8 + 4 * with_res + 4 * snake) * B * C * L
-                    rows.append({"C": C, "r": r, "k": k, "dilation": d, "ntaps": mlo + mhi + 1, "snake": snake,
+                    rows.append({"C": C, "r": r, "k": k, "dilation": d, "fold_in": fin, "fold_out": fout,
+                                 "ntaps": mlo + mhi + 1, "tile_rows": S + 2 * halo, "useful_rows": S, "snake": snake,
                                  "res": with_res, "launches_per_step": per_step, "ms": round(ms, 4),
                                  "tensor_share_of_peak": round(tensor_flop / (ms * 1e-3) / PEAK_BF16, 3),
                                  "hbm_bytes": hbm_bytes, "hbm_share_of_peak": round(hbm_bytes / (ms * 1e-3) / PEAK_HBM, 3)})

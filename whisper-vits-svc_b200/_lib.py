@@ -163,8 +163,8 @@ SIGNATURES = {
     "svcb_op_amp_conv_tc_scratch_bytes": (c_size_t, [c_int32] * 3),
     "svcb_op_amp_conv_tc": (c_int, [c_void_p] * 9 + [c_int32] * 7 + [c_float, c_void_p, c_size_t, c_void_p]),
     "svcb_op_amp_s2d_link_scratch_bytes": (c_size_t, [c_int32] * 3),
-    "svcb_op_amp_s2d_link": (c_int, [c_void_p] * 12 + [c_int32] * 5 + [c_void_p, c_size_t, c_void_p]),
-    "svcb_op_amp_s2d_link_ragged": (c_int, [c_void_p] * 13 + [c_int32] * 5 + [c_void_p, c_size_t, c_void_p]),
+    "svcb_op_amp_s2d_link": (c_int, [c_void_p] * 12 + [c_int32] * 6 + [c_void_p, c_size_t, c_void_p]),
+    "svcb_op_amp_s2d_link_ragged": (c_int, [c_void_p] * 13 + [c_int32] * 6 + [c_void_p, c_size_t, c_void_p]),
     "svcb_op_tc_gemm_selftest": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int32] * 4 + [c_void_p]),
 }
 

@@ -104,8 +104,8 @@ struct ResBlock {
   const uint8_t *c1_tc[3], *c2_tc[3];  // bf16 hi/lo tensor-core images of the same weights
   // narrow stages (C * r = 160, r = s2d_r): block-Toeplitz matrices of the same convs (pack.py:pack_conv_s2d_slots)
   const uint8_t *c1_s2d[3] = {nullptr, nullptr, nullptr}, *c2_s2d[3] = {nullptr, nullptr, nullptr};
-  int s2d_r = 0, s2d_ml1[3], s2d_nt1[3], s2d_ml2[3], s2d_nt2[3];
-  uint64_t s2d_tc1[3], s2d_tc2[3];      // the output columns each tap reaches (s2d_tap_plan)
+  int s2d_r = 0;
+  S2dPlan s2d1[3], s2d2[3];             // c1's fold, taps and the columns each reaches (s2d_tap_plan); c2's (fold 1)
   SnakeW act[6];
   int k, dil[3];
   AmpForm form = AMP_FP32;
@@ -442,17 +442,19 @@ static AmpConvParams amp_conv_params(const void* hi, const void* lo, int B, int 
 
 // narrow stages: every link = block-Toeplitz wgmma conv with the next SnakeAlias in its epilogue.  Link k = 2d + half
 // is c1[d] from S2D image 0 to image 1 or c2[d] from image 1 to image 0 (a.s2d = hi, lo of each); its output image is
-// SnakeAlias k + 1, none after the block's last conv.
+// SnakeAlias k + 1, none after the block's last conv.  Image 0 is written in the fold of the c1 link that reads it.
 static int run_amp_s2d(Ctx& ctx, const Stage& a, const ResBlock& R, int j) {
   const SnakeW& s0 = R.act[0];
-  RUN(launch_snake_pack_s2d(a.X, a.s2d[0], a.s2d[1], s0.ea, s0.ib, s0.fu, s0.fd, a.B, a.C, a.L, ctx.stream, &s0.taps, a.lens, a.lscale));
+  RUN(launch_snake_pack_s2d(a.X, a.s2d[0], a.s2d[1], s0.ea, s0.ib, s0.fu, s0.fd, a.B, a.C, a.L, ctx.stream, &s0.taps, a.lens, a.lscale,
+                            R.s2d1[0].fold));
   const float* cur = a.X;
   for (int k = 0; k < 6; ++k) {
     const int d = k / 2, half = k % 2;
     AmpS2dParams q = s2d_link_params(a.B, a.C, a.L, R.k, a.s2d + 2 * half, a.s2d + 2 - 2 * half, k < 5 ? &R.act[k + 1] : nullptr);
     q.wpk = half ? R.c2_s2d[d] : R.c1_s2d[d]; q.bias = half ? R.c2[d].b : R.c1[d].b;
-    q.ntaps = half ? R.s2d_nt2[d] : R.s2d_nt1[d]; q.mlo = half ? R.s2d_ml2[d] : R.s2d_ml1[d];
-    q.tap_cols = half ? R.s2d_tc2[d] : R.s2d_tc1[d];
+    const S2dPlan& pl = half ? R.s2d2[d] : R.s2d1[d];
+    q.ntaps = pl.ntaps; q.mlo = pl.mlo; q.tap_cols = pl.tap_cols; q.fin = pl.fold;
+    if (half && d < 2) q.fout = R.s2d1[d + 1].fold;
     q.lens = a.lens; q.lscale = a.lscale;
     if (half) { q.res = cur; q.y = a.out(d); q.accum = a.accum(d, j); q.out_div = a.out_div(d, j); cur = q.y; }
     RUN(launch_amp_s2d_link(q, ctx.stream));
@@ -685,7 +687,7 @@ static int run_generator(const svcb_model* m, Ctx& ctx, const float* spk, const 
     const size_t mark = ctx.off;
     if (forms[0] == AMP_S2D) {   // (every block of a stage has the same channel count: all or none take this form)
       // two ping-pong S2D images (hi, lo each), cleared once per stage: rows outside the sequences are the
-      // convolutions' zero padding and are never written by the link kernels
+      // convolutions' zero padding; the writers store zeros over an item's first rows past its end (S2D_TAIL)
       const size_t ib = s2d_image_bytes(B, Ln, rb[0].s2d_r);
       uint8_t* base = ctx.alloc<uint8_t>(4 * ib);
       SVCB_TRY(ctx.check());
@@ -909,11 +911,12 @@ static int resolve(svcb_model* m, Resolver& R) {
       }
       rb.s2d_r = s2d_link_factor(ch);
       for (int d = 0; d < 3 && rb.s2d_r; ++d) {
-        s2d_tap_plan(rb.k, rb.dil[d], rb.s2d_r, rb.s2d_ml1[d], rb.s2d_nt1[d], rb.s2d_tc1[d]);
-        s2d_tap_plan(rb.k, 1, rb.s2d_r, rb.s2d_ml2[d], rb.s2d_nt2[d], rb.s2d_tc2[d]);
+        // c1 runs on the fold its plan picks (its blob entry holds the undilated conv's matrices when folded)
+        s2d_tap_plan(rb.k, rb.dil[d], rb.s2d_r, rb.s2d1[d]);
+        s2d_tap_plan(rb.k, 1, rb.s2d_r, rb.s2d2[d]);
         const uint64_t per_tap = 2ull * 160 * 160 / 2;   // fp32-typed elements of one (hi, lo) pair
-        rb.c1_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c1." + std::to_string(d) + ".s2d", per_tap * rb.s2d_nt1[d]));
-        rb.c2_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c2." + std::to_string(d) + ".s2d", per_tap * rb.s2d_nt2[d]));
+        rb.c1_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c1." + std::to_string(d) + ".s2d", per_tap * rb.s2d1[d].ntaps));
+        rb.c2_s2d[d] = reinterpret_cast<const uint8_t*>(R.get(p + ".c2." + std::to_string(d) + ".s2d", per_tap * rb.s2d2[d].ntaps));
       }
       for (int a = 0; a < 6; ++a) rb.act[a] = R.snake(p + ".act." + std::to_string(a), ch);
       rb.fallback = !tc ? AMP_FP32 : amp_block_fused_supported(ch, rb.k, rb.dil) ? AMP_BLOCK_FUSED : AMP_TC;
@@ -1221,11 +1224,17 @@ size_t svcb_op_amp_s2d_link_scratch_bytes(int32_t B, int32_t C, int32_t L) {
 static int op_amp_s2d_link(const char* who, const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                            const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                            const float* fd, const void* w_s2d, const float* bias, const int32_t* lens_host, int32_t B,
-                           int32_t C, int32_t L, int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes,
-                           svcb_stream stream) {
+                           int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t out_dilation, void* scratch,
+                           size_t scratch_bytes, svcb_stream stream) {
   g_launches = 0;
   const int r = s2d_link_factor(C);
   if (B <= 0 || !s2d_fits(L, r)) { set_error(std::string(who) + ": need C in {40, 20, 10}, L % (160/C) == 0 and L % 8 == 0"); return SVCB_E_BAD_SHAPE; }
+  S2dPlan pl;
+  if (!s2d_tap_plan(K, dilation, r, pl)) { set_error(std::string(who) + ": too many taps"); return SVCB_E_BAD_SHAPE; }
+  if (out_dilation < 1 || out_dilation > 5 || (out_dilation > 1 && (pl.fold > 1 || !y_act))) {
+    set_error(std::string(who) + ": out_dilation must be in [1, 5], and > 1 only with y_act and an unfolded input");
+    return SVCB_E_BAD_SHAPE;
+  }
   const size_t img = align256(s2d_image_bytes(B, L, r));
   SVCB_TRY(check_workspace(scratch, scratch_bytes, 4 * img + (lens_host ? (size_t)B * sizeof(int32_t) : 0), who));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1243,33 +1252,34 @@ static int op_amp_s2d_link(const char* who, const float* x, float* y, const floa
     SVCB_CUDA_CHECK(cudaMemcpyAsync(lens, lens_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   }
   SVCB_CUDA_CHECK(cudaMemsetAsync(b0, 0, 4 * img, s));
-  SVCB_TRY(launch_snake_pack_s2d(x, img4[0], img4[1], ea_in, ib_in, fu, fd, B, C, L, s, nullptr, lens, 1));
+  SVCB_TRY(launch_snake_pack_s2d(x, img4[0], img4[1], ea_in, ib_in, fu, fd, B, C, L, s, nullptr, lens, 1, pl.fold));
   SnakeW act{ea_out, ib_out, fu, fd};
   if (y_act) SVCB_TRY(snake_taps_from_device(fu, fd, &act.taps));
   AmpS2dParams q = s2d_link_params(B, C, L, K, img4, img4 + 2, y_act ? &act : nullptr);
   q.wpk = static_cast<const uint8_t*>(w_s2d); q.bias = bias; q.res = res; q.y = y; q.lens = lens;
-  if (!s2d_tap_plan(K, dilation, r, q.mlo, q.ntaps, q.tap_cols)) { set_error(std::string(who) + ": too many taps"); return SVCB_E_BAD_SHAPE; }
+  q.mlo = pl.mlo; q.ntaps = pl.ntaps; q.tap_cols = pl.tap_cols; q.fin = pl.fold; q.fout = out_dilation;
   SVCB_TRY(launch_amp_s2d_link(q, s));
-  if (y_act) SVCB_TRY(launch_s2d_unpack(q.o_hi, q.o_lo, y_act, B, C, L, s));
+  if (y_act) SVCB_TRY(launch_s2d_unpack(q.o_hi, q.o_lo, y_act, B, C, L, s, out_dilation));
   return SVCB_OK;
 }
 
 int svcb_op_amp_s2d_link(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                          const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                          const float* fd, const void* w_s2d, const float* bias, int32_t B, int32_t C, int32_t L,
-                         int32_t K, int32_t dilation, void* scratch, size_t scratch_bytes, svcb_stream stream) {
+                         int32_t K, int32_t dilation, int32_t out_dilation, void* scratch, size_t scratch_bytes,
+                         svcb_stream stream) {
   return op_amp_s2d_link("svcb_op_amp_s2d_link", x, y, res, y_act, ea_in, ib_in, ea_out, ib_out, fu, fd, w_s2d, bias,
-                         nullptr, B, C, L, K, dilation, scratch, scratch_bytes, stream);
+                         nullptr, B, C, L, K, dilation, out_dilation, scratch, scratch_bytes, stream);
 }
 
 int svcb_op_amp_s2d_link_ragged(const float* x, float* y, const float* res, float* y_act, const float* ea_in,
                                 const float* ib_in, const float* ea_out, const float* ib_out, const float* fu,
                                 const float* fd, const void* w_s2d, const float* bias, const int32_t* lens_host,
-                                int32_t B, int32_t C, int32_t L, int32_t K, int32_t dilation, void* scratch,
-                                size_t scratch_bytes, svcb_stream stream) {
+                                int32_t B, int32_t C, int32_t L, int32_t K, int32_t dilation, int32_t out_dilation,
+                                void* scratch, size_t scratch_bytes, svcb_stream stream) {
   if (!lens_host) { set_error("svcb_op_amp_s2d_link_ragged: lens_host is null"); return SVCB_E_BAD_SHAPE; }
   return op_amp_s2d_link("svcb_op_amp_s2d_link_ragged", x, y, res, y_act, ea_in, ib_in, ea_out, ib_out, fu, fd, w_s2d,
-                         bias, lens_host, B, C, L, K, dilation, scratch, scratch_bytes, stream);
+                         bias, lens_host, B, C, L, K, dilation, out_dilation, scratch, scratch_bytes, stream);
 }
 
 int svcb_op_snake_alias(const float* x, float* y, const float* ea, const float* inv_b,

@@ -359,7 +359,9 @@ struct AmpS2dParams {
                                 // FIR FMAs take them as operands and no register holds a tap
   int B = 0, C = 0, L = 0, K = 0;   // K = taps of the original conv (bookkeeping only)
   int Rp = 0;                   // image rows per (item, octet) = s2d_rows(L, r)
-  int ntaps = 0, mlo = 0;       // Toeplitz row offsets -mlo .. ntaps-1-mlo (pack.py:s2d_taps)
+  int fin = 1, fout = 1;        // folds of the input and the output image (amp_s2d.cu; at most one > 1)
+  int ntaps = 0, mlo = 0;       // Toeplitz row offsets -mlo .. ntaps-1-mlo (pack.py:s2d_taps); row shift m * fin
+  int halo = 0, stride = 0, a_off = 0;   // tile geometry (s2d_tile): set by launch_amp_s2d_link
   uint64_t tap_cols = 0;        // 3 bits per tap (s2d_tap_plan): the output columns its matrix can reach
   int accum = 0;               // y = y_old + v
   float out_div = 0.f;          // then / out_div when != 0
@@ -379,13 +381,23 @@ __host__ __device__ inline size_t qkv_heads_off(int b, int w, int h, int t, int 
 int launch_amp_s2d_link(const AmpS2dParams& p, cudaStream_t s);
 int launch_snake_pack_s2d(const float* x, void* hi, void* lo, const float* ea, const float* inv_b, const float* fu,
                           const float* fd, int B, int C, int L, cudaStream_t s, const SnakeTapsV* taps = nullptr,
-                          const int* lens = nullptr, int lscale = 1);
-int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, int L, cudaStream_t s);
+                          const int* lens = nullptr, int lscale = 1, int fold = 1);
+int launch_s2d_unpack(const void* hi, const void* lo, float* y, int B, int C, int L, cudaStream_t s, int fold = 1);
 int s2d_rows(int L, int r);
 size_t s2d_image_bytes(int B, int L, int r);
-// Toeplitz taps of a 'same' Conv1d(k, dil) over rows of r samples (pack.py:s2d_taps) and, per tap, the output
-// columns it reaches (pack.py:s2d_tap_cols) as AmpS2dParams::tap_cols; false when there are more taps than fit
-bool s2d_tap_plan(int k, int dil, int r, int& mlo, int& ntaps, uint64_t& tap_cols);
+// How a link runs: the fold of its input image, its Toeplitz taps over rows of r samples of that image (pack.py:
+// s2d_taps of the conv, or of the undilated conv when folded) and, per tap, the output columns it reaches
+// (pack.py:s2d_tap_cols) as AmpS2dParams::tap_cols
+struct S2dPlan {
+  int fold = 1, mlo = 0, ntaps = 0;
+  uint64_t tap_cols = 0;
+};
+struct S2dTile {
+  int halo = 0, stride = 0, a_off = 0;
+};
+// The plan of a c1 link, Conv1d(k, dil) (pack.py:s2d_fold); false when there are more taps than fit
+bool s2d_tap_plan(int k, int dil, int r, S2dPlan& pl);
+S2dTile s2d_tile(int r, int fin, int fout, int mlo, int mhi);
 
 // ----------------------------------------------------------------------------- fused AMP block (C = 10, 20)
 struct AmpBlockParams {

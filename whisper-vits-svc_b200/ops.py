@@ -89,10 +89,12 @@ def amp_conv_tc(x, alpha, beta, fu, fd, weight, bias, dilation=1, res=None, nspl
     return y
 
 
-def amp_s2d_link(x, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=None, alpha_out=None, beta_out=None):
+def amp_s2d_link(x, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=None, alpha_out=None, beta_out=None,
+                 out_dilation=1):
     """SnakeAlias_in -> Conv1d(C->C, K, dilation, 'same') + bias (+res) [-> SnakeAlias_out] in space-to-depth
-    form (C = 20 / 10).  Returns (y, y_act): the fp32 result and, when alpha_out is given, the next link's
-    operand image decoded back to fp32."""
+    form (C = 20 / 10), on the input fold pack.s2d_fold picks.  Returns (y, y_act): the fp32 result and, when
+    alpha_out is given, the next link's operand image decoded back to fp32 (written folded for a next link of
+    dilation out_dilation when that is > 1)."""
     x = _c(x)
     B, C, L = x.shape
     K = weight.shape[-1]
@@ -104,7 +106,7 @@ def amp_s2d_link(x, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=Non
     ea_i, ib_i = snake_params(alpha_in, beta_in)
     ea_o, ib_o = snake_params(alpha_out, beta_out) if alpha_out is not None else (None, None)
     fu, fd = _c(fu.reshape(-1).to(x.device)), _c(fd.reshape(-1).to(x.device))
-    w = pack.pack_conv_s2d_slots(weight.detach().cpu().float(), dilation, r).to(x.device)
+    w = pack.pack_conv_s2d_link(weight.detach().cpu().float(), dilation, r).to(x.device)
     b = _c(bias)
     rs = _c(res) if res is not None else None
     y = torch.empty_like(x)
@@ -113,16 +115,17 @@ def amp_s2d_link(x, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=Non
     _lib.call("op_amp_s2d_link", x.data_ptr(), y.data_ptr(), rs.data_ptr() if rs is not None else None,
               y_act.data_ptr() if y_act is not None else None, ea_i.data_ptr(), ib_i.data_ptr(),
               ea_o.data_ptr() if ea_o is not None else None, ib_o.data_ptr() if ib_o is not None else None,
-              fu.data_ptr(), fd.data_ptr(), w.data_ptr(), b.data_ptr(), B, C, L, K, dilation,
+              fu.data_ptr(), fd.data_ptr(), w.data_ptr(), b.data_ptr(), B, C, L, K, dilation, out_dilation,
               scratch.data_ptr(), scratch.numel(), device=x.device)
     return y, y_act
 
 
 def amp_s2d_link_ragged(x, lens, alpha_in, beta_in, fu, fd, weight, bias, dilation=1, res=None, alpha_out=None,
-                        beta_out=None):
+                        beta_out=None, out_dilation=1):
     """amp_s2d_link over a ragged batch: item b is x[b, :, :lens[b]] (each a multiple of 8 and of 160 / C).
     Returns (y, y_act, out_hi, out_lo): y and y_act as amp_s2d_link's, zero past each item's end, and the
-    output S2D image as written, bf16 [B, 20, Rp, 8] hi and lo (None without alpha_out)."""
+    output S2D image as written (folded when out_dilation > 1), bf16 [B, 20, Rp, 8] hi and lo (None without
+    alpha_out)."""
     x = _c(x)
     B, C, L = x.shape
     K = weight.shape[-1]
@@ -134,7 +137,7 @@ def amp_s2d_link_ragged(x, lens, alpha_in, beta_in, fu, fd, weight, bias, dilati
     ea_i, ib_i = snake_params(alpha_in, beta_in)
     ea_o, ib_o = snake_params(alpha_out, beta_out) if alpha_out is not None else (None, None)
     fu, fd = _c(fu.reshape(-1).to(x.device)), _c(fd.reshape(-1).to(x.device))
-    w = pack.pack_conv_s2d_slots(weight.detach().cpu().float(), dilation, r).to(x.device)
+    w = pack.pack_conv_s2d_link(weight.detach().cpu().float(), dilation, r).to(x.device)
     b = _c(bias)
     rs = _c(res) if res is not None else None
     ln = torch.as_tensor(lens, dtype=torch.int32).cpu().contiguous()
@@ -145,7 +148,7 @@ def amp_s2d_link_ragged(x, lens, alpha_in, beta_in, fu, fd, weight, bias, dilati
     _lib.call("op_amp_s2d_link_ragged", x.data_ptr(), y.data_ptr(), rs.data_ptr() if rs is not None else None,
               y_act.data_ptr() if y_act is not None else None, ea_i.data_ptr(), ib_i.data_ptr(),
               ea_o.data_ptr() if ea_o is not None else None, ib_o.data_ptr() if ib_o is not None else None,
-              fu.data_ptr(), fd.data_ptr(), w.data_ptr(), b.data_ptr(), ln.data_ptr(), B, C, L, K, dilation,
+              fu.data_ptr(), fd.data_ptr(), w.data_ptr(), b.data_ptr(), ln.data_ptr(), B, C, L, K, dilation, out_dilation,
               scratch.data_ptr(), scratch.numel(), device=x.device)
     if alpha_out is None:
         return y, y_act, None, None

@@ -153,6 +153,48 @@ def pack_conv_s2d_slots(w: torch.Tensor, dil: int, r: int) -> torch.Tensor:
     return img[:, :, :, s2d_column_order(r)].contiguous().view(torch.float32).reshape(-1)
 
 
+S2D_FOLD_MAX = 5   # largest fold of a folded S2D image (csrc/amp_s2d.cu)
+
+
+def s2d_tile(r: int, fin: int, fout: int, mlo: int, mhi: int):
+    """(halo, stride, a_off) of a link's tiles: halo rows on each side, useful rows per tile, A-panel row of the
+    tile's first row, for an input image of fold fin and an output image of fold fout — must match
+    csrc/amp_s2d.cu:s2d_tile.  A folded input has tiles of whole blocks and a halo of one block; a folded output has
+    whole output blocks of useful rows."""
+    if fin > 1:
+        rows = min(128, 144 - (mlo + mhi) * fin) // fin * fin
+        return fin, rows - 2 * fin, mlo * fin
+    halo = 1 if r >= 8 else 2
+    return halo, (128 - 2 * halo) // fout * fout, 8
+
+
+def _col_units(k: int, dil: int, r: int) -> int:
+    return sum((n1 - n0) // 40 for n0, n1 in s2d_tap_cols(k, dil, r))
+
+
+def s2d_fold(k: int, dil: int, r: int) -> int:
+    """The fold a c1 link Conv1d(k, dil) reads its input in: dil when the link has more than 3 full taps of column
+    work and the undilated conv's column work per useful tile row is lower, else 1 — must match
+    csrc/amp_s2d.cu:s2d_tap_plan.  Folded, row
+    b*dil + q of the image holds the samples b*r*dil + q + j*dil and tap m shifts by m*dil rows."""
+    if dil < 2 or dil > S2D_FOLD_MAX:
+        return 1
+    mlo, mhi = s2d_taps(k, dil, r)
+    ulo, uhi = s2d_taps(k, 1, r)
+    _, s1, _ = s2d_tile(r, 1, 1, mlo, mhi)
+    hd, sd, ad = s2d_tile(r, dil, 1, ulo, uhi)
+    if sd <= 0 or hd + ad > 16:
+        return 1
+    cu = _col_units(k, dil, r)      # links of up to 3 full taps are bound by their Snake epilogue: left unfolded
+    return dil if cu > 12 and _col_units(k, 1, r) * s1 < cu * sd else 1
+
+
+def pack_conv_s2d_link(w: torch.Tensor, dil: int, r: int) -> torch.Tensor:
+    """The weights of a link Conv1d(w, dil) as csrc/amp_s2d.cu runs it: pack_conv_s2d_slots of the conv, or of
+    the undilated conv when the link reads a folded input (s2d_fold)."""
+    return pack_conv_s2d_slots(w, 1 if s2d_fold(w.shape[-1], dil, r) > 1 else dil, r)
+
+
 def tc_tiling(cout: int, cin: int):
     """(kch, cin_pad, bn, ntiles) — must match csrc/api.cu:tc_tiling."""
     kch = 32
@@ -333,7 +375,7 @@ def pack_svc_state_dict(sd: Dict[str, torch.Tensor], cfg: dict) -> List[Tuple[st
             put(f"dec.res.{n}.c1.{d}.tc", pack_conv_tc(w1))
             put(f"dec.res.{n}.c2.{d}.tc", pack_conv_tc(w2))
             if r:   # narrow stages: block-Toeplitz matrices for csrc/amp_s2d.cu
-                put(f"dec.res.{n}.c1.{d}.s2d", pack_conv_s2d_slots(w1, cfg["res_dilations"][j][d], r))
+                put(f"dec.res.{n}.c1.{d}.s2d", pack_conv_s2d_link(w1, cfg["res_dilations"][j][d], r))
                 put(f"dec.res.{n}.c2.{d}.s2d", pack_conv_s2d_slots(w2, 1, r))
         for a in range(6):
             _snake(put, f"dec.res.{n}.act.{a}", sd, f"{p}.activations.{a}")
