@@ -315,6 +315,26 @@ size_t svcb_praat_f0_workspace_bytes(int64_t total_samples, int32_t B);
 int svcb_praat_f0_ragged(const double* x, const int64_t* offsets_host, int32_t B, double* out, void* ws, size_t ws_bytes,
                          svcb_stream stream);
 
+/* ------------------------------------------------------------------ salience-based F0 (pitch/inference.py) */
+/* Replaces pitch/inference.py:31-41 before its np.repeat and moving average: libf0's salience(x, Fs=16000, H=320, N=2048,
+ * F_min=45, F_max=1760) with its defaults (10 cents per bin, 636 bins, 10 harmonics weighted 0.9^idx, smoothing over 11
+ * bins, gamma 0, transitions within 5 bins at 1 and beyond at 0.01, no constraint region), in fp64, for a ragged batch:
+ * item b is x[offsets_host[b] .. offsets_host[b+1]) (float32, n_b >= 320 samples at 16 kHz: two frames); B >= 1.
+ * f0: float64, item b's n_b / 320 + 1 frames following item b-1's from f0[0].  Optional taps, each may be NULL, laid out
+ * per item as [636][frames] blocks following each other from index 0 (item b's at 636 x its first frame): y_tap the
+ * binned spectrogram before smoothing, z_tap the thresholded salience; path_tap (int32, one per frame) the bins of the
+ * path.  Each item is bitwise that of a lone call.  ws: svcb_salience_f0_workspace_bytes(sum of n_b, B) bytes,
+ * 256-byte aligned (about 30 bytes per sample). */
+size_t svcb_salience_f0_workspace_bytes(int64_t total_samples, int32_t B);
+int svcb_salience_f0_ragged(const float* x, const int64_t* offsets_host, int32_t B, double* f0, double* y_tap,
+                            double* z_tap, int32_t* path_tap, void* ws, size_t ws_bytes, svcb_stream stream);
+/* The DP and trace back alone, on a given salience: item b is z[636 x frame_offsets_host[b] ..) as [636][F_b]
+ * (F_b = frame_offsets_host[b+1] - frame_offsets_host[b] >= 1, frame_offsets_host[0] >= 0); path: int32, the path's
+ * bins, F_b per item following each other from path[0], whatever frame_offsets_host[0] is.  ws: svcb_salience_dp_workspace_bytes(sum of F_b) bytes, 256-byte aligned. */
+size_t svcb_salience_dp_workspace_bytes(int64_t total_frames);
+int svcb_salience_dp_ragged(const double* z, const int64_t* frame_offsets_host, int32_t B, int32_t* path, void* ws,
+                            size_t ws_bytes, svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */

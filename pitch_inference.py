@@ -2,7 +2,11 @@
 """Drop-in for the reference's pitch/inference.py (same flags): the F0 of one recording by CREPE-full on the H100
 (`compute_f0_sing`: 20 ms hop, Viterbi in 512-frame segments, every value twice, mean over 5), written as the `.pit.csv`
 the inference command lines read, one line per 10 ms.  The weights are crepe/assets/full.pth, where the reference keeps
-them.  The wav is read as `hubert_infer.load_audio` reads it (16 kHz)."""
+them.  The wav is read as `hubert_infer.load_audio` reads it (16 kHz).
+
+--f0 picks another of the reference's extractors, each on the device and written by the same `save_csv_pitch`:
+`mouth` is compute_f0_mouth (Praat's autocorrelation pitch, praat_f0.py) and `salience` is compute_f0_salience
+(libf0's salience tracker, salience_f0.py).  The default, `sing`, is the CREPE path above."""
 import argparse
 import os
 import sys
@@ -22,10 +26,17 @@ if __name__ == "__main__":
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
     parser.add_argument("-p", "--pit", help="pit", dest="pit", required=True)  # csv for excel
+    parser.add_argument("--f0", choices=("sing", "mouth", "salience"), default="sing", help="F0 extractor")
     args = parser.parse_args()
     print(args.wav)
     print(args.pit)
     require_cuda()
-    from whisper_vits_svc_b200 import crepe_infer
+    if args.f0 == "sing":
+        from whisper_vits_svc_b200 import crepe_infer
 
-    crepe_infer.pred_pit(crepe_infer.load_model(MODEL, "cuda"), args.wav, args.pit)
+        crepe_infer.pred_pit(crepe_infer.load_model(MODEL, "cuda"), args.wav, args.pit)
+    else:
+        from whisper_vits_svc_b200 import hostio, praat_f0, salience_f0
+
+        compute = praat_f0.compute_f0_mouth if args.f0 == "mouth" else salience_f0.compute_f0_salience
+        hostio.save_csv_pitch(compute(args.wav, "cuda"), args.pit)
