@@ -183,13 +183,7 @@ WHISPER_PIN_CASES = [(dict(n_audio_state=256, n_audio_head=4, n_audio_layer=8), 
                      (dict(n_audio_state=384, n_audio_head=6, n_audio_layer=4), 1, 77)]
 
 
-def to_float64(x):
-    """Floating tensors of a (nested) dict / tensor as float64; everything else unchanged."""
-    if torch.is_tensor(x):
-        return x.double() if x.is_floating_point() else x
-    if isinstance(x, dict):
-        return {k: to_float64(v) for k, v in x.items()}
-    return x
+to_float64 = O.to_float64
 
 
 @contextlib.contextmanager

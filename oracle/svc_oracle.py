@@ -44,6 +44,16 @@ def fold_weight_norm(sd: SD, prefix: str) -> torch.Tensor:
     return torch._weight_norm(v, g, 0)
 
 
+def to_float64(x):
+    """Floating tensors of a (nested) dict / tensor as float64; everything else unchanged.  Every function
+    of this module runs unchanged on a float64 state dict and float64 inputs."""
+    if torch.is_tensor(x):
+        return x.double() if x.is_floating_point() else x
+    if isinstance(x, dict):
+        return {k: to_float64(v) for k, v in x.items()}
+    return x
+
+
 def sequence_mask(lengths: torch.Tensor, max_len: int) -> torch.Tensor:
     """vits/commons.py:147-151"""
     pos = torch.arange(max_len, dtype=lengths.dtype, device=lengths.device)
@@ -127,32 +137,47 @@ def ffn(sd: SD, p: str, x: torch.Tensor, mask: torch.Tensor, k: int = 3):
     return h * mask
 
 
-def prior_encoder(sd: SD, ppg, ppg_l, vec, pit, eps, n_layers=6, stages: Optional[dict] = None):
-    """TextEncoder.forward, vits/models.py:39-52; Encoder.forward attentions.py:60-72.
-    `eps` replaces torch.randn_like(m) at models.py:51."""
+def prior_front(sd: SD, ppg, ppg_l, vec, pit):
+    """TextEncoder.forward up to the encoder (vits/models.py:40-46): pre(ppg) + hub(vec) + pit embedding.
+    Returns the sum (unmasked, as the encoder receives it) and the frame mask [B,1,T]."""
     f0c = f0_to_coarse(pit)
     x = ppg.transpose(1, -1)
     mask = sequence_mask(ppg_l, x.shape[2]).unsqueeze(1).to(x.dtype)
     x = F.conv1d(x, sd["enc_p.pre.weight"], sd["enc_p.pre.bias"], padding=2) * mask
     v = F.conv1d(vec.transpose(1, -1), sd["enc_p.hub.weight"], sd["enc_p.hub.bias"], padding=2) * mask
-    x = x + v + F.embedding(f0c, sd["enc_p.pit.weight"]).transpose(1, 2)
-    if stages is not None:
-        stages["enc_front"] = x
+    return x + v + F.embedding(f0c, sd["enc_p.pit.weight"]).transpose(1, 2), mask
+
+
+def encoder_layer(sd: SD, i: int, x, mask):
+    """Encoder layer i (attentions.py:63-70): attention + LayerNorm, FFN + LayerNorm."""
+    e = "enc_p.enc."
     attn_mask = mask.unsqueeze(2) * mask.unsqueeze(-1)
-    x = x * mask
-    for i in range(n_layers):
-        e = "enc_p.enc."
-        y = rel_attention(sd, f"{e}attn_layers.{i}", x, attn_mask)
-        x = channel_layer_norm(x + y, sd[f"{e}norm_layers_1.{i}.gamma"], sd[f"{e}norm_layers_1.{i}.beta"])
-        y = ffn(sd, f"{e}ffn_layers.{i}", x, mask)
-        x = channel_layer_norm(x + y, sd[f"{e}norm_layers_2.{i}.gamma"], sd[f"{e}norm_layers_2.{i}.beta"])
-        if stages is not None:
-            stages[f"enc_layer{i}"] = x
+    y = rel_attention(sd, f"{e}attn_layers.{i}", x, attn_mask)
+    x = channel_layer_norm(x + y, sd[f"{e}norm_layers_1.{i}.gamma"], sd[f"{e}norm_layers_1.{i}.beta"])
+    y = ffn(sd, f"{e}ffn_layers.{i}", x, mask)
+    return channel_layer_norm(x + y, sd[f"{e}norm_layers_2.{i}.gamma"], sd[f"{e}norm_layers_2.{i}.beta"])
+
+
+def prior_proj(sd: SD, x, mask, eps):
+    """The encoder's final mask (attentions.py:71), proj and the reparameterisation (vits/models.py:48-51)."""
     x = x * mask
     stats = F.conv1d(x, sd["enc_p.proj.weight"], sd["enc_p.proj.bias"]) * mask
     m, logs = torch.split(stats, stats.shape[1] // 2, dim=1)
-    z_p = (m + eps * torch.exp(logs)) * mask
-    return z_p, mask
+    return (m + eps * torch.exp(logs)) * mask
+
+
+def prior_encoder(sd: SD, ppg, ppg_l, vec, pit, eps, n_layers=6, stages: Optional[dict] = None):
+    """TextEncoder.forward, vits/models.py:39-52; Encoder.forward attentions.py:60-72.
+    `eps` replaces torch.randn_like(m) at models.py:51."""
+    x, mask = prior_front(sd, ppg, ppg_l, vec, pit)
+    if stages is not None:
+        stages["enc_front"] = x
+    x = x * mask
+    for i in range(n_layers):
+        x = encoder_layer(sd, i, x, mask)
+        if stages is not None:
+            stages[f"enc_layer{i}"] = x
+    return prior_proj(sd, x, mask, eps), mask
 
 
 # --------------------------------------------------------------------------- flow
@@ -235,12 +260,8 @@ def amp_block(sd: SD, p: str, x: torch.Tensor, k: int, dilations=(1, 3, 5)) -> t
     return x
 
 
-def generator(sd: SD, hp, spk, x, source, stages: Optional[dict] = None):
-    """Generator.inference, vits_decoder/generator.py:175-200 (+ SpeakerAdapter :36-47)."""
-    rates = list(hp.gen.upsample_rates)
-    ksz = list(hp.gen.upsample_kernel_sizes)
-    rk = list(hp.gen.resblock_kernel_sizes)
-    rd = [tuple(d) for d in hp.gen.resblock_dilation_sizes]
+def gen_pre(sd: SD, spk, x):
+    """SpeakerAdapter (generator.py:36-47) -> conv_pre -> Mish (generator.py:177-179)."""
     # SpeakerAdapter: biased variance, eps inside the sqrt
     xt = x.transpose(1, -1)
     mean = xt.mean(dim=-1, keepdim=True)
@@ -251,30 +272,53 @@ def generator(sd: SD, hp, spk, x, source, stages: Optional[dict] = None):
     y = y * scale.unsqueeze(1) + bias.unsqueeze(1)
     x = y.transpose(1, -1)
     x = F.conv1d(x, sd["dec.conv_pre.weight"], sd["dec.conv_pre.bias"], padding=3)
-    x = x * torch.tanh(F.softplus(x))
-    if stages is not None:
-        stages["gen_pre"] = x
-    for i, (u, k) in enumerate(zip(rates, ksz)):
-        w = fold_weight_norm(sd, f"dec.ups.{i}")
-        x = F.conv_transpose1d(x, w, sd[f"dec.ups.{i}.bias"], stride=u, padding=(k - u) // 2)
-        nw = sd[f"dec.noise_convs.{i}.weight"]
-        if i + 1 < len(rates):
-            s = int(np.prod(rates[i + 1:]))
-            x = x + F.conv1d(source, nw, sd[f"dec.noise_convs.{i}.bias"], stride=s, padding=s // 2)
-        else:
-            x = x + F.conv1d(source, nw, sd[f"dec.noise_convs.{i}.bias"])
-        if stages is not None:
-            stages[f"gen_up{i}"] = x
-        acc = None
-        for j, kk in enumerate(rk):
-            r = amp_block(sd, f"dec.resblocks.{i * len(rk) + j}", x, kk, rd[j])
-            acc = r if acc is None else acc + r
-        x = acc / len(rk)
-        if stages is not None:
-            stages[f"gen_stage{i}"] = x
+    return x * torch.tanh(F.softplus(x))
+
+
+def gen_upsample(sd: SD, hp, i: int, x, source):
+    """Stage i's input: ups[i](x) + noise_convs[i](source) (generator.py:183-186)."""
+    rates = list(hp.gen.upsample_rates)
+    u, k = rates[i], list(hp.gen.upsample_kernel_sizes)[i]
+    w = fold_weight_norm(sd, f"dec.ups.{i}")
+    x = F.conv_transpose1d(x, w, sd[f"dec.ups.{i}.bias"], stride=u, padding=(k - u) // 2)
+    nw = sd[f"dec.noise_convs.{i}.weight"]
+    if i + 1 < len(rates):
+        s = int(np.prod(rates[i + 1:]))
+        return x + F.conv1d(source, nw, sd[f"dec.noise_convs.{i}.bias"], stride=s, padding=s // 2)
+    return x + F.conv1d(source, nw, sd[f"dec.noise_convs.{i}.bias"])
+
+
+def gen_amp_stage(sd: SD, hp, i: int, x):
+    """Stage i's output: the mean of its AMP blocks (generator.py:188-194)."""
+    rk = list(hp.gen.resblock_kernel_sizes)
+    rd = [tuple(d) for d in hp.gen.resblock_dilation_sizes]
+    acc = None
+    for j, kk in enumerate(rk):
+        r = amp_block(sd, f"dec.resblocks.{i * len(rk) + j}", x, kk, rd[j])
+        acc = r if acc is None else acc + r
+    return acc / len(rk)
+
+
+def gen_tail(sd: SD, x):
+    """activation_post -> conv_post -> tanh (generator.py:196-199)."""
     x = snake_alias(sd, "dec.activation_post", x)
     x = F.conv1d(x, sd["dec.conv_post.weight"], None, padding=3)
     return torch.tanh(x)
+
+
+def generator(sd: SD, hp, spk, x, source, stages: Optional[dict] = None):
+    """Generator.inference, vits_decoder/generator.py:175-200 (+ SpeakerAdapter :36-47)."""
+    x = gen_pre(sd, spk, x)
+    if stages is not None:
+        stages["gen_pre"] = x
+    for i in range(len(hp.gen.upsample_rates)):
+        x = gen_upsample(sd, hp, i, x, source)
+        if stages is not None:
+            stages[f"gen_up{i}"] = x
+        x = gen_amp_stage(sd, hp, i, x)
+        if stages is not None:
+            stages[f"gen_stage{i}"] = x
+    return gen_tail(sd, x)
 
 
 # --------------------------------------------------------------------------- NSF source
