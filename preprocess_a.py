@@ -13,14 +13,15 @@ import os
 import sys
 
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
+from whisper_vits_svc_b200 import dataset
 
 MAX_PADDED = 64 * 30 * 48000   # padded input samples per device batch: 64 clips of 30 s at 48 kHz, about 0.8 GB
 
 
 def resample_jobs(wav_dir, out_dir):
-    """(wav path, output path) of every file: prepare/preprocess_a.py's walk, in sorted order."""
-    from whisper_vits_svc_b200 import dataset
-    return dataset.speaker_wavs(wav_dir, out_dir, ".wav")
+    """(wav path, output path) of every file: prepare/preprocess_a.py's walk, in sorted order; under torchrun, this
+    rank's share of them (dataset.rank_share)."""
+    return dataset.rank_share(dataset.speaker_wavs(wav_dir, out_dir, ".wav"))
 
 
 def load_clip(path):
@@ -57,6 +58,7 @@ def resample_files(jobs, sr, threads, batch, max_padded=MAX_PADDED, device="cuda
                                max_padded=max_padded)
 
 
+@dataset.rank_main
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
@@ -81,8 +83,7 @@ def main(argv=None):
         st = resample_files(jobs, args.sr, threads, args.batch)
     finally:
         resample.release_filters()
-    if st["failed"]:
-        print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    dataset.report_failed(st["failed"], len(jobs))
     return 0
 
 

@@ -17,14 +17,15 @@ sys.path.append(os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
 from pitch_inference import MODEL, require_cuda
+from whisper_vits_svc_b200 import dataset
 
 MAX_PADDED = 64 * 30 * 16000   # padded samples per device batch: 64 items of 30 s
 
 
 def pit_jobs(wav_dir, pit_dir):
-    """(wav path, output path without .npy) of every file: prepare/preprocess_crepe.py:62-69."""
-    from whisper_vits_svc_b200 import dataset
-    return dataset.speaker_wavs(wav_dir, pit_dir, ".pit")
+    """(wav path, output path without .npy) of every file: prepare/preprocess_crepe.py:62-69; under torchrun, this
+    rank's share of them (dataset.rank_share)."""
+    return dataset.rank_share(dataset.speaker_wavs(wav_dir, pit_dir, ".pit"))
 
 
 def extract_pitch(jobs, model, threads, batch, max_padded=MAX_PADDED):
@@ -44,6 +45,7 @@ def extract_pitch(jobs, model, threads, batch, max_padded=MAX_PADDED):
                                size=lambda a: a.shape[0], max_padded=max_padded)
 
 
+@dataset.rank_main
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
@@ -59,8 +61,7 @@ def main(argv=None):
     jobs = pit_jobs(args.wav, args.pit)
     model = crepe_infer.load_model(MODEL, "cuda")
     st = extract_pitch(jobs, model, os.cpu_count() if args.threads == 0 else args.threads, args.batch)
-    if st["failed"]:
-        print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    dataset.report_failed(st["failed"], len(jobs))
     return 0
 
 

@@ -17,13 +17,15 @@ import sys
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
+from whisper_vits_svc_b200 import dataset
+
 MAX_PADDED = 64 * 30 * 16000   # padded samples per device batch: 64 items of 30 s
 
 
 def pit_jobs(wav_dir, pit_dir):
-    """(wav path, output path without .npy) of every file: prepare/preprocess_f0_mouth.py's walk."""
-    from whisper_vits_svc_b200 import dataset
-    return dataset.speaker_wavs(wav_dir, pit_dir, ".pit")
+    """(wav path, output path without .npy) of every file: prepare/preprocess_f0_mouth.py's walk; under torchrun, this
+    rank's share of them (dataset.rank_share)."""
+    return dataset.rank_share(dataset.speaker_wavs(wav_dir, pit_dir, ".pit"))
 
 
 def load(wav):
@@ -36,7 +38,6 @@ def load(wav):
 
 def extract_f0(jobs, run, threads, batch, max_padded=MAX_PADDED):
     """Write every job's .pit.npy; run(list of clips) -> list of padded float64 F0 arrays."""
-    from whisper_vits_svc_b200 import dataset
 
     out = dict(jobs)
     return dataset.run_batched(list(out), load, run,
@@ -44,6 +45,7 @@ def extract_f0(jobs, run, threads, batch, max_padded=MAX_PADDED):
                                threads, batch, size=lambda a: a.shape[0], max_padded=max_padded)
 
 
+@dataset.rank_main
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
@@ -62,8 +64,7 @@ def main(argv=None):
         st = extract_f0(jobs, ex.f0_batch, os.cpu_count() if args.thread_count == 0 else args.thread_count, args.batch)
     finally:
         ex.close()
-    if st["failed"]:
-        print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    dataset.report_failed(st["failed"], len(jobs))
     return 0
 
 

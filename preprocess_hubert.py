@@ -15,13 +15,15 @@ import sys
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
+from whisper_vits_svc_b200 import dataset
+
 MAX_PADDED = 32 * 20 * 16000   # padded samples per device batch: 32 items of 20 s, about 9 GB of workspace
 
 
 def vec_jobs(wav_dir, vec_dir):
-    """(wav path, output path without .npy) of every file: prepare/preprocess_hubert.py:51-58."""
-    from whisper_vits_svc_b200 import dataset
-    return dataset.speaker_wavs(wav_dir, vec_dir, ".vec")
+    """(wav path, output path without .npy) of every file: prepare/preprocess_hubert.py:51-58; under torchrun, this
+    rank's share of them (dataset.rank_share)."""
+    return dataset.rank_share(dataset.speaker_wavs(wav_dir, vec_dir, ".vec"))
 
 
 def extract_vecs(jobs, hubert, threads, batch, max_padded=MAX_PADDED):
@@ -42,6 +44,7 @@ def extract_vecs(jobs, hubert, threads, batch, max_padded=MAX_PADDED):
                                size=lambda a: a.shape[0], max_padded=max_padded)
 
 
+@dataset.rank_main
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
@@ -57,8 +60,7 @@ def main(argv=None):
     hubert = hubert_infer.load_model(os.path.join("hubert_pretrain", "hubert-soft-0d54a1f4.pt"), "cuda")
     st = extract_vecs(jobs, hubert, os.cpu_count() if args.threads == 0 else args.threads, args.batch)
     print(f"padding overhead: {st['padded'] / max(st['samples'], 1):.3f} (padded samples / samples)")
-    if st["failed"]:
-        print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    dataset.report_failed(st["failed"], len(jobs))
     return 0
 
 

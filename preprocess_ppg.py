@@ -15,13 +15,17 @@ import sys
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
+from whisper_vits_svc_b200 import dataset
+
 MAX_PADDED = 32 * 30 * 16000   # padded samples per device batch: 32 items of 30 s, about 1.4 GB of large-v2 workspace
 
 
 def ppg_jobs(wav_dir, ppg_dir):
-    """(wav path, output path without .npy) of every file still to do: prepare/preprocess_ppg.py:57-69."""
-    from whisper_vits_svc_b200 import dataset
-    return [(w, p) for w, p in dataset.speaker_wavs(wav_dir, ppg_dir, ".ppg") if not os.path.isfile(f"{p}.npy")]
+    """(wav path, output path without .npy) of every file still to do: prepare/preprocess_ppg.py:57-69.  Under
+    torchrun the full walk is shared before the done files are dropped, so that other ranks' new outputs cannot
+    change this rank's share."""
+    return [(w, p) for w, p in dataset.rank_share(dataset.speaker_wavs(wav_dir, ppg_dir, ".ppg"))
+            if not os.path.isfile(f"{p}.npy")]
 
 
 def extract_ppgs(jobs, whisper, threads, batch, max_padded=MAX_PADDED):
@@ -43,6 +47,7 @@ def extract_ppgs(jobs, whisper, threads, batch, max_padded=MAX_PADDED):
                                max_padded=max_padded)
 
 
+@dataset.rank_main
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
@@ -58,8 +63,7 @@ def main(argv=None):
     whisper = whisper_infer.load_model(os.path.join("whisper_pretrain", "large-v2.pt"), "cuda")
     st = extract_ppgs(jobs, whisper, os.cpu_count() if args.threads == 0 else args.threads, args.batch)
     print(f"padding overhead: {st['padded'] / max(st['samples'], 1):.3f} (padded samples / samples)")
-    if st["failed"]:
-        print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    dataset.report_failed(st["failed"], len(jobs))
     return 0
 
 

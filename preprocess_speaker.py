@@ -14,9 +14,12 @@ from argparse import RawTextHelpFormatter
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
 import numpy as np
 
+from whisper_vits_svc_b200 import dataset
+
 
 def get_spk_wavs(dataset_path, output_path):
-    """prepare/preprocess_speaker.py:18-29 (creates the output directories as the reference does)."""
+    """prepare/preprocess_speaker.py:18-29 (creates the output directories as the reference does); under torchrun,
+    this rank's share of the files."""
     wav_files = []
     os.makedirs(f"./{output_path}", exist_ok=True)
     for spks in os.listdir(dataset_path):
@@ -27,7 +30,7 @@ def get_spk_wavs(dataset_path, output_path):
                     wav_files.append(f"./{dataset_path}/{spks}/{file}")
         elif spks.endswith(".wav"):
             wav_files.append(f"./{dataset_path}/{spks}")
-    return wav_files
+    return dataset.rank_share(wav_files, path=lambda w: w)
 
 
 def embed_path(wav_file, dataset_path, output_path):
@@ -38,7 +41,6 @@ def embed_path(wav_file, dataset_path, output_path):
 def extract_speaker_embeddings(wav_files, dataset_path, output_path, model, concurrency, batch=32):
     """Embed every file in device batches; returns the number of files that failed (each is reported and skipped).
     The loader threads run at most two batches ahead of the device, so host memory stays bounded."""
-    from whisper_vits_svc_b200 import dataset
 
     def save(f, e):
         np.save(embed_path(f, dataset_path, output_path), e, allow_pickle=False)
@@ -47,6 +49,7 @@ def extract_speaker_embeddings(wav_files, dataset_path, output_path, model, conc
                                save, concurrency, batch)["failed"]
 
 
+@dataset.rank_main
 def main(argv=None):
     parser = argparse.ArgumentParser(description="""Compute embedding vectors for each wav file in a dataset.""",
                                      formatter_class=RawTextHelpFormatter)
@@ -64,8 +67,7 @@ def main(argv=None):
     wav_files = get_spk_wavs(args.dataset_path, args.output_path)
     process_num = os.cpu_count() if args.thread_count == 0 else args.thread_count
     n_failed = extract_speaker_embeddings(wav_files, args.dataset_path, args.output_path, model, process_num, args.batch)
-    if n_failed:
-        print(f"{n_failed} of {len(wav_files)} files failed", file=sys.stderr)
+    dataset.report_failed(n_failed, len(wav_files))
     return 0
 
 

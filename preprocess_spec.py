@@ -14,13 +14,15 @@ import sys
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
 import torch
 
+from whisper_vits_svc_b200 import dataset
+
 MAX_PADDED = 64 * 30 * 32000   # padded samples per device batch: 64 clips of 30 s, about 0.6 GB of audio and spectra
 
 
 def spec_jobs(wav_dir, spe_dir):
-    """(wav path, output path) of every file: prepare/preprocess_spec.py's walk."""
-    from whisper_vits_svc_b200 import dataset
-    return dataset.speaker_wavs(wav_dir, spe_dir, ".pt")
+    """(wav path, output path) of every file: prepare/preprocess_spec.py's walk; under torchrun, this rank's share of
+    them (dataset.rank_share)."""
+    return dataset.rank_share(dataset.speaker_wavs(wav_dir, spe_dir, ".pt"))
 
 
 def compute_specs(jobs, hp, threads, batch, max_padded=MAX_PADDED, device="cuda"):
@@ -37,6 +39,7 @@ def compute_specs(jobs, hp, threads, batch, max_padded=MAX_PADDED, device="cuda"
                                size=len, max_padded=max_padded)
 
 
+@dataset.rank_main
 def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-w", "--wav", help="wav", dest="wav", required=True)
@@ -58,8 +61,7 @@ def main(argv=None):
     jobs = spec_jobs(args.wav, args.spe)
     threads = os.cpu_count() // 2 + 1 if args.thread_count == 0 else args.thread_count
     st = compute_specs(jobs, hp, threads, args.batch)
-    if st["failed"]:
-        print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    dataset.report_failed(st["failed"], len(jobs))
     return 0
 
 

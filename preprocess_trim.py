@@ -15,14 +15,15 @@ import os
 import sys
 
 sys.path.append(os.path.dirname(os.path.abspath(__file__)))
+from whisper_vits_svc_b200 import dataset
 
 MAX_PADDED = 64 * 30 * 48000   # samples per device batch, as the other preprocess CLIs plan them
 
 
 def trim_jobs(in_dir, out_dir):
-    """(wav path, output path) of every file: prepare/preprocess_trim.py's walk, in sorted order."""
-    from whisper_vits_svc_b200 import dataset
-    return dataset.speaker_wavs(in_dir, out_dir, ".wav")
+    """(wav path, output path) of every file: prepare/preprocess_trim.py's walk, in sorted order; under torchrun, this
+    rank's share of them (dataset.rank_share)."""
+    return dataset.rank_share(dataset.speaker_wavs(in_dir, out_dir, ".wav"))
 
 
 def save_trimmed(wav, out_path, x, rate, flags):
@@ -53,19 +54,24 @@ def trim_files(jobs, threads, batch, max_padded=MAX_PADDED, device="cuda"):
                                max_padded=max_padded)
 
 
-if __name__ == "__main__":
+@dataset.rank_main
+def main(argv=None):
     parser = argparse.ArgumentParser()
     parser.add_argument("-i", help="input path", dest="inPath", required=True)
     parser.add_argument("-o", help="output path", dest="outPath", required=True)
     parser.add_argument("-t", "--thread_count", help="thread count to process, set 0 to use all cpu cores",
                         dest="thread_count", type=int, default=1)
     parser.add_argument("--batch", type=int, default=64, help="maximum files per device batch")
-    args = parser.parse_args()
+    args = parser.parse_args(argv)
     print(args.inPath)
     print(args.outPath)
     os.makedirs(args.outPath, exist_ok=True)
     jobs = trim_jobs(args.inPath, args.outPath)
     threads = os.cpu_count() // 2 + 1 if args.thread_count == 0 else args.thread_count
     st = trim_files(jobs, threads, args.batch)
-    if st["failed"]:
-        print(f"{st['failed']} of {len(jobs)} files failed", file=sys.stderr)
+    dataset.report_failed(st["failed"], len(jobs))
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -6,7 +6,12 @@ Every step runs its CLI's `main` in this one process, so torch is imported, the 
 loaded once instead of ten times.  The models are loaded one step at a time and each `main` frees its model before it
 returns, so the peak device memory is that of the largest step.  Files that fail inside a step are reported and
 skipped by that step; a step that returns non-zero or raises stops the run with status 1, as the reference's loop
-stops at the first failing command.  -t is accepted and, as in the reference, not passed on to the steps."""
+stops at the first failing command.  -t is accepted and, as in the reference, not passed on to the steps.
+
+Under torchrun (`python -m torch.distributed.run --nproc-per-node 8 svc_preprocessing.py`) each rank runs the device
+steps (1-6 and 8) on its share of the files on cuda:(LOCAL_RANK % device count), and rank 0 alone runs the speaker
+average, the file lists and the loader check (7, 9 and 10) once the others are done.  A step that fails on any rank
+stops every rank with status 1."""
 import argparse
 import gc
 import importlib
@@ -29,6 +34,8 @@ STEPS = [
     "preprocess_train.py",
     "preprocess_zzz.py",
 ]
+# the steps that take the whole data set on the host: under torchrun, rank 0 runs them alone
+HOST_STEPS = ("preprocess_speaker_ave.py", "preprocess_train.py", "preprocess_zzz.py")
 
 
 def step_main(step):
@@ -37,28 +44,43 @@ def step_main(step):
     return importlib.import_module(script[:-len(".py")]).main, argv
 
 
+def run_steps(steps, step_main=step_main):
+    """Run `steps` in turn; 0, or 1 at the first step that raises or returns non-zero.  Under torchrun every rank
+    runs the device steps on its share of the files, and rank 0 alone runs the host steps while the others wait.
+    After each step the ranks agree on its status, so that all of them stop at a failing step and none is left
+    waiting for another; they share one gloo group over all the steps."""
+    from whisper_vits_svc_b200 import dataset, shard
+    rank = shard.env_world()[0]
+    with dataset.process_group():
+        for step in steps:
+            if rank == 0:
+                print(f"Command: python {step}", flush=True)
+            status = 0
+            if rank == 0 or step.split()[0] not in HOST_STEPS:
+                try:
+                    run, step_argv = step_main(step)   # an import that fails on one rank still joins the agreement
+                    status = run(step_argv)
+                except (Exception, SystemExit):
+                    traceback.print_exc()
+                    status = 1
+                finally:
+                    sys.stdout.flush()
+                    gc.collect()
+                    torch.cuda.empty_cache()
+            if dataset.sum_over_ranks([int(bool(status))])[0]:
+                return 1
+    return 0
+
+
 def main(argv=None):
     assert torch.cuda.is_available(), "\033[31m You need GPU to Train! \033[0m"
-    print("CPU Count is :", os.cpu_count())
+    from whisper_vits_svc_b200 import shard
+    if shard.env_world()[0] == 0:
+        print("CPU Count is :", os.cpu_count())
     parser = argparse.ArgumentParser()
     parser.add_argument("-t", type=int, default=0, help="thread count")
     parser.parse_args(argv)
-
-    for step in STEPS:
-        print(f"Command: python {step}", flush=True)
-        run, step_argv = step_main(step)
-        try:
-            status = run(step_argv)
-        except (Exception, SystemExit):
-            traceback.print_exc()
-            return 1
-        finally:
-            sys.stdout.flush()
-            gc.collect()
-            torch.cuda.empty_cache()
-        if status:
-            return 1
-    return 0
+    return run_steps(STEPS)
 
 
 if __name__ == "__main__":
