@@ -335,6 +335,35 @@ size_t svcb_salience_dp_workspace_bytes(int64_t total_frames);
 int svcb_salience_dp_ragged(const double* z, const int64_t* frame_offsets_host, int32_t B, int32_t* path, void* ws,
                             size_t ws_bytes, svcb_stream stream);
 
+/* ------------------------------------------------------------------ pYIN F0 (pyin_f0.py) */
+/* libf0's pyin(x, Fs=16000, N=2048, H=160, F_min=50, F_max=1000) with its defaults (518 bins of 10 cents, 1036 HMM
+ * states, 99 thresholds with Beta(1, 18) weights, transitions within 5 bins), in fp64, for a ragged batch: item b is
+ * x[offsets_host[b] .. offsets_host[b+1]) (float32 at 16 kHz, n_b >= 1 sample); B >= 1.  The wrapper and its parameters
+ * are this project's choice (pyin_f0.compute_f0_pyin); no reference command calls pyin.
+ * tab: the device table of SVCB_PYIN_TAB_DOUBLES doubles computed by the host as the reference computes it (pyin_f0.py
+ * tables()): the thresholds, the Beta weights, F_axis, then per HMM column its predecessors with A > 0 (ascending, as
+ * exact doubles, -1 past the end) and their log(A + tiny).
+ * f0, conf: float64, n_b // 160 + 1 per item, following each other from f0[0] / conf[0]; f0 is 0 where unvoiced.
+ * Optional taps (null to skip), per item following each other: cmndf_tap [321][F_b], obs_tap the observations
+ * [1036][F_b], path_tap (int32, one per frame) the Viterbi states.  Each item is bitwise that of a lone call.
+ * ws: svcb_pyin_f0_workspace_bytes(sum of n_b, B) bytes, 256-byte aligned (about 90 bytes per sample). */
+#define SVCB_PYIN_TAB_THR 0
+#define SVCB_PYIN_TAB_BETA 99
+#define SVCB_PYIN_TAB_FAXIS 198
+#define SVCB_PYIN_TAB_BIDX 716
+#define SVCB_PYIN_TAB_BLOG 13148
+#define SVCB_PYIN_TAB_DOUBLES 25580
+size_t svcb_pyin_f0_workspace_bytes(int64_t total_samples, int32_t B);
+int svcb_pyin_f0_ragged(const float* x, const int64_t* offsets_host, int32_t B, const double* tab, double* f0,
+                        double* conf, double* cmndf_tap, double* obs_tap, int32_t* path_tap, void* ws, size_t ws_bytes,
+                        svcb_stream stream);
+/* The Viterbi and trace back alone, on given observations: item b is obs[1036 x frame_offsets_host[b] ..) as
+ * [1036][F_b] (F_b >= 1, frame_offsets_host[0] >= 0); path: int32, F_b per item following each other from path[0].
+ * ws: svcb_pyin_dp_workspace_bytes(sum of F_b) bytes, 256-byte aligned. */
+size_t svcb_pyin_dp_workspace_bytes(int64_t total_frames);
+int svcb_pyin_dp_ragged(const double* obs, const int64_t* frame_offsets_host, int32_t B, const double* tab,
+                        int32_t* path, void* ws, size_t ws_bytes, svcb_stream stream);
+
 /* ------------------------------------------------------------------ feature retrieval (IVF-Flat, L2) */
 /* An IndexIVFFlat of the reference's feature_retrieval/ (svc_train_retrieval.py writes them with faiss).
  * d % 64 == 0 and 64 <= d <= 2048, nlist >= 1, 1 <= nprobe <= 8 (faiss's nprobe; nprobe > nlist probes every list). */

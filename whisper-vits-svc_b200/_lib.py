@@ -109,6 +109,10 @@ SIGNATURES = {
     "svcb_salience_f0_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32] + [c_void_p] * 5 + [c_size_t, c_void_p]),
     "svcb_salience_dp_workspace_bytes": (c_size_t, [c_int64]),
     "svcb_salience_dp_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "svcb_pyin_f0_workspace_bytes": (c_size_t, [c_int64, c_int32]),
+    "svcb_pyin_f0_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32] + [c_void_p] * 7 + [c_size_t, c_void_p]),
+    "svcb_pyin_dp_workspace_bytes": (c_size_t, [c_int64]),
+    "svcb_pyin_dp_ragged": (c_int, [c_void_p, POINTER(c_int64), c_int32] + [c_void_p] * 3 + [c_size_t, c_void_p]),
     "svcb_ivf_create": (c_int, [c_void_p, c_size_t, POINTER(TensorEntry), c_int32, POINTER(IvfConfig), POINTER(c_void_p)]),
     "svcb_ivf_destroy": (None, [c_void_p]),
     "svcb_ivf_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
